@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- headline measurement of the GPTQ-4bit hot path on B200 (contract: see DESIGN.md "Measurement").
+"""bench.py -- headline measurement of the GPTQ-4bit hot path on H100 (contract: see DESIGN.md "Measurement").
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--model 7b] [--ctx 1920]
-                    [--groupsize 128] [--act-order] [--seq 2048]
+                    [--groupsize 128] [--act-order] [--seq 2048] [--dump-outputs DIR]
 
 One "step" = one decode token of a Llama-shaped stack on random GPTQ tensors of the named architecture (no checkpoints
 exist offline): every layer's rms_norm + q/k/v projections + rope + cache write, attention over ctx cached positions,
@@ -18,6 +18,10 @@ o_proj + residual, rms_norm + gate/up + silu*mul + down + residual, then final n
   kernels  : the per-op launches (what the unchanged model.py drives) timed per launch, with their own fractions.
   cpu_baseline : the oracle's CPU port of dequant + GEMV on the box's host cores (bounded sample, own process, explicit
              thread count).
+
+--dump-outputs DIR writes what the timed path returned in its last timed step (the logits, float32) to DIR/logits.npy.  All
+inputs come from fixed seeds, so two builds run with the same arguments can be compared output for output, within a
+tolerance: the persistent kernel adds its split-K partials with fp32 `red.add`, so its logits are not bitwise reproducible.
 
 --impl reference times that CPU restatement (the reference ships no CPU path for q4; BASELINE.md section 3) and loads
 nothing of this repo's native code.
@@ -50,14 +54,17 @@ def parse():
     ap.add_argument("--no-fused-step", action="store_true", help="time the per-op path even where the persistent kernel applies")
     ap.add_argument("--no-per-op", action="store_true", help="skip the per-op comparison rows (large models: saves time)")
     ap.add_argument("--cpu-seconds", type=float, default=8.0, help="CPU sample budget per repetition (reference arm / cpu_baseline)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's outputs to DIR/<name>.npy")
     a = ap.parse_args()
+    if a.steps < 1:
+        ap.error("--steps must be >= 1")
     if a.ctx is None:
         a.ctx = a.seq - 128
     return a
 
 
 class ClockSampler:
-    """SM clock / throttle reasons DURING the timed region, sampled by a separate `nvidia-smi -lms` process (B200_PROFILING.md):
+    """SM clock / throttle reasons DURING the timed region, sampled by a separate `nvidia-smi -lms` process:
     an in-process NVML thread was seen to take ~60 ms per sample when several ranks share a box and stalled the launch loop."""
 
     FIELDS = "clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
@@ -98,15 +105,25 @@ class ClockSampler:
 
 
 def measured_peaks():
-    """(hbm GB/s, bf16 TF/s burst, bf16 TF/s sustained, kind).  The fallback (B200_PROFILING.md) is used LOUDLY."""
+    """(hbm GB/s, bf16 TF/s burst, bf16 TF/s sustained, kind).  The fallback (H100 SXM data sheet, 700 W) is used LOUDLY."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         if "hbm_gbs" in d and "bf16_tflops" in d:
             return d["hbm_gbs"], d["bf16_tflops"], d.get("bf16_tflops_sustained", d["bf16_tflops"]), "measured"
-    print("bench.py: WARNING: MEASURED_PEAKS.json absent or incomplete -- roofline fractions are against the FALLBACK peaks "
-          "(6650 GB/s, 1590 TF/s) of B200_PROFILING.md", file=sys.stderr, flush=True)
-    return 6650.0, 1590.0, 1400.0, "fallback"
+    print("bench.py: WARNING: MEASURED_PEAKS.json absent or incomplete -- roofline fractions are against the H100 SXM data sheet "
+          "(3350 GB/s, 989 TF/s dense fp16/bf16)", file=sys.stderr, flush=True)
+    return 3350.0, 989.0, 989.0, "datasheet"
+
+
+def power_limit(index):
+    """The card's power limit in W (part of every absolute number the line states), or None when nvidia-smi cannot say."""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                             stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, timeout=10).stdout
+        return float(out.strip().splitlines()[0])
+    except Exception:
+        return None
 
 
 def host_threads():
@@ -199,7 +216,7 @@ def run_reference(args):
     cands = sorted({c for c in (ncpu, lim or ncpu, ncpu // 2, ncpu // 4, 64, 32, 16, 8) if c and 1 <= c <= ncpu}, reverse=True)
     _, threads, _ = cpu_sample(shape, args.groupsize, args.act_order, min(args.cpu_seconds, 3.0), cands)      # warm-up + pick the fastest team size
     samples = []
-    for _ in range(max(1, min(args.steps, 3))):
+    for _ in range(args.steps):
         ms_layer, used, n = cpu_sample(shape, args.groupsize, args.act_order, args.cpu_seconds, threads)
         samples.append(ms_layer)
     ms_layer = sorted(samples)[len(samples) // 2]
@@ -266,6 +283,7 @@ def main():
     gs = args.groupsize
     hbm_peak, tf_peak, tf_sustained, peak_kind = measured_peaks()
     ext = cuda_ext.exllama_ext
+    torch.manual_seed(1234)                           # hidden state and KV cache: the same on every run and every rank (the weights have their own seeds)
 
     stack = DecodeStack(shape, groupsize=gs, act_order=args.act_order, device=str(dev), max_seq=args.seq,
                         tp_rank=rank, tp_size=world, tp_group=None)
@@ -305,7 +323,7 @@ def main():
         torch.cuda.current_stream().wait_stream(side); torch.cuda.synchronize()
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g, capture_error_mode="thread_local"):
-            fn()
+            g.out = fn()                           # the graph's output tensor: each replay rewrites it
         return g
 
     def time_events(fn, n):
@@ -341,7 +359,7 @@ def main():
         use_graph = not args.no_graph and (world == 1 or (fused_ar and not args.act_order) or os.environ.get("EXL_BENCH_TP_GRAPH", "0") == "1")
         # (act-order + tensor parallel falls back to NCCL for the MLP; NCCL inside stream capture hung on this stack in round 1)
         graph = capture(per_op_step) if use_graph else None
-        step_device = graph.replay if graph is not None else per_op_step
+        step_device = (lambda: (graph.replay(), graph.out)[1]) if graph is not None else per_op_step
         launches_per_step = launches_per_op
         mode = "per-op kernels, " + ("CUDA graph" if graph is not None else "eager")
 
@@ -357,10 +375,14 @@ def main():
     torch.cuda.cudart().cudaProfilerStart()          # no-op unless run under `ncu --profile-from-start off`
     e0.record()
     for _ in range(args.steps):
-        step_device()
+        last_out = step_device()
     e1.record()
     barrier()
     torch.cuda.cudart().cudaProfilerStop()
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "logits.npy"), last_out.detach().float().cpu().numpy())
     ms = e0.elapsed_time(e1)
     clocks = sampler.result() if rank == 0 else None
     t = torch.tensor([ms], device=dev, dtype=torch.float64)
@@ -564,7 +586,8 @@ def main():
                        "decode_mode": mode, "parallelism": f"tp{world}", "cuda_graph": graph is not None,
                        "allreduce": (("inside decode_step_kernel: peer-memory reductions + cross-GPU barrier" if use_step else
                                       ("fused GEMV epilogue over NVLink peer memory" if fused_ar else "nccl")) if world > 1 else None),
-                       "l2": f"weights ({(wbytes + head_bytes) / 1e9:.2f} GB/token/rank) >> L2 (126 MB): every step streams them from HBM"},
+                       "l2": f"weights ({(wbytes + head_bytes) / 1e9:.2f} GB/token/rank) >> L2 (50 MB): every step streams them from HBM",
+                       "gpu": torch.cuda.get_device_name(dev), "power_limit_w": power_limit(local_rank)},
             "e2e": {"value": round(1000.0 / e2e_ms, 2), "unit": "tok/s", "h2d_bytes_per_step": host_in.numel() * 2,
                     "d2h_bytes_per_step": host_out.numel() * 4, "ms_per_step": round(e2e_ms, 4),
                     "mode": "C ABI call per step (exl_decode_step)" if use_step else "plugin API calls per op, eager"},

@@ -1,4 +1,4 @@
-"""exllama_b200 -- B200 (sm_100a) implementation of the exllama_ext operator surface.
+"""exllama_b200 -- H100 (sm_90a) implementation of the exllama_ext operator surface.
 
 Layout:
   csrc/            hand-written CUDA kernels + the C ABI (include/exl_b200.h) + the pybind shim

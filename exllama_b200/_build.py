@@ -1,9 +1,9 @@
-"""In-tree build of the native pieces (sm_100a only).
+"""In-tree build of the native pieces (sm_90a only).
 
   libexl_b200.so      : nvcc, all kernels + the C ABI, no torch dependency
   exllama_ext*.so     : torch C++ extension (pybind shim, g++ only) linked against libexl_b200.so
 
-Both land next to this file so they travel with the repo snapshot to the GPU box.
+Both land next to this file, so the package imports straight from the source tree.
 """
 from __future__ import annotations
 
@@ -20,7 +20,8 @@ EXT_SO = os.path.join(HERE, "exllama_ext.so")
 CU_SOURCES = ["capi.cu", "q4_gemv.cu", "q4_matrix.cu", "elementwise.cu", "half_matmul.cu", "q4_gemm_tc.cu", "decode_attn.cu", "decode_step.cu"]
 HEADERS = ["exl_common.cuh", "decode_step_sched.h", os.path.join("..", "..", "include", "exl_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-gencode", "arch=compute_100a,code=sm_100a",
+ARCH = "arch=compute_90a,code=sm_90a"          # H100 (Hopper): wgmma, TMA, clusters
+NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-gencode", ARCH,
               "-Xcompiler", "-fPIC"]
 
 
@@ -50,7 +51,7 @@ def build_lib(force: bool = False, verbose: bool = False) -> str:
             out, _ = p.communicate()
             if p.returncode != 0:
                 raise RuntimeError("nvcc failed: " + " ".join(cmd) + "\n" + out.decode())
-        cmd = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB_SO] + objs + ["-lcublas"]
+        cmd = [NVCC, "-shared", "-gencode", ARCH, "-o", LIB_SO] + objs + ["-lcublas"]
         subprocess.check_call(cmd)
     return LIB_SO
 

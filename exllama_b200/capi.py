@@ -2,7 +2,7 @@
 
 This is the thinnest possible host side: torch is used only for device memory and streams
 (tensor.data_ptr(), torch.cuda.current_stream()).  There is no CPU fallback: if the library is
-missing or no sm_100 device is present, calls raise.
+missing or no sm_90 device is present, calls raise.
 """
 from __future__ import annotations
 

@@ -45,8 +45,8 @@ ExlDevice* exl_device_state(int device)
     }
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) { exl_set_err(EXL_ERR_CUDA, "cudaGetDeviceProperties failed"); return nullptr; }
-    if (prop.major != 10) {
-        exl_set_err(EXL_ERR_CUDA, "device %d is sm_%d%d; libexl_b200 is built for sm_100a (B200) only", device, prop.major, prop.minor);
+    if (prop.major != 9) {
+        exl_set_err(EXL_ERR_CUDA, "device %d is sm_%d%d; libexl_b200 is built for sm_90a (H100) only", device, prop.major, prop.minor);
         return nullptr;
     }
     DeviceGuard guard(device);
@@ -203,7 +203,7 @@ int exl_q4_get_x_map_host(const exl_q4_matrix* w, uint32_t* out_host)
 static int q4_matmul_recons_cublas(ExlDevice* ds, const half* x, int M, const exl_q4_matrix* w, half* out, bool no_zero, cudaStream_t stream)
 {
     // reference prefill path: column_remap -> reconstruct -> Hgemm (q4_matmul.cu:301-344); kept as an explicit,
-    // selectable GPU path (force_path = 3) and as the large-M route until the tcgen05 kernel covers a shape.
+    // selectable GPU path (force_path = 3) and as the large-M route until the wgmma kernel covers a shape.
     const int64_t dq_numel = (int64_t)w->K * w->N;
     half* dq = ds->temp_dq_numel >= dq_numel ? ds->temp_dq : nullptr;
     half* xm = nullptr;
@@ -234,7 +234,7 @@ static int q4_matmul_dispatch(ExlDevice* ds, const half* x, int M, const exl_q4_
     if (path == 0 && !gemv_ok) path = 3;
     if (path == 0) {
         // M <= 8: one skinny pass.  8 < M <= 48: still HBM-bound, a few skinny passes (each re-streams the packed weights,
-        // 0.5 B / weight) beat a tensor-core tile that is mostly padding.  Above: tcgen05 fused-dequant GEMM.
+        // 0.5 B / weight) beat a tensor-core tile that is mostly padding.  Above: wgmma fused-dequant GEMM.
         if (M <= EXL_SKINNY_MAX_M) path = 1;
         else if (M <= 48 || !exl_tc_gemm_supported(w, M)) path = (M <= 64) ? 1 : 3;
         else path = 2;

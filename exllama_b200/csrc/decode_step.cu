@@ -1,4 +1,4 @@
-// decode_step.cu -- ONE persistent cooperative kernel for a whole decode token (bsz 1, q_len 1) on sm_100a.
+// decode_step.cu -- ONE persistent cooperative kernel for a whole decode token (bsz 1, q_len 1) on sm_90a.
 //
 // SURVEY.md 8f-4 ("host loop: a C++ decoder_layer op / whole-step capture") and the answer to VERDICT r1 item 1: the five
 // launches per layer (q4_attn, decode_attn, q4_attn_2, q4_mlp x2) were latency-bound -- launch + setup + x-dependent
@@ -19,7 +19,7 @@
 //    phase and layer boundaries -- the thing separate launches could not do.
 //  * Work of a GEMV phase = (128-column tile) x (128-row K stage) units, flattened tile-major and cut into G equal contiguous
 //    ranges (G = grid size): every SM streams the same number of bytes whatever the matrix shapes (65B gate/up: 172 tiles on
-//    148 SMs is no longer a problem).  A warp accumulates its 32 columns over the stages it sees and, at a tile boundary,
+//    132 SMs is no longer a problem).  A warp accumulates its 32 columns over the stages it sees and, at a tile boundary,
 //    adds its fp32 partial into the phase's accumulator in L2 with red.global.add.v4.f32 -- the split-K reduction is the
 //    grid barrier that the data dependence needs anyway.
 //  * Inner product exactly as q4_gemv.cu (integer tensor cores, nibbles as the A operand straight from the ring, x carried
@@ -196,14 +196,12 @@ __device__ __forceinline__ void imma_z(int (&c)[4], uint32_t a0, uint32_t a1, ui
         : "=r"(c[0]), "=r"(c[1]), "=r"(c[2]), "=r"(c[3]) : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1), "r"(0));
 }
 
-// acc += w.lo * x.lo + w.hi * x.hi for two packed fp16 pairs: mixed-precision FMA (fma.rn.f32.f16 -> SASS FHFMA, fp16 x fp16 + fp32, one
-// rounding).  The product of two fp16 values is exact in fp32, so this is bit-identical to converting both to fp32 and fmaf() -- without
-// the four conversions.
+// acc += w.lo * x.lo + w.hi * x.hi for two packed fp16 pairs, in that order.  The product of two fp16 values is exact in fp32, so
+// converting both to fp32 and fmaf() rounds once per term (sm_90 has no mixed fp16 x fp16 + fp32 FMA instruction).
 __device__ __forceinline__ float fhfma2(uint32_t w, uint32_t x, float acc)
 {
-    asm("{\n\t.reg .b16 wl, wh, xl, xh;\n\tmov.b32 {wl, wh}, %1;\n\tmov.b32 {xl, xh}, %2;\n\t"
-        "fma.rn.f32.f16 %0, wl, xl, %0;\n\tfma.rn.f32.f16 %0, wh, xh, %0;\n\t}" : "+f"(acc) : "r"(w), "r"(x));
-    return acc;
+    const float2 wf = __half22float2(*reinterpret_cast<const half2*>(&w)), xf = __half22float2(*reinterpret_cast<const half2*>(&x));
+    return fmaf(wf.y, xf.y, fmaf(wf.x, xf.x, acc));
 }
 
 __device__ __forceinline__ half silu_h(half x)

@@ -1,4 +1,4 @@
-// exl_common.cuh -- shared declarations for libexl_b200.so (sm_100a only).
+// exl_common.cuh -- shared declarations for libexl_b200.so (sm_90a only).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -26,7 +26,7 @@ struct exl_q4_matrix
     uint32_t* x_map;     // [K] or nullptr (act-order: x column feeding sequential row k)
     // TMA descriptor of qweight as a 2-D int32 tensor [K/8, N], box 16 rows x 32 columns, 128-byte swizzle (q4_gemv.cu)
     alignas(64) CUtensorMap tmap_w;
-    // same tensor, box 8 rows x 128 columns, no swizzle: the packed-word tile of one k-block of the tcgen05 GEMM (q4_gemm_tc.cu)
+    // same tensor, box 8 rows x 128 columns, no swizzle: the packed-word tile of one k-block of the wgmma GEMM (q4_gemm_tc.cu)
     alignas(64) CUtensorMap tmap_wp;
     // decode_step.cu: ONE op per 8 KB unit -- qweight viewed as [N/32][K/8][32] (dims fastest first: 32 columns, k8-row, column group),
     // box 32 x 16 x 4 with the 128-byte swizzle: the same shared-memory image as four tmap_w boxes side by side.  valid3 == 0 when
@@ -142,7 +142,7 @@ int exl_gemv_launch(ExlDevice* ds, const half* x, int M, const exl_q4_matrix* co
 int exl_encode_weight_tmap(exl_q4_matrix* w);
 int exl_reconstruct_launch(const exl_q4_matrix* w, half* out, cudaStream_t stream);
 
-// q4_gemm_tc.cu : tcgen05 fused-dequant GEMM (prefill)
+// q4_gemm_tc.cu : wgmma fused-dequant GEMM (prefill)
 int exl_tc_gemm_launch(ExlDevice* ds, const half* x, int M, const exl_q4_matrix* w, half* out, bool no_zero, cudaStream_t stream);
 bool exl_tc_gemm_supported(const exl_q4_matrix* w, int M);
 

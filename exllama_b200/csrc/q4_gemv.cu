@@ -1,4 +1,4 @@
-// q4_gemv.cu -- decode hot path: fused 4-bit unpack + scale/zero + skinny GEMM (M <= 8) for sm_100a.
+// q4_gemv.cu -- decode hot path: fused 4-bit unpack + scale/zero + skinny GEMM (M <= 8) for sm_90a.
 //
 // Replaces the reference's q4_matmul_kernel + dot_product_8* (exllama_ext/cuda_func/q4_matmul.cu:34-212,
 // exllama_ext/matrix.cuh:87-286) and, through the fused prologue/epilogues, rms_norm (rms_norm.cu),

@@ -1,4 +1,4 @@
-"""Drop-in mirror of the reference's cuda_ext.py (/root/reference/cuda_ext.py:43-167).
+"""Drop-in mirror of the reference's cuda_ext.py (cuda_ext.py:43-167).
 
 Same public names -- `exllama_ext` (the extension module, reached by model.py as cuda_ext.exllama_ext.*),
 `none_tensor`, `ext_make_q4`, `ext_q4_matmul`, `ext_half_matmul`, `ext_rope_`, `ext_rms_norm`, `ext_rms_norm_`,
@@ -6,7 +6,7 @@ Same public names -- `exllama_ext` (the extension module, reached by model.py as
 reference's model.py / generator.py / test_benchmark_inference.py run unchanged with this module on
 sys.path in place of the original (see INTEGRATION.md).
 
-Differences from the reference shim: the extension is built ahead of time in-tree for sm_100a
+Differences from the reference shim: the extension is built ahead of time in-tree for sm_90a
 (exllama_b200/_build.py) instead of JIT-compiled with no arch flags (cuda_ext.py:43-64), and it is loaded by
 file path (the reference's `from exllama_ext import ...` no longer resolves under torch >= 2.11, SURVEY.md 8c).
 There is no fallback: a missing extension raises ImportError.

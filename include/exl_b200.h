@@ -1,9 +1,9 @@
 /*
- * exl_b200.h -- C ABI of libexl_b200.so: the B200 (sm_100a) implementation of the
+ * exl_b200.h -- C ABI of libexl_b200.so: the H100 (sm_90a) implementation of the
  * exllama_ext operator surface (GPTQ 4-bit matmul + the fused Llama ops around it).
  *
  * Drop-in boundary.  The reference binds this path as a torch C++ extension
- * (pybind11 module `exllama_ext`, /root/reference/exllama_ext/exllama_ext.cpp:743-762,
+ * (pybind11 module `exllama_ext`, exllama_ext/exllama_ext.cpp:743-762,
  * loaded by cuda_ext.py:43-64).  Every entry point below is what one of those 16
  * pybind functions needs underneath once the torch::Tensor arguments are
  * reduced to raw pointers and sizes; the citation on each declaration is the
@@ -21,7 +21,7 @@
  *    exl_last_error() returns a human-readable message for the calling thread.
  *  - like the reference, the library keeps global per-process state (tuning,
  *    per-device scratch, handle list) and is not re-entrant across host threads.
- *  - there is NO CPU fallback anywhere: if no sm_100 device is present the
+ *  - there is NO CPU fallback anywhere: if no sm_90 device is present the
  *    compute entry points fail with EXL_ERR_CUDA.
  */
 #ifndef EXL_B200_H
@@ -48,7 +48,7 @@ int exl_version(void);
 /* --- tuning / buffers ------------------------------------------------------ */
 
 /* exllama_ext.cpp:89-112 set_tuning_params.  The *_no_half2 and concurrent_streams
-   flags are accepted and stored for API compatibility; the sm_100a kernels have a
+   flags are accepted and stored for API compatibility; the sm_90a kernels have a
    single code path (fp32 accumulation) and fuse what concurrent_streams overlapped. */
 int exl_set_tuning_params(int matmul_recons_thd, int fused_mlp_thd, int sdp_thd, int matmul_fused_remap,
                           int rmsnorm_no_half2, int rope_no_half2, int matmul_no_half2, int silu_no_half2,
@@ -80,7 +80,7 @@ int exl_q4_get_x_map_host(const exl_q4_matrix* w, uint32_t* out_host);
 
 /* exllama_ext.cpp:199-240 q4_matmul: out[M,N] (=|+=) x[M,K] . W.  no_zero != 0 accumulates into out
    (q4_matmul.cu:78-82).  Dispatch: skinny-M fused unpack+GEMV kernel for M <= EXL_SKINNY_MAX_M, tensor-core
-   (tcgen05) fused-dequant GEMM above. force_path: 0 auto, 1 skinny, 2 tensor-core GEMM, 3 reconstruct+cuBLAS. */
+   (wgmma) fused-dequant GEMM above. force_path: 0 auto, 1 skinny, 2 tensor-core GEMM, 3 reconstruct+cuBLAS. */
 int exl_q4_matmul(const void* x, int M, const exl_q4_matrix* w, void* out, int no_zero, int force_path, void* stream);
 
 /* q4_matrix.cu:212-223 Q4Matrix::reconstruct: out half [K, N] = dequantised W (bit-exact with the reference). */

@@ -1,5 +1,5 @@
 """Generates tests/golden/decode_attn_torch.npz: the regular-attention branch of the reference
-(/root/reference/model.py:383-409: repeat_kv, matmul, /= sqrt(head_dim), softmax, matmul, transpose) executed with
+(the reference's model.py:383-409: repeat_kv, matmul, /= sqrt(head_dim), softmax, matmul, transpose) executed with
 torch on the CPU, once in float32 (softmax dtype float32) and once with the reference's fp16 rounding points, on small
 seeded inputs.  The statements below are the reference's tensor program restated on views of the same shapes; the
 fixture pins oracle.decode_attn_f64 (both modes).  Run in the build container:  python oracle/gen_golden_attn.py"""

@@ -8,17 +8,18 @@
  * The reference (turboderp/exllama @ 3b013cd) ships NO CPU implementation of
  * the q4 path (exllama_ext/cpu_func holds only rep_penalty.cpp); every
  * function below restates a CUDA kernel's arithmetic on the host and cites
- * the reference file:line it follows (paths relative to /root/reference/).
+ * the reference file:line it follows (paths relative to the reference checkout).
  *
- * Parity pinning (every file named here exists; the GPU pins run under `pytest -m gpu` on the B200 box):
+ * Parity pinning (every file named here exists; the GPU pins run under `pytest -m gpu` on an H100):
  *   - orc_rep_penalty / orc_apply_rep_penalty: bit-exact against the reference's own
  *     rep_penalty.cpp compiled into oracle/_ref/librep_penalty_ref.so and against
  *     tests/golden/rep_penalty_ref.npz (oracle/gen_golden_cpu.py)  -- tests/test_oracle.py.
  *   - make_x_map / make_sequential / q4_matmul (decode + reconstruct flavours): against the
- *     reference's kernels compiled for sm_100a into oracle/_ref/libexllama_ref.so
+ *     reference's kernels compiled for sm_90a into oracle/_ref/libexllama_ref.so, whose outputs
+ *     are stored in tests/golden/ref_gpu.npz (oracle/gen_golden_ref_gpu.py)
  *     -- tests/test_gpu_q4_matmul.py::test_against_reference_*.
  *   - rms_norm, rope, column_remap, half_matmul, update_cache and silu_mul (through the fused
- *     q4_attn / q4_attn_2 / q4_mlp blocks): three-way against the same library
+ *     q4_attn / q4_attn_2 / q4_mlp blocks): three-way against the same stored outputs
  *     -- tests/test_gpu_ref_pin.py.
  *   - orc_decode_attn: tests/golden/decode_attn_torch.npz (oracle/gen_golden_attn.py: the
  *     reference's attention tensor program model.py:383-409 run with torch on the CPU).

@@ -27,12 +27,13 @@ _f = C.c_float
 
 
 def build(force: bool = False) -> None:
-    """Compile liboracle.so (and oracle/_ref/* when /root/reference exists)."""
+    """Compile liboracle.so, and oracle/_ref/* when EXLLAMA_REFERENCE names a checkout of the reference."""
     so = os.path.join(_HERE, "liboracle.so")
     if force or not os.path.exists(so) or os.path.getmtime(so) < os.path.getmtime(os.path.join(_HERE, "gptq_oracle.c")):
         subprocess.check_call(["make", "-C", _HERE, os.path.join(_HERE, "liboracle.so")], stdout=subprocess.DEVNULL)
-    if os.path.isdir("/root/reference/exllama_ext"):
-        subprocess.check_call(["make", "-C", _HERE, "ref"], stdout=subprocess.DEVNULL)
+    ref = os.environ.get("EXLLAMA_REFERENCE")
+    if ref and os.path.isdir(os.path.join(ref, "exllama_ext")):
+        subprocess.check_call(["make", "-C", _HERE, "ref", "REF=" + ref], stdout=subprocess.DEVNULL)
 
 
 def lib() -> C.CDLL:

@@ -1,5 +1,5 @@
 // extern "C" shim over the reference's OWN cpu_func/rep_penalty.cpp (compiled
-// from /root/reference in place; see oracle/Makefile).  TEST INFRASTRUCTURE ONLY.
+// from the reference checkout in place; see oracle/Makefile).  TEST INFRASTRUCTURE ONLY.
 #include "cpu_func/rep_penalty.h"
 extern "C" {
 void ref_rep_penalty(int vocab_size, const uint64_t* seq, float* rep_mask, float penalty_max,

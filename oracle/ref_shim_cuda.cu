@@ -1,7 +1,7 @@
 // extern "C" shim over the reference's OWN CUDA kernels (exllama_ext/cuda_func/*.cu,
-// cuda_buffers.cu), compiled unmodified from /root/reference for sm_100a into
+// cuda_buffers.cu), compiled unmodified from the reference checkout for sm_90a into
 // oracle/_ref/libexllama_ref.so (see oracle/Makefile).  This is the live GPU
-// oracle on the B200 box.  TEST INFRASTRUCTURE ONLY -- never loaded by the product.
+// oracle (oracle/gen_golden_ref_gpu.py).  TEST INFRASTRUCTURE ONLY -- never loaded by the product.
 //
 // The entry points mirror include/exl_b200.h so tests can drive both libraries
 // with the same arguments.  All reference kernels run on the legacy default stream.

@@ -1,5 +1,5 @@
 // Stub standing in for <ATen/cuda/CUDAContext.h> when the reference's .cu files
-// are compiled (unmodified, where they lie under /root/reference) into
+// are compiled (unmodified, where they lie in the reference checkout) into
 // oracle/_ref/libexllama_ref.so WITHOUT torch.  The reference .cu files only
 // need cuBLAS types and the TORCH_CHECK macro from that header.
 // TEST INFRASTRUCTURE ONLY (see oracle/Makefile).

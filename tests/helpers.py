@@ -34,6 +34,16 @@ def ulp_diff_f16(a, b):
     return np.abs(key(a) - key(b))
 
 
+GOLDEN = os.path.join(ROOT, "tests", "golden")
+
+
+def golden_cols(n, seed, k=512):
+    """The fixed sample of output columns stored for a golden array whose last axis has n entries (all of them when n <= k)."""
+    if n <= k:
+        return np.arange(n)
+    return np.sort(np.random.default_rng(seed).choice(n, k, replace=False))
+
+
 def to_cuda(*arrays):
     import torch
     out = []
@@ -43,7 +53,8 @@ def to_cuda(*arrays):
 
 
 class RefLib:
-    """oracle/_ref/libexllama_ref.so: the reference's own kernels compiled for sm_100a (GPU box only)."""
+    """oracle/_ref/libexllama_ref.so: the reference's own kernels compiled for sm_90a (oracle/gen_golden_ref_gpu.py and tools only;
+    the tests read what it computed from tests/golden/ref_gpu.npz)."""
 
     def __init__(self):
         from oracle import oracle as O

@@ -16,8 +16,8 @@ from exllama_b200.shapes import SHAPES
 from exllama_b200.tp import plan_shards
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SMEM_OPTIN = 232448          # cudaDevAttrMaxSharedMemoryPerBlockOptin on sm_100 (227 KB)
-SMS = 148
+SMEM_OPTIN = 232448          # cudaDevAttrMaxSharedMemoryPerBlockOptin on sm_90 (227 KB)
+SMS = 132                    # H100 SXM
 
 
 @pytest.fixture(scope="module")
@@ -124,6 +124,6 @@ def test_attention_table_reset_is_confined_to_short_contexts(lib):
     rc, msg = check(lib, s.hidden, s.hidden, s.inter, s.heads, s.vocab, SMS, 0, 2047, False, c)
     assert rc == 0, msg
     assert c["gaps"] > 0                      # the hazard is real (found by this test before the reset existed) ...
-    assert c["resets"] == 48                  # ... and confined: 32 heads x nph units < 148 CTAs, nph >= 2 -> contexts 17 .. 64
+    assert c["resets"] == 48                  # ... and confined: 32 heads x nph units < 132 CTAs, nph >= 2 -> contexts 17 .. 64
     rc, msg = check(lib, s.hidden, s.hidden, s.inter, s.heads, s.vocab, SMS, 65, 2047, False, c)
     assert rc == 0 and c["gaps"] == 0 and c["resets"] == 0

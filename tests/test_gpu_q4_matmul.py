@@ -1,10 +1,12 @@
 """GPU parity of q4_matmul through the C ABI (ctypes -> libexl_b200.so), against the float64 oracle on the same
-seeded inputs, and -- when oracle/_ref/libexllama_ref.so travelled with the snapshot -- against the reference's
-own kernels compiled for sm_100a.  Tolerance: see helpers.REL_TOL / RMS_TOL (fp16 output rounding)."""
+seeded inputs, and against what the reference's own kernels computed on an H100 from the same inputs
+(tests/golden/ref_gpu.npz, oracle/gen_golden_ref_gpu.py).  Tolerance: see helpers.REL_TOL / RMS_TOL (fp16 output rounding)."""
+import os
+
 import numpy as np
 import pytest
 
-from helpers import RefLib, assert_close_ref64, to_cuda
+from helpers import GOLDEN, assert_close_ref64, golden_cols, to_cuda
 
 pytestmark = pytest.mark.gpu
 
@@ -149,12 +151,14 @@ def test_skinny_unsupported_groupsize_takes_general_route(oracle, M, K, N, gs, a
 
 
 TC_CASES = [(128, 1024, 512, 128, False), (200, 2048, 384, 32, True), (1, 512, 128, 64, False), (77, 4096, 1152, 128, True),
-            (384, 1024, 1024, 1024, False), (130, 2816, 96, 128, False)]
+            (384, 1024, 1024, 1024, False), (130, 2816, 96, 128, False),
+            # M > 128 and ceil(M / 256) * ceil(N / 128) >= SMs / 2: the 256-row (MT = 2) tiles, with a partial last M tile
+            (300, 1024, 8448, 128, False), (260, 512, 8448, 32, True)]
 
 
 @pytest.mark.parametrize("M,K,N,gs,act", TC_CASES)
 def test_tcgen05_gemm_vs_ref64(oracle, M, K, N, gs, act):
-    """force_path=2: the tcgen05 fused-dequant GEMM.  Its B operand is bit-identical to the reference's reconstructed
+    """force_path=2: the wgmma fused-dequant GEMM.  Its B operand is bit-identical to the reference's reconstructed
     weights (fp16-rounded scale * (q - zp)), accumulated in fp32 -> compare against the `recons` flavour of ref64."""
     import torch
     from exllama_b200 import capi
@@ -164,6 +168,8 @@ def test_tcgen05_gemm_vs_ref64(oracle, M, K, N, gs, act):
     out = capi.q4_matmul(to_cuda(x), q4, force_path=2)
     torch.cuda.synchronize()
     assert capi.last_q4_path() == "tc_gemm"
+    if N >= 8192:
+        assert M > 128 and (M + 255) // 256 * ((N + 127) // 128) >= torch.cuda.get_device_properties(0).multi_processor_count // 2
     ref = oracle.ref64_with_act_order(x, qw, qz, sc, g_idx, recons=True)
     assert_close_ref64(out.cpu().numpy(), ref, what=f"tc_gemm M{M} K{K} N{N} g{gs} act{act}")
     res = oracle.synth_x(M, N, seed=99)
@@ -183,37 +189,31 @@ def test_reconstruct_bit_exact(oracle):
 
 
 # ---------------------------------------------------------------------------------------------------
-# against the reference's own kernels (oracle/_ref/libexllama_ref.so)
+# against the reference's own kernels (their outputs, stored as a fixed column sample)
 # ---------------------------------------------------------------------------------------------------
 
 @pytest.fixture(scope="module")
-def reflib():
-    try:
-        r = RefLib()
-    except FileNotFoundError:
-        pytest.skip("oracle/_ref/libexllama_ref.so not present")
-    r.prepare_buffers(inter=11008, max_rows=256, dq_numel=4096 * 11008)
-    return r
+def golden():
+    return np.load(os.path.join(GOLDEN, "ref_gpu.npz"))
 
 
 @pytest.mark.parametrize("M,K,N,gs,act", [(1, 4096, 4096, 128, False), (1, 4096, 11008, 128, False),
                                           (4, 5120, 5120, 128, True), (7, 2048, 6656, 32, True)])
-def test_against_reference_decode_kernel(oracle, reflib, M, K, N, gs, act):
+def test_against_reference_decode_kernel(oracle, golden, M, K, N, gs, act):
     """|new - ref_ext| within 2e-2 (the reference accumulates in fp16 with atomics) AND our error against the
     float64 restatement is no larger than the reference's own (SURVEY.md 8c)."""
-    import torch
     from exllama_b200 import capi
     qw, qz, sc, g_idx = _mk(oracle, K, N, gs, act, seed=41)
     x = oracle.synth_x(M, K, seed=7)
-    mine = capi.q4_matmul(to_cuda(x), _q4(capi, qw, qz, sc, g_idx)).cpu().numpy().astype(np.float64)
-    tq, tz, ts = to_cuda(qw.copy(), qz, sc)
-    h = reflib.make_q4(tq, tz, ts, g_idx)
-    theirs = reflib.q4_matmul(to_cuda(x), h, N, mode=0).cpu().numpy().astype(np.float64)
+    c = golden_cols(N, N)
+    mine = capi.q4_matmul(to_cuda(x), _q4(capi, qw, qz, sc, g_idx)).cpu().numpy().astype(np.float64)[:, c]
+    key = f"decode_{M}_{K}_{N}_{gs}_{int(act)}"
+    theirs = golden[key].astype(np.float64)
     if act:
         # both implementations must have produced the same sequential qweight and x_map
-        np.testing.assert_array_equal(tq.cpu().numpy(), oracle.make_sequential(qw, oracle.make_x_map(g_idx, K // gs)))
-    # column sample for ref64 (full oracle is O(MKN) on the CPU)
-    ref_full = oracle.ref64_with_act_order(x, qw, qz, sc, g_idx) if K * N <= 4096 * 4096 * 2 else None
+        np.testing.assert_array_equal(golden[key + "_qweight"], oracle.make_sequential(qw, oracle.make_x_map(g_idx, K // gs))[:, c[:32]])
+    # ref64 (full oracle is O(MKN) on the CPU) where cheap enough
+    ref_full = oracle.ref64_with_act_order(x, qw, qz, sc, g_idx)[:, c] if K * N <= 4096 * 4096 * 2 else None
     rms = np.sqrt(np.mean(theirs ** 2))
     assert np.all(np.abs(mine - theirs) <= 2e-2 * np.abs(theirs) + 2e-2 * rms)
     if ref_full is not None:
@@ -221,14 +221,12 @@ def test_against_reference_decode_kernel(oracle, reflib, M, K, N, gs, act):
         assert e_mine <= e_ref * 1.05 + 1e-6, (e_mine, e_ref)
 
 
-def test_against_reference_recons_path(oracle, reflib):
+def test_against_reference_recons_path(oracle, golden):
     from exllama_b200 import capi
     M, K, N, gs = 64, 4096, 4096, 128
     qw, qz, sc, _ = _mk(oracle, K, N, gs, False, seed=43)
     x = oracle.synth_x(M, K, seed=8)
-    mine = capi.q4_matmul(to_cuda(x), _q4(capi, qw, qz, sc, None)).cpu().numpy().astype(np.float64)
-    tq, tz, ts = to_cuda(qw.copy(), qz, sc)
-    h = reflib.make_q4(tq, tz, ts, None)
-    theirs = reflib.q4_matmul(to_cuda(x), h, N, mode=1).cpu().numpy().astype(np.float64)
+    mine = capi.q4_matmul(to_cuda(x), _q4(capi, qw, qz, sc, None)).cpu().numpy().astype(np.float64)[:, golden_cols(N, N)]
+    theirs = golden["recons_64_4096_4096"].astype(np.float64)
     rms = np.sqrt(np.mean(theirs ** 2))
     assert np.all(np.abs(mine - theirs) <= 2e-2 * np.abs(theirs) + 2e-2 * rms)

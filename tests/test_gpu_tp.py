@@ -1,4 +1,4 @@
-"""Tensor-parallel GPU parity (needs >= 2 GPUs on the box: run with `gpurun --gpus 2`; skipped otherwise).
+"""Tensor-parallel GPU parity (needs >= 2 GPUs on one machine; skipped otherwise).
 tools/tp_check.py under torchrun: identical full GPTQ tensors on every rank -> column / row shards ->
 (a) q4_attn_2_tp / q4_mlp_tp + NCCL all-reduce and (b) the fused GEMV + NVLink one-shot all-reduce kernels, both against
 the single-rank float64 oracle; (b) additionally bitwise identical on every rank, over 60 back-to-back launches and 30

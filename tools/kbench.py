@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Kernel-level sweep of q4_matmul (decode shapes): achieved HBM GB/s of our kernel and, when
-oracle/_ref/libexllama_ref.so is present, of the reference's kernel compiled for sm_100a, on a rotating pool of
-distinct weight sets (>= 1 GB, defeats the 126 MB L2).  CUDA-event timing, never under a profiler.
+oracle/_ref/libexllama_ref.so is present, of the reference's kernel compiled for sm_90a, on a rotating pool of
+distinct weight sets (>= 1 GB, defeats the 50 MB L2).  CUDA-event timing, never under a profiler.
     python tools/kbench.py [--m 1] [--shapes 7b] [--ref] [--json out.json]"""
 import argparse
 import json

@@ -1,4 +1,4 @@
-// micro-benchmark: legacy mma.sync throughput/latency on sm_100a: HMMA m16n8k16 f16->f32 vs IMMA m16n8k32 u8.s8->s32
+// micro-benchmark: legacy mma.sync throughput/latency on sm_90a: HMMA m16n8k16 f16->f32 vs IMMA m16n8k32 u8.s8->s32
 #include <cstdio>
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -31,11 +31,11 @@ __global__ void k(int iters, int* out, long long* cyc)
 template <int MODE, int ILP>
 void run(const char* name, int warps)
 {
-    int* out; long long* cyc; cudaMalloc(&out, 148 * 1024 * 4); cudaMalloc(&cyc, 8);
+    int* out; long long* cyc; cudaMalloc(&out, 132 * 1024 * 4); cudaMalloc(&cyc, 8);
     int iters = 4096;
-    k<MODE, ILP><<<148, warps * 32>>>(iters, out, cyc);
+    k<MODE, ILP><<<132, warps * 32>>>(iters, out, cyc);
     cudaDeviceSynchronize();
-    k<MODE, ILP><<<148, warps * 32>>>(iters, out, cyc);
+    k<MODE, ILP><<<132, warps * 32>>>(iters, out, cyc);
     cudaDeviceSynchronize();
     long long h; cudaMemcpy(&h, cyc, 8, cudaMemcpyDeviceToHost);
     double per = (double)h / (iters * ILP);

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Prefill q4_matmul sweep: tcgen05 fused-dequant GEMM (path 2) vs reconstruct + cuBLAS (path 3, the reference's algorithm)
-and, with --ref, the reference's own q4_matmul_recons_cuda compiled for sm_100a.  CUDA-event timing over a rotating pool."""
+"""Prefill q4_matmul sweep: wgmma fused-dequant GEMM (path 2) vs reconstruct + cuBLAS (path 3, the reference's algorithm)
+and, with --ref, the reference's own q4_matmul_recons_cuda compiled for sm_90a.  CUDA-event timing over a rotating pool."""
 import argparse, json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,15 +1,15 @@
 #!/usr/bin/env python
 """Drop-in demonstration (VERDICT r1 item 4 / row N1): run the reference's UNCHANGED test_benchmark_inference.py
-(/root/reference/test_benchmark_inference.py:161-222: `-p` perf and `-ppl` perplexity) on a synthetic model directory,
+(test_benchmark_inference.py:161-222: `-p` perf and `-ppl` perplexity) on a synthetic model directory,
 once over the reference's own extension and once over this repo's, and compare what it prints.
 
-    python tools/run_dropin.py --model-dir /tmp/synth7b [--exts ref,ours] [--out gpurun_out/dropin.json] [-- extra args]
+    python tools/run_dropin.py --model-dir /tmp/synth7b [--exts ref,ours] [--out dropin.json] [-- extra args]
 
-The reference's files are the verbatim copies staged by tools/stage_reference.py under baseline/_ref/exllama/ (the GPU box
-has no /root/reference).  Nothing in them is edited; the harness only prepares the interpreter before running the script:
+The reference's files are the verbatim copies staged by tools/stage_reference.py under baseline/_ref/exllama/ (a GPU machine
+need not have the reference checkout).  Nothing in them is edited; the harness only prepares the interpreter before running the script:
   ours : sys.modules["cuda_ext"] = exllama_b200.cuda_ext            (INTEGRATION.md 1a)
   ref  : the pre-built reference extension is registered as `exllama_ext` and torch.utils.cpp_extension.load is made to
-         return it, so the reference's cuda_ext.py imports unchanged without a 40 s JIT compile on the box (and without
+         return it, so the reference's cuda_ext.py imports unchanged without a 40 s JIT compile (and without
          tripping over torch >= 2.11 no longer leaving JIT modules importable by name, SURVEY.md 8c caveat 1).
 """
 import argparse
@@ -18,6 +18,7 @@ import os
 import re
 import subprocess
 import sys
+import tempfile
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -69,7 +70,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--model-dir", required=True)
     ap.add_argument("--exts", default="ref,ours")
-    ap.add_argument("--out", default=os.path.join(ROOT, "gpurun_out", "dropin.json"))
+    ap.add_argument("--out", default=os.path.join(tempfile.gettempdir(), "dropin.json"))
     ap.add_argument("--length", type=int, default=2048)
     ap.add_argument("--ppl-chunks", type=int, default=None, help="default: the script's own default (100)")
     ap.add_argument("--no-ppl", action="store_true")

@@ -1,13 +1,13 @@
 #!/usr/bin/env python
 """Stage the UNMODIFIED reference for the drop-in run (VERDICT r1 item 4, SURVEY.md 8d "model level").
 
-The GPU box has no /root/reference, so the reference's Python files, its extension sources and its sample dataset
-are copied verbatim into the git-ignored `baseline/_ref/exllama/` (it travels with gpurun, it never enters the
+A GPU machine need not have the reference checkout, so the reference's Python files, its extension sources and its sample dataset
+are copied verbatim into the git-ignored `baseline/_ref/exllama/` (it travels with the working tree, it never enters the
 history), and its extension is built ahead of time, from those copies, into
-`baseline/_ref/exllama_ext_ref.so` with exactly the flags cuda_ext.py:43-64 passes plus the sm_100a gencode
+`baseline/_ref/exllama_ext_ref.so` with exactly the flags cuda_ext.py:43-64 passes plus the sm_90a gencode
 (the reference passes no arch flags; on the GPU box torch would add the detected arch itself).
 
-Run here (needs /root/reference):  python tools/stage_reference.py
+Run with the reference checkout:  EXLLAMA_REFERENCE=<path> python tools/stage_reference.py
 """
 import os
 import shutil
@@ -15,7 +15,7 @@ import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.environ.get("EXL_REFERENCE", "/root/reference")
+REF = os.environ.get("EXLLAMA_REFERENCE", "")
 DST = os.path.join(ROOT, "baseline", "_ref", "exllama")
 EXT_SO = os.path.join(ROOT, "baseline", "_ref", "exllama_ext_ref.so")
 
@@ -25,7 +25,7 @@ PY_FILES = ["model.py", "tokenizer.py", "generator.py", "alt_generator.py", "lor
 
 def stage(force=False):
     if not os.path.isdir(REF):
-        print(f"stage_reference: {REF} absent (GPU box?) -- using what is already staged", file=sys.stderr)
+        print(f"stage_reference: EXLLAMA_REFERENCE={REF!r} is not a reference checkout -- using what is already staged", file=sys.stderr)
         return os.path.exists(EXT_SO)
     os.makedirs(DST, exist_ok=True)
     for f in PY_FILES:
@@ -56,7 +56,7 @@ def stage(force=False):
         obj = os.path.join(build_dir, os.path.basename(s) + ".o")
         objs.append(obj)
         if s.endswith(".cu"):
-            cmd = ["nvcc", "-O3", "-lineinfo", "-gencode", "arch=compute_100a,code=sm_100a", "--expt-relaxed-constexpr",
+            cmd = ["nvcc", "-O3", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a", "--expt-relaxed-constexpr",
                    "-D__CUDA_NO_HALF_OPERATORS__", "-D__CUDA_NO_HALF_CONVERSIONS__", "-D__CUDA_NO_BFLOAT16_CONVERSIONS__",
                    "-D__CUDA_NO_HALF2_OPERATORS__", "-Xcompiler", "-fPIC"] + common + sum((["-isystem", i] for i in inc), []) + ["-c", src, "-o", obj]
         else:

@@ -1,6 +1,6 @@
-"""Turn the ncu outputs of tools/collect_r1.sh into the small, tracked summaries under profiles/.
-  python tools/summarise_ncu.py launches gpurun_out/launches_bench_r1.csv profiles/launches_bench_r1_summary.csv
-  python tools/summarise_ncu.py full gpurun_out/decode_layer_r1.ncu-rep profiles/decode_layer_ncu_r1.json"""
+"""Turn Nsight Compute outputs (a --csv launch list, or a --set full report) into small summaries.
+  python tools/summarise_ncu.py launches launches.csv launches_summary.csv
+  python tools/summarise_ncu.py full decode_layer.ncu-rep decode_layer_ncu.json"""
 import csv
 import io
 import json

@@ -5,6 +5,7 @@ established; kineto + graph-launched cluster/PDL kernels is an unusual mix) -- a
 import json
 import os
 import sys
+import tempfile
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
@@ -39,7 +40,8 @@ torch.cuda.synchronize()
 with profile(activities=[ProfilerActivity.CUDA, ProfilerActivity.CPU]) as prof:
     g.replay()
     torch.cuda.synchronize()
-path = "gpurun_out/timeline_trace.json"
+path = os.path.join(tempfile.mkdtemp(), "timeline_trace.json")
+print("trace", path)
 prof.export_chrome_trace(path)
 ev = [e for e in json.load(open(path))["traceEvents"] if e.get("cat") == "kernel"]
 ev.sort(key=lambda e: e["ts"])

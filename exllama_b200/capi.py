@@ -221,17 +221,18 @@ class _DecodeDesc(C.Structure):
     _fields_ = [("n_layers", i32), ("num_heads", i32), ("head_dim", i32), ("max_seq_len", i32), ("vocab", i32), ("rms_eps", f32),
                 ("mats", C.POINTER(vp)), ("ln1", C.POINTER(vp)), ("ln2", C.POINTER(vp)), ("key_cache", C.POINTER(vp)),
                 ("value_cache", C.POINTER(vp)), ("sin", vp), ("cos", vp), ("final_norm", vp), ("lm_head", vp),
-                ("tp_rank", i32), ("tp_world", i32)]
+                ("tp_rank", i32), ("tp_world", i32), ("num_kv_heads", i32)]
 
 
 class DecodePlan:
     """exl_decode_plan: the whole decode token as one persistent kernel (csrc/decode_step.cu).
 
     handles: per layer the 7 Q4 handles (q, k, v, o, gate, up, down) as integers / c_void_p; every tensor passed here is
-    borrowed and must outlive the plan."""
+    borrowed and must outlive the plan.  num_kv_heads (grouped-query attention, default num_heads): k_proj / v_proj are
+    num_kv_heads * head_dim wide; single GPU only."""
 
     def __init__(self, handles, ln1, ln2, key_cache, value_cache, sin, cos, num_heads, head_dim, max_seq_len, eps,
-                 final_norm=None, lm_head=None, tp_rank=0, tp_world=1):
+                 final_norm=None, lm_head=None, tp_rank=0, tp_world=1, num_kv_heads=None):
         n = len(handles)
         self._keep = (ln1, ln2, key_cache, value_cache, sin, cos, final_norm, lm_head)
         flat = []
@@ -251,6 +252,7 @@ class DecodePlan:
         d.final_norm = final_norm.data_ptr() if final_norm is not None else None
         d.lm_head = lm_head.data_ptr() if lm_head is not None else None
         d.tp_rank, d.tp_world = tp_rank, tp_world
+        d.num_kv_heads = num_kv_heads if num_kv_heads is not None else num_heads      # k / v caches: [num_kv_heads, max_seq, head_dim]
         self.vocab = d.vocab
         self.tp_world = tp_world
         self.handle = vp()

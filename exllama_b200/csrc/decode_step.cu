@@ -28,12 +28,14 @@
 //  * The x-dependent part of a phase (residual add + RMS norm, rope + cache write, softmax-combine, silu*mul; then per-segment
 //    quantisation of the K range this CTA needs) runs after the barrier out of L2-resident fp32 accumulators; the residual
 //    stream itself lives in every CTA's shared memory in fp16, rounded where the reference rounds it.
-//  * ATT: (head, 16-position chunk) units, online softmax per warp in fp32 (as decode_attn.cu), partial (m, l, o) per CTA to
-//    L2, combined in the O prologue.  The newest K/V row never round-trips through HBM before it is used.
+//  * ATT: (KV head, 16-position chunk) units, online softmax per warp in fp32 (as decode_attn.cu), partial (m, l, o) per CTA and
+//    query head to L2, combined in the O prologue.  The newest K/V row never round-trips through HBM before it is used.  Under
+//    grouped-query attention one 8 KB stage of K/V serves all n_rep query heads of its group: the K/V bytes are read once per KV head.
 //  * HEAD: lm_head [vocab, hidden] fp16 streamed as 8 KB stages, fp32 dot products, fp32 logits by red.global.add.
 //
-// Restrictions (checked on the host; anything else uses the per-op kernels): head_dim 128, kv_heads == heads, groupsize 32 * 2^n
-// (or one group), widths multiples of 128, act-order only without tensor parallelism (template flag ACT: x is gathered through
+// Restrictions (checked on the host; anything else uses the per-op kernels): head_dim 128, heads % kv_heads == 0 (grouped-query
+// attention only without tensor parallelism), groupsize 32 * 2^n (or one group), widths multiples of 128, act-order only without
+// tensor parallelism (template flag ACT: x is gathered through
 // each matrix's x_map while it is staged).  Tensor parallel (template flag TP): the row-parallel partials are exchanged by
 // {value, epoch} stores into the peers' memory, see StepArgs.  Every wait is bounded by wall time and traps on expiry.
 #include "exl_common.cuh"
@@ -66,14 +68,15 @@ struct alignas(64) LayerDesc
     CUtensorMap tz[7];                 // ::tmap_qz
     const uint32_t* xmap[7];           // act-order: x column feeding sequential row k of each matrix (exl_q4_matrix::x_map), else NULL
     const half* ln1; const half* ln2;
-    half* kc; half* vc;                // [heads, max_seq, 128]
+    half* kc; half* vc;                // [kv_heads, max_seq, 128]
 };
 
 struct StepArgs
 {
     const LayerDesc* layers; int n_layers;
-    int H, HQ, I;                      // hidden, attention width (heads * 128), intermediate width
-    int heads, max_seq, past_len;
+    int H, HQ, HKV, I;                 // hidden, attention width (heads * 128), k / v width (kv_heads * 128), intermediate width
+    int heads, kv_heads, n_rep;        // query heads, KV heads, query heads per KV head (1: multi-head attention)
+    int max_seq, past_len;
     int gshift;                        // log2(groupsize / 32); 30 = one group per matrix
     int depth;                         // ring stages per pipeline (4 pipelines)
     int spt_max;                       // max K / 128 over the phases
@@ -86,7 +89,7 @@ struct StepArgs
     const half* sin; const half* cos;  // [max_seq, 128]
     const half* final_norm; const half* lm_head; float* logits; int vocab;     // optional head
     float* acc_qkv; float* acc_o; float* acc_gu; float* acc_d;                 // fp32 phase accumulators in L2
-    float* att_part; int att_slots;    // [heads][att_slots][PART_LD]
+    float* att_part; int att_slots;    // [heads][att_slots][PART_LD] (query heads)
     unsigned long long* bar;           // grid barrier: monotonic arrival counter (this GPU's CTAs only)
     // tensor parallel (world > 1): after a row-parallel projection (o_proj, down_proj) every rank's partial [H] vector -- already
     // reduced over its own CTAs in L2 -- is stored straight into slot [rank] of EVERY peer over NVLink as 8-byte {value, epoch}
@@ -275,9 +278,10 @@ __device__ __forceinline__ void grid_barrier(unsigned long long* ctr, unsigned l
     consumer_sync();
 }
 
-// ACT: act-order matrices present; TP: tensor parallel.  Compile-time so that the common kernel (neither) carries none of their
-// address arithmetic, branches or code (the runtime-flag version of the same source was 10 % slower on the plain 7B step).
-template <bool ACT, bool TP>
+// ACT: act-order matrices present; TP: tensor parallel; GQA: grouped-query attention (kv_heads < heads, single GPU).  Compile-time so
+// that the common kernel (none of them) carries none of their address arithmetic, branches or code (the runtime-flag version of the
+// same source was 10 % slower on the plain 7B step; a runtime n_rep branch around the attention phase made ptxas spill in it).
+template <bool ACT, bool TP, bool GQA>
 __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid_constant__ StepArgs a)
 {
     extern __shared__ __align__(128) unsigned char smem[];
@@ -289,7 +293,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
     const uint32_t xs_slot = (uint32_t)a.spt_max * 256u, seg_slot = (uint32_t)a.spt_max * 32u;
     unsigned char* xs = ring + (size_t)nst * STAGE_STRIDE;                            // xstages x 16 k8-rows x 16 B: quantised x planes by K stage
     unsigned char* segt = xs + (size_t)xstages * 256;                                  // xstages x 4 x {sum x_q, x scale}
-    half* xres = reinterpret_cast<half*>(segt + (size_t)xstages * 32);                // [H] residual stream (fp16, as the reference keeps it)
+    half* xres = reinterpret_cast<half*>(xs + stage_area_bytes(xstages, a.n_rep));    // [H] residual stream (fp16, as the reference keeps it)
     float* parts = reinterpret_cast<float*>(xres + a.H);                               // [2 segments][17][PART_LD] attention partials of the warps (+ the new token)
     float* q_s = parts + 2 * 17 * PART_LD;                                             // [2][128] scaled q of the segment's head
     float* kn_s = q_s + 2 * TILE;                                                      // [2][128] newest k row (after rope)
@@ -297,6 +301,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
     half* qh_s = reinterpret_cast<half*>(vn_s + 2 * TILE);                             // [2][128] q of the segment's head after rope, fp16 as the reference holds it (unscaled)
     unsigned char* wnorm = reinterpret_cast<unsigned char*>(qh_s + 2 * TILE);          // [H / 8][16 B]: norm weights of the rows this CTA quantises next (by k8-row slot)
     half* xh = reinterpret_cast<half*>(xs);                                            // HEAD: normalised x [H] (xs is free by then)
+    float* gparts = reinterpret_cast<float*>(xs);                 // ATT with GQA: [2 segments][n_rep][5][PART_LD] (xs is free then)
     __shared__ __align__(8) unsigned long long full_bar[4 * MAX_DEPTH], empty_bar[4 * MAX_DEPTH];
     __shared__ float s_red[DS_NCW];
     __shared__ unsigned long long s_base, s_base_x;
@@ -322,13 +327,13 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         s_rng[tid - 32][3] = p.spt > 0 ? min(hi - lo, p.spt) : 0;
     } else if (tid >= 64 && tid < 64 + ZR_COUNT) {
         const int k = tid - 64;
-        const int n = k == ZR_QKV ? (3 * a.HQ) >> 2 : (k == ZR_H ? a.H >> 2 : (k == ZR_GU ? (2 * a.I) >> 2 : (k == ZR_LOGITS ? a.vocab >> 2 : a.H >> 1)));
+        const int n = k == ZR_QKV ? (a.HQ + 2 * a.HKV) >> 2 : (k == ZR_H ? a.H >> 2 : (k == ZR_GU ? (2 * a.I) >> 2 : (k == ZR_LOGITS ? a.vocab >> 2 : a.H >> 1)));
         s_zr[k][0] = share_lo(n, cta, G); s_zr[k][1] = share_lo(n, cta + 1, G);
     } else if (tid >= 128 && tid < 128 + a.heads) {
         const Phase pa = phase_of(a, PH_ATT, G);
-        const int h = tid - 128;
-        s_clo[h] = (unsigned short)cta_of((long long)h * pa.tpm, pa.U, pa.G);
-        s_chi[h] = (unsigned short)cta_of((long long)(h + 1) * pa.tpm - 1, pa.U, pa.G);
+        const int h = tid - 128, kvh = h / a.n_rep;                // a query head's partials come from the CTAs of its KV head
+        s_clo[h] = (unsigned short)cta_of((long long)kvh * pa.tpm, pa.U, pa.G);
+        s_chi[h] = (unsigned short)cta_of((long long)(kvh + 1) * pa.tpm - 1, pa.U, pa.G);
     }
     __syncthreads();
 
@@ -376,7 +381,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
                 }
                 if (u0 + i0 >= u1) continue;
                 int tile = (u0 + i0) / p.spt, s = (u0 + i0) - tile * p.spt;
-                int mi = tile / p.tpm, ct = tile - mi * p.tpm;
+                int mi = mat_of_tile(p, tile), ct = tile - mat_tile0(p, mi);
                 #pragma unroll 1
                 for (int u = u0 + i0; u < u1; u += 4) {
                     const int m = p.mat0 + mi;
@@ -388,7 +393,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
                     else if (lane == 2) tma_load_2d(base + META_ZQ, &L->tz[m], ct * 16, grow, fb);
                     advance();
                     s += 4;
-                    while (s >= p.spt) { s -= p.spt; if (++ct == p.tpm) { ct = 0; mi++; } }
+                    while (s >= p.spt) { s -= p.spt; if (++ct == mat_tiles(p, mi)) { ct = 0; mi++; } }
                 }
             }
         }
@@ -575,10 +580,10 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
     // range that crosses a matrix boundary stages twice, into slot (matrix - first matrix).  make_get(m) returns the 8-value getter.
     auto stage_phase = [&](const Phase& p, int u0, int u1, auto make_get) {
         if (u1 <= u0) return;
-        const int per_mat = p.tpm * p.spt;
-        const int mi0 = u0 / per_mat, mi1 = ACT ? (u1 - 1) / per_mat : mi0;
+        const int mi0 = mat_of_tile(p, u0 / p.spt), mi1 = ACT ? mat_of_tile(p, (u1 - 1) / p.spt) : mi0;
         for (int mi = mi0; mi <= mi1; mi++) {
-            const int ua = ACT ? max(u0, mi * per_mat) : u0, ub = ACT ? min(u1, (mi + 1) * per_mat) : u1;
+            const int m_lo = mat_tile0(p, mi) * p.spt, m_hi = m_lo + mat_tiles(p, mi) * p.spt;
+            const int ua = ACT ? max(u0, m_lo) : u0, ub = ACT ? min(u1, m_hi) : u1;
             stage_xd(ua % p.spt, min(ub - ua, p.spt), p.spt, make_get(p.mat0 + mi), mi - mi0);
         }
     };
@@ -609,10 +614,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         int cur_tile = tile;
         float acc[4] = {0.f, 0.f, 0.f, 0.f};
         auto flush_tile = [&]() {
-            if (t == 0) {
-                const int mi = cur_tile / p.tpm, col0 = (cur_tile - mi * p.tpm) * TILE;
-                red_add_v4(p.acc + (size_t)mi * p.N + col0 + lane_col, acc[0], acc[1], acc[2], acc[3]);
-            }
+            if (t == 0) red_add_v4(p.acc + (size_t)cur_tile * TILE + lane_col, acc[0], acc[1], acc[2], acc[3]);     // tiles are numbered matrix by matrix
             acc[0] = acc[1] = acc[2] = acc[3] = 0.f;
         };
         // every address below is a 32-bit shared-memory address built from per-lane constants computed once per phase
@@ -629,12 +631,12 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         // 10 % slower plain kernel (measured by A/B builds on one box: any one of these blocks removed restored the speed)
         [[maybe_unused]] int mi_first = 0;                  // staging slot of a tile = its matrix - the first matrix of the CTA's range
         [[maybe_unused]] uint32_t xoff = 0u, soff = 0u;
-        if constexpr (ACT) { mi_first = (u0 / p.spt) / p.tpm; xoff = (uint32_t)(cur_tile / p.tpm - mi_first) * xs_slot; soff = (uint32_t)(cur_tile / p.tpm - mi_first) * seg_slot; }
+        if constexpr (ACT) { mi_first = mat_of_tile(p, u0 / p.spt); xoff = (uint32_t)(mat_of_tile(p, cur_tile) - mi_first) * xs_slot; soff = (uint32_t)(mat_of_tile(p, cur_tile) - mi_first) * seg_slot; }
         bool ready = mbar_try(full0 + ls * 8, par);
         for (; u < u1; u += 4) {
             if (tile != cur_tile) {
                 flush_tile(); cur_tile = tile;
-                if constexpr (ACT) { const uint32_t sl = (uint32_t)(tile / p.tpm - mi_first); xoff = sl * xs_slot; soff = sl * seg_slot; }
+                if constexpr (ACT) { const uint32_t sl = (uint32_t)(mat_of_tile(p, tile) - mi_first); xoff = sl * xs_slot; soff = sl * seg_slot; }
             }
             const uint32_t tok = mbar_wait_tok(full0 + ls * 8, par, ready);
             const int ls_cur = ls;
@@ -755,6 +757,137 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         }
     };
 
+    // ---- ATT under grouped-query attention (n_rep > 1).  A unit is (KV head, 16-position chunk) and its stage of K/V serves all n_rep
+    // query heads of the group: warp wn of a pipeline takes the query heads r = wn, wn + 4, ... over all 16 positions of the stage.  The
+    // running (m, l, o) of a (segment, query head, pipeline) lives in shared memory (gparts, on the x staging area, which is dead between
+    // the QKV GEMV and the O prologue), so a query head of a segment ends with 4 pipeline partials + the new token's, combined into the
+    // CTA's slot of att_part as in the multi-head path.
+    auto att_gqa = [&](const LayerDesc* L, int u0, int u1, int nph, int h0, int nseg) {
+        const int nr = a.n_rep;
+        const float scale = rsqrtf((float)TILE);
+        const int l16 = lane & 15, sub = lane >> 4;
+        half* gq = reinterpret_cast<half*>(xs + gqa_qh_off(nr));        // [2][n_rep][128] q after rope, fp16 (unscaled)
+        float* gkn = reinterpret_cast<float*>(xs + gqa_kn_off(nr));    // [2][128] newest k row (after rope)
+        float* gvn = gkn + 2 * TILE;                                    // [2][128] newest v row
+        auto owner = [&](int kvh) { return min(u1, (kvh + 1) * nph) == (kvh + 1) * nph; };      // holds the KV head's last chunk
+        const half* sr = a.sin + (size_t)a.past_len * TILE;
+        const half* cr = a.cos + (size_t)a.past_len * TILE;
+        // rope q of every query head of the segments (rope.cu:48-67, as the multi-head path); rope k and write the k / v cache rows
+        // once per KV head, by its owner; every pipeline partial to neutral
+        for (int i = tid; i < nseg * nr * TILE; i += DS_CONSUMERS) {
+            const int d = i & 127, w = i >> 7, sg = w / nr;
+            const float* aq = a.acc_qkv + (size_t)((h0 + sg) * nr + (w - sg * nr)) * TILE;
+            const half qv = __float2half_rn(__ldcg(aq + d)), qo = __float2half_rn(__ldcg(aq + (d ^ 64)));
+            const half sn = d < 64 ? __hneg(sr[d]) : sr[d];
+            gq[w * TILE + d] = __hfma(qv, cr[d], __hmul(qo, sn));
+        }
+        for (int i = tid; i < nseg * TILE; i += DS_CONSUMERS) {
+            const int d = i & 127, sg = i >> 7, kvh = h0 + sg;
+            if (!owner(kvh)) continue;
+            const half sn = d < 64 ? __hneg(sr[d]) : sr[d];
+            const float* ak = a.acc_qkv + a.HQ + (size_t)kvh * TILE;
+            const half kv = __float2half_rn(__ldcg(ak + d)), ko = __float2half_rn(__ldcg(ak + (d ^ 64)));
+            const half kr = __hfma(kv, cr[d], __hmul(ko, sn));
+            const half vv = __float2half_rn(__ldcg(a.acc_qkv + a.HQ + a.HKV + (size_t)kvh * TILE + d));
+            gkn[sg * TILE + d] = __half2float(kr); gvn[sg * TILE + d] = __half2float(vv);
+            const size_t off = ((size_t)kvh * a.max_seq + a.past_len) * TILE + d;      // cache layout q4_attn.cu:32-51, kv_heads rows
+            L->kc[off] = kr; L->vc[off] = vv;
+        }
+        for (int i = tid; i < nseg * nr * 4 * PART_LD; i += DS_CONSUMERS) {
+            const int w = i / (4 * PART_LD), e = i - w * 4 * PART_LD;
+            gparts[w * 5 * PART_LD + e] = (e % PART_LD) == 128 ? -INFINITY : 0.f;
+        }
+        consumer_sync();
+        constexpr float LOG2E = 1.4426950408889634f;
+        int u = u0 + ((wk - jbase) & 3);
+        int kvh = u / nph, ch = u - kvh * nph;
+        for (; u < u1; u += 4) {
+            const int sg = kvh - h0;
+            int nv = a.past_len - ch * 16; nv = nv < 0 ? 0 : (nv > 16 ? 16 : nv);
+            const uint32_t sb = ring_a + (uint32_t)ls * STAGE_STRIDE + mbar_wait_tok(full0 + ls * 8, par, false);
+            float dep = 0.f;
+            for (int r = wn; r < nr && !(a.debug & 2); r += 4) {
+                const uint4 qh = *reinterpret_cast<const uint4*>(gq + (sg * nr + r) * TILE + l16 * 8);
+                // scores of the 16 positions: position it * 2 + sub in the lanes of half-warp sub (16 lanes x 8 dims)
+                float sc[8], smax = -INFINITY;
+                #pragma unroll
+                for (int it = 0; it < 8; it++) {
+                    const uint4 kv = lds128(sb + (uint32_t)(it * 2 + sub) * 256u + (uint32_t)l16 * 16u);
+                    float d = 0.f;
+                    d = fhfma2(kv.x, qh.x, d); d = fhfma2(kv.y, qh.y, d); d = fhfma2(kv.z, qh.z, d); d = fhfma2(kv.w, qh.w, d);
+                    d += __shfl_xor_sync(0xffffffffu, d, 8); d += __shfl_xor_sync(0xffffffffu, d, 4);
+                    d += __shfl_xor_sync(0xffffffffu, d, 2); d += __shfl_xor_sync(0xffffffffu, d, 1);
+                    sc[it] = it * 2 + sub < nv ? d * scale : -INFINITY;
+                    smax = fmaxf(smax, sc[it]);
+                }
+                smax = fmaxf(smax, __shfl_xor_sync(0xffffffffu, smax, 16));
+                dep += smax;
+                if (smax > -INFINITY) {
+                    float* st = gparts + ((sg * nr + r) * 5 + wk) * PART_LD;
+                    const float m = st[128], lsum = st[129];
+                    float4 o = *reinterpret_cast<const float4*>(st + lane * 4);
+                    const float mnew = fmaxf(m, smax);
+                    const float alpha = ex2_ftz((m - mnew) * LOG2E);
+                    float psum = 0.f;
+                    #pragma unroll
+                    for (int it = 0; it < 8; it++) { sc[it] = ex2_ftz((sc[it] - mnew) * LOG2E); psum += sc[it]; }
+                    psum += __shfl_xor_sync(0xffffffffu, psum, 16);
+                    o.x *= alpha; o.y *= alpha; o.z *= alpha; o.w *= alpha;
+                    #pragma unroll
+                    for (int q = 0; q < 16; q++) {
+                        const float wgt = __shfl_sync(0xffffffffu, sc[q >> 1], (q & 1) * 16);
+                        const uint2 vv = lds64_if(sb + 4096u + (uint32_t)q * 256u + (uint32_t)lane * 8u, q < nv);
+                        const float2 f0 = __half22float2(*reinterpret_cast<const half2*>(&vv.x));
+                        const float2 f1 = __half22float2(*reinterpret_cast<const half2*>(&vv.y));
+                        o.x = fmaf(wgt, f0.x, o.x); o.y = fmaf(wgt, f0.y, o.y); o.z = fmaf(wgt, f1.x, o.z); o.w = fmaf(wgt, f1.y, o.w);
+                    }
+                    *reinterpret_cast<float4*>(st + lane * 4) = o;
+                    __syncwarp();                                   // every lane has read (m, l) before lane 0 replaces them
+                    if (lane == 0) { st[128] = mnew; st[129] = lsum * alpha + psum; }
+                    dep += o.x;
+                }
+            }
+            __syncwarp();
+            // the arrive consumes values computed from every load of the stage: it cannot be scheduled before them
+            if (lane == 0) mbar_arrive_dep(empty0 + ls * 8, dep);
+            if (++ls == depth) { ls = 0; par ^= 1u; }
+            ch += 4;
+            while (ch >= nph) { ch -= nph; kvh++; }
+        }
+        // the new token (KV heads whose last chunk this CTA holds): score q . k_new, weight 1 in its own partial, per query head
+        for (int w = warp; w < nseg * nr; w += DS_NCW) {
+            const int sg = w / nr;
+            if (!owner(h0 + sg)) continue;
+            float d = 0.f;
+            #pragma unroll
+            for (int c = 0; c < 4; c++) d = fmaf(__half2float(gq[w * TILE + lane * 4 + c]) * scale, gkn[sg * TILE + lane * 4 + c], d);
+            #pragma unroll
+            for (int off = 16; off > 0; off >>= 1) d += __shfl_xor_sync(0xffffffffu, d, off);
+            float* pw = gparts + (w * 5 + 4) * PART_LD;
+            *reinterpret_cast<float4*>(pw + lane * 4) = *reinterpret_cast<const float4*>(gvn + sg * TILE + lane * 4);
+            if (lane == 0) { pw[128] = d; pw[129] = 1.0f; }
+        }
+        consumer_sync();
+        // this CTA's partial of every query head of its segments -> its slot of the head's CTA range
+        for (int i = tid; i < nseg * nr * TILE; i += DS_CONSUMERS) {
+            const int d = i & 127, w = i >> 7, sg = w / nr, h = (h0 + sg) * nr + (w - sg * nr);
+            const float* pp = gparts + w * 5 * PART_LD;
+            const int np = owner(h0 + sg) ? 5 : 4;
+            float M = -INFINITY;
+            for (int k = 0; k < np; k++) M = fmaxf(M, pp[k * PART_LD + 128]);
+            float Lt = 0.f, ov = 0.f;
+            for (int k = 0; k < np; k++) {
+                const float mw = pp[k * PART_LD + 128];
+                const float wgt = mw == -INFINITY ? 0.f : __expf(mw - M);
+                Lt = fmaf(pp[k * PART_LD + 129], wgt, Lt);
+                ov = fmaf(pp[k * PART_LD + d], wgt, ov);
+            }
+            float* dst = a.att_part + ((size_t)h * a.att_slots + (cta - (int)s_clo[h])) * PART_LD;
+            dst[d] = ov;
+            if (d == 0) { dst[128] = M; dst[129] = Lt; }
+        }
+    };
+
     float rm = 0.f;
     #pragma unroll 1
     for (int l = 0; l < a.n_layers; l++) {
@@ -788,144 +921,147 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             const int l16 = lane & 15, sub = lane >> 4;
             const int h0 = u1 > u0 ? u0 / nph : 0;
             const int nseg = u1 > u0 ? (u1 - 1) / nph - h0 + 1 : 0;            // <= 2 (heads <= grid, checked on the host)
-            // every segment's q (and the new k / v rows where this CTA owns the head's last chunk): one L2 round trip
-            if (tid < nseg * TILE) {
-                const int sg = tid >> 7, d = tid & 127, h = h0 + sg;
-                const bool owner = min(u1, (h + 1) * nph) == (h + 1) * nph;
-                // fp16 projection result, rope in fp16 with the reference's instruction order (rope.cu:48-67)
-                const half* sr = a.sin + (size_t)a.past_len * TILE;
-                const half* cr = a.cos + (size_t)a.past_len * TILE;
-                const float* aq = a.acc_qkv + (size_t)h * TILE;
-                const half qv = __float2half_rn(__ldcg(aq + d)), qo = __float2half_rn(__ldcg(aq + (d ^ 64)));
-                const half sn = d < 64 ? __hneg(sr[d]) : sr[d];
-                const half qr = __hfma(qv, cr[d], __hmul(qo, sn));
-                qh_s[sg * TILE + d] = qr;
-                q_s[sg * TILE + d] = __half2float(qr) * scale;
-                if (owner) {
-                    const float* ak = a.acc_qkv + a.HQ + (size_t)h * TILE;
-                    const half kv = __float2half_rn(__ldcg(ak + d)), ko = __float2half_rn(__ldcg(ak + (d ^ 64)));
-                    const half kr = __hfma(kv, cr[d], __hmul(ko, sn));
-                    const half vv = __float2half_rn(__ldcg(a.acc_qkv + 2 * a.HQ + (size_t)h * TILE + d));
-                    kn_s[sg * TILE + d] = __half2float(kr); vn_s[sg * TILE + d] = __half2float(vv);
-                    const size_t off = ((size_t)h * a.max_seq + a.past_len) * TILE + d;      // cache layout q4_attn.cu:32-51
-                    L->kc[off] = kr; L->vc[off] = vv;
+            if constexpr (GQA) att_gqa(L, u0, u1, nph, h0, nseg);
+            else {
+                // every segment's q (and the new k / v rows where this CTA owns the head's last chunk): one L2 round trip
+                if (tid < nseg * TILE) {
+                    const int sg = tid >> 7, d = tid & 127, h = h0 + sg;
+                    const bool owner = min(u1, (h + 1) * nph) == (h + 1) * nph;
+                    // fp16 projection result, rope in fp16 with the reference's instruction order (rope.cu:48-67)
+                    const half* sr = a.sin + (size_t)a.past_len * TILE;
+                    const half* cr = a.cos + (size_t)a.past_len * TILE;
+                    const float* aq = a.acc_qkv + (size_t)h * TILE;
+                    const half qv = __float2half_rn(__ldcg(aq + d)), qo = __float2half_rn(__ldcg(aq + (d ^ 64)));
+                    const half sn = d < 64 ? __hneg(sr[d]) : sr[d];
+                    const half qr = __hfma(qv, cr[d], __hmul(qo, sn));
+                    qh_s[sg * TILE + d] = qr;
+                    q_s[sg * TILE + d] = __half2float(qr) * scale;
+                    if (owner) {
+                        const float* ak = a.acc_qkv + a.HQ + (size_t)h * TILE;
+                        const half kv = __float2half_rn(__ldcg(ak + d)), ko = __float2half_rn(__ldcg(ak + (d ^ 64)));
+                        const half kr = __hfma(kv, cr[d], __hmul(ko, sn));
+                        const half vv = __float2half_rn(__ldcg(a.acc_qkv + 2 * a.HQ + (size_t)h * TILE + d));
+                        kn_s[sg * TILE + d] = __half2float(kr); vn_s[sg * TILE + d] = __half2float(vv);
+                        const size_t off = ((size_t)h * a.max_seq + a.past_len) * TILE + d;      // cache layout q4_attn.cu:32-51
+                        L->kc[off] = kr; L->vc[off] = vv;
+                    }
                 }
-            }
-            consumer_sync();
-            {
-                // this pipeline's stages, in order; the 4 warps of the pipeline take 4 positions of each 16-position chunk
-                uint4 qh = make_uint4(0u, 0u, 0u, 0u);          // 8 fp16 q values of this lane's dims
-                float m = -INFINITY, lsum = 0.f, o[4] = {0.f, 0.f, 0.f, 0.f};
-                int cur = -1;                                  // segment the running (m, l, o) belongs to
-                auto put_part = [&]() {
-                    float* pw = parts + (cur * 17 + warp) * PART_LD;
-                    *reinterpret_cast<float4*>(pw + lane * 4) = make_float4(o[0], o[1], o[2], o[3]);
-                    if (lane == 0) { pw[128] = m; pw[129] = lsum; }
-                };
-                int u = u0 + ((wk - jbase) & 3);
-                int h = u / nph, ch = u - h * nph;             // (head, chunk) of the unit, advanced without divisions
-                // 32-bit shared addresses from per-lane constants, as in the GEMV loop: K row of position wn * 4 + it * 2 + sub (16 lanes x
-                // 16 B), V row of position wn * 4 + q (32 lanes x 8 B)
-                const uint32_t k_lane = (uint32_t)((wn * 4 + sub) * 256 + l16 * 16);
-                const uint32_t v_lane = (uint32_t)(4096 + wn * 4 * 256 + lane * 8);
-                constexpr float LOG2E = 1.4426950408889634f;
-                for (; u < u1; u += 4) {
-                    const int sg = h - h0;
-                    if (sg != cur) {
-                        if (cur >= 0) put_part();
-                        cur = sg; m = -INFINITY; lsum = 0.f; o[0] = o[1] = o[2] = o[3] = 0.f;
-                        qh = *reinterpret_cast<const uint4*>(qh_s + sg * TILE + l16 * 8);
-                    }
-                    int nv = a.past_len - ch * 16; nv = nv < 0 ? 0 : (nv > 16 ? 16 : nv);
-                    // the zero token ties the (freely schedulable) asm loads below to the wait
-                    const uint32_t sb = ring_a + (uint32_t)ls * STAGE_STRIDE + mbar_wait_tok(full0 + ls * 8, par, false);
-                    float sc2[2];
-                    float smax = -INFINITY;
-                    #pragma unroll
-                    for (int it = 0; it < 2; it++) {
-                        const int pp = wn * 4 + it * 2 + sub;
-                        const uint4 kv = lds128(sb + k_lane + it * 512);
-                        float d = 0.f;
-                        d = fhfma2(kv.x, qh.x, d); d = fhfma2(kv.y, qh.y, d); d = fhfma2(kv.z, qh.z, d); d = fhfma2(kv.w, qh.w, d);
-                        d += __shfl_xor_sync(0xffffffffu, d, 8); d += __shfl_xor_sync(0xffffffffu, d, 4);
-                        d += __shfl_xor_sync(0xffffffffu, d, 2); d += __shfl_xor_sync(0xffffffffu, d, 1);
-                        sc2[it] = pp < nv ? d * scale : -INFINITY;
-                        smax = fmaxf(smax, sc2[it]);
-                    }
-                    smax = fmaxf(smax, __shfl_xor_sync(0xffffffffu, smax, 16));
-                    if (smax > -INFINITY && !(a.debug & 2)) {           // this warp has at least one valid position in the chunk
-                        const float mnew = fmaxf(m, smax);
-                        const float alpha = ex2_ftz((m - mnew) * LOG2E);
-                        sc2[0] = ex2_ftz((sc2[0] - mnew) * LOG2E); sc2[1] = ex2_ftz((sc2[1] - mnew) * LOG2E);
-                        float psum = sc2[0] + sc2[1];
-                        psum += __shfl_xor_sync(0xffffffffu, psum, 16);
-                        lsum = lsum * alpha + psum;
+                consumer_sync();
+                {
+                    // this pipeline's stages, in order; the 4 warps of the pipeline take 4 positions of each 16-position chunk
+                    uint4 qh = make_uint4(0u, 0u, 0u, 0u);          // 8 fp16 q values of this lane's dims
+                    float m = -INFINITY, lsum = 0.f, o[4] = {0.f, 0.f, 0.f, 0.f};
+                    int cur = -1;                                  // segment the running (m, l, o) belongs to
+                    auto put_part = [&]() {
+                        float* pw = parts + (cur * 17 + warp) * PART_LD;
+                        *reinterpret_cast<float4*>(pw + lane * 4) = make_float4(o[0], o[1], o[2], o[3]);
+                        if (lane == 0) { pw[128] = m; pw[129] = lsum; }
+                    };
+                    int u = u0 + ((wk - jbase) & 3);
+                    int h = u / nph, ch = u - h * nph;             // (head, chunk) of the unit, advanced without divisions
+                    // 32-bit shared addresses from per-lane constants, as in the GEMV loop: K row of position wn * 4 + it * 2 + sub (16 lanes x
+                    // 16 B), V row of position wn * 4 + q (32 lanes x 8 B)
+                    const uint32_t k_lane = (uint32_t)((wn * 4 + sub) * 256 + l16 * 16);
+                    const uint32_t v_lane = (uint32_t)(4096 + wn * 4 * 256 + lane * 8);
+                    constexpr float LOG2E = 1.4426950408889634f;
+                    for (; u < u1; u += 4) {
+                        const int sg = h - h0;
+                        if (sg != cur) {
+                            if (cur >= 0) put_part();
+                            cur = sg; m = -INFINITY; lsum = 0.f; o[0] = o[1] = o[2] = o[3] = 0.f;
+                            qh = *reinterpret_cast<const uint4*>(qh_s + sg * TILE + l16 * 8);
+                        }
+                        int nv = a.past_len - ch * 16; nv = nv < 0 ? 0 : (nv > 16 ? 16 : nv);
+                        // the zero token ties the (freely schedulable) asm loads below to the wait
+                        const uint32_t sb = ring_a + (uint32_t)ls * STAGE_STRIDE + mbar_wait_tok(full0 + ls * 8, par, false);
+                        float sc2[2];
+                        float smax = -INFINITY;
                         #pragma unroll
-                        for (int c = 0; c < 4; c++) o[c] *= alpha;
-                        m = mnew;
-                        #pragma unroll
-                        for (int q = 0; q < 4; q++) {
-                            // positions past the context end: weight 0 (their score is -inf) times a row that is not loaded (zeros)
-                            const float wgt = __shfl_sync(0xffffffffu, sc2[q >> 1], (q & 1) * 16);
-                            const uint2 vv = lds64_if(sb + v_lane + q * 256, wn * 4 + q < nv);
-                            const float2 f0 = __half22float2(*reinterpret_cast<const half2*>(&vv.x));
-                            const float2 f1 = __half22float2(*reinterpret_cast<const half2*>(&vv.y));
-                            o[0] = fmaf(wgt, f0.x, o[0]); o[1] = fmaf(wgt, f0.y, o[1]); o[2] = fmaf(wgt, f1.x, o[2]); o[3] = fmaf(wgt, f1.y, o[3]);
+                        for (int it = 0; it < 2; it++) {
+                            const int pp = wn * 4 + it * 2 + sub;
+                            const uint4 kv = lds128(sb + k_lane + it * 512);
+                            float d = 0.f;
+                            d = fhfma2(kv.x, qh.x, d); d = fhfma2(kv.y, qh.y, d); d = fhfma2(kv.z, qh.z, d); d = fhfma2(kv.w, qh.w, d);
+                            d += __shfl_xor_sync(0xffffffffu, d, 8); d += __shfl_xor_sync(0xffffffffu, d, 4);
+                            d += __shfl_xor_sync(0xffffffffu, d, 2); d += __shfl_xor_sync(0xffffffffu, d, 1);
+                            sc2[it] = pp < nv ? d * scale : -INFINITY;
+                            smax = fmaxf(smax, sc2[it]);
+                        }
+                        smax = fmaxf(smax, __shfl_xor_sync(0xffffffffu, smax, 16));
+                        if (smax > -INFINITY && !(a.debug & 2)) {           // this warp has at least one valid position in the chunk
+                            const float mnew = fmaxf(m, smax);
+                            const float alpha = ex2_ftz((m - mnew) * LOG2E);
+                            sc2[0] = ex2_ftz((sc2[0] - mnew) * LOG2E); sc2[1] = ex2_ftz((sc2[1] - mnew) * LOG2E);
+                            float psum = sc2[0] + sc2[1];
+                            psum += __shfl_xor_sync(0xffffffffu, psum, 16);
+                            lsum = lsum * alpha + psum;
+                            #pragma unroll
+                            for (int c = 0; c < 4; c++) o[c] *= alpha;
+                            m = mnew;
+                            #pragma unroll
+                            for (int q = 0; q < 4; q++) {
+                                // positions past the context end: weight 0 (their score is -inf) times a row that is not loaded (zeros)
+                                const float wgt = __shfl_sync(0xffffffffu, sc2[q >> 1], (q & 1) * 16);
+                                const uint2 vv = lds64_if(sb + v_lane + q * 256, wn * 4 + q < nv);
+                                const float2 f0 = __half22float2(*reinterpret_cast<const half2*>(&vv.x));
+                                const float2 f1 = __half22float2(*reinterpret_cast<const half2*>(&vv.y));
+                                o[0] = fmaf(wgt, f0.x, o[0]); o[1] = fmaf(wgt, f0.y, o[1]); o[2] = fmaf(wgt, f1.x, o[2]); o[3] = fmaf(wgt, f1.y, o[3]);
+                            }
+                        }
+                        __syncwarp();
+                        // the arrive consumes values computed from every load of the stage: it cannot be scheduled before them
+                        if (lane == 0) mbar_arrive_dep(empty0 + ls * 8, o[0] + smax);
+                        if (++ls == depth) { ls = 0; par ^= 1u; }
+                        ch += 4;
+                        while (ch >= nph) { ch -= nph; h++; }
+                    }
+                    if (cur >= 0) put_part();
+                    // segments this warp saw no stage of: an empty partial
+                    for (int sg = 0; sg < nseg; sg++) {
+                        const int first = max(u0, (h0 + sg) * nph), last = min(u1, (h0 + sg + 1) * nph);
+                        // did this pipeline get a stage of segment sg?  stages of the segment: local indices [first - u0, last - u0)
+                        const int i0 = (first - u0) + ((wk - (jbase + (first - u0))) & 3);
+                        if (i0 >= last - u0) {
+                            float* pw = parts + (sg * 17 + warp) * PART_LD;
+                            *reinterpret_cast<float4*>(pw + lane * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+                            if (lane == 0) { pw[128] = -INFINITY; pw[129] = 0.f; }
                         }
                     }
-                    __syncwarp();
-                    // the arrive consumes values computed from every load of the stage: it cannot be scheduled before them
-                    if (lane == 0) mbar_arrive_dep(empty0 + ls * 8, o[0] + smax);
-                    if (++ls == depth) { ls = 0; par ^= 1u; }
-                    ch += 4;
-                    while (ch >= nph) { ch -= nph; h++; }
-                }
-                if (cur >= 0) put_part();
-                // segments this warp saw no stage of: an empty partial
-                for (int sg = 0; sg < nseg; sg++) {
-                    const int first = max(u0, (h0 + sg) * nph), last = min(u1, (h0 + sg + 1) * nph);
-                    // did this pipeline get a stage of segment sg?  stages of the segment: local indices [first - u0, last - u0)
-                    const int i0 = (first - u0) + ((wk - (jbase + (first - u0))) & 3);
-                    if (i0 >= last - u0) {
-                        float* pw = parts + (sg * 17 + warp) * PART_LD;
-                        *reinterpret_cast<float4*>(pw + lane * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (lane == 0) { pw[128] = -INFINITY; pw[129] = 0.f; }
+                    if (warp < nseg) {
+                        // the new token itself (segments whose last chunk this CTA holds): score q . k_new, weight 1 in its own partial
+                        const int sg = warp, h = h0 + sg;
+                        if (min(u1, (h + 1) * nph) == (h + 1) * nph) {
+                            float d = 0.f;
+                            #pragma unroll
+                            for (int c = 0; c < 4; c++) d = fmaf(q_s[sg * TILE + lane * 4 + c], kn_s[sg * TILE + lane * 4 + c], d);
+                            #pragma unroll
+                            for (int off = 16; off > 0; off >>= 1) d += __shfl_xor_sync(0xffffffffu, d, off);
+                            float* pw = parts + (sg * 17 + 16) * PART_LD;
+                            *reinterpret_cast<float4*>(pw + lane * 4) = *reinterpret_cast<const float4*>(vn_s + sg * TILE + lane * 4);
+                            if (lane == 0) { pw[128] = d; pw[129] = 1.0f; }
+                        }
                     }
                 }
-                if (warp < nseg) {
-                    // the new token itself (segments whose last chunk this CTA holds): score q . k_new, weight 1 in its own partial
-                    const int sg = warp, h = h0 + sg;
-                    if (min(u1, (h + 1) * nph) == (h + 1) * nph) {
-                        float d = 0.f;
-                        #pragma unroll
-                        for (int c = 0; c < 4; c++) d = fmaf(q_s[sg * TILE + lane * 4 + c], kn_s[sg * TILE + lane * 4 + c], d);
-                        #pragma unroll
-                        for (int off = 16; off > 0; off >>= 1) d += __shfl_xor_sync(0xffffffffu, d, off);
-                        float* pw = parts + (sg * 17 + 16) * PART_LD;
-                        *reinterpret_cast<float4*>(pw + lane * 4) = *reinterpret_cast<const float4*>(vn_s + sg * TILE + lane * 4);
-                        if (lane == 0) { pw[128] = d; pw[129] = 1.0f; }
+                consumer_sync();
+                if (tid < nseg * TILE) {
+                    const int sg = tid >> 7, d = tid & 127, h = h0 + sg;
+                    const bool owner = min(u1, (h + 1) * nph) == (h + 1) * nph;
+                    const float* pp = parts + sg * 17 * PART_LD;
+                    const int np = owner ? 17 : 16;
+                    float M = -INFINITY;
+                    for (int w = 0; w < np; w++) M = fmaxf(M, pp[w * PART_LD + 128]);
+                    float Lt = 0.f, ov = 0.f;
+                    for (int w = 0; w < np; w++) {
+                        const float mw = pp[w * PART_LD + 128];
+                        const float wgt = mw == -INFINITY ? 0.f : __expf(mw - M);
+                        Lt = fmaf(pp[w * PART_LD + 129], wgt, Lt);
+                        ov = fmaf(pp[w * PART_LD + d], wgt, ov);
                     }
+                    const int slot_id = cta - (int)s_clo[h];
+                    float* dst = a.att_part + ((size_t)h * a.att_slots + slot_id) * PART_LD;
+                    dst[d] = ov;
+                    if (d == 0) { dst[128] = M; dst[129] = Lt; }
                 }
-            }
-            consumer_sync();
-            if (tid < nseg * TILE) {
-                const int sg = tid >> 7, d = tid & 127, h = h0 + sg;
-                const bool owner = min(u1, (h + 1) * nph) == (h + 1) * nph;
-                const float* pp = parts + sg * 17 * PART_LD;
-                const int np = owner ? 17 : 16;
-                float M = -INFINITY;
-                for (int w = 0; w < np; w++) M = fmaxf(M, pp[w * PART_LD + 128]);
-                float Lt = 0.f, ov = 0.f;
-                for (int w = 0; w < np; w++) {
-                    const float mw = pp[w * PART_LD + 128];
-                    const float wgt = mw == -INFINITY ? 0.f : __expf(mw - M);
-                    Lt = fmaf(pp[w * PART_LD + 129], wgt, Lt);
-                    ov = fmaf(pp[w * PART_LD + d], wgt, ov);
-                }
-                const int slot_id = cta - (int)s_clo[h];
-                float* dst = a.att_part + ((size_t)h * a.att_slots + slot_id) * PART_LD;
-                dst[d] = ov;
-                if (d == 0) { dst[128] = M; dst[129] = Lt; }
             }
             jbase += u1 - u0;
             stamp(l, 4);
@@ -1147,10 +1283,11 @@ struct exl_decode_plan
     int grid = 0;
 };
 
-static const void* step_kernel_for(bool act, bool tp)
+static const void* step_kernel_for(bool act, bool tp, bool gqa)
 {
-    if (act) return tp ? (const void*)decode_step_kernel<true, true> : (const void*)decode_step_kernel<true, false>;
-    return tp ? (const void*)decode_step_kernel<false, true> : (const void*)decode_step_kernel<false, false>;
+    if (gqa) return act ? (const void*)decode_step_kernel<true, false, true> : (const void*)decode_step_kernel<false, false, true>;     // no GQA under TP
+    if (act) return tp ? (const void*)decode_step_kernel<true, true, false> : (const void*)decode_step_kernel<true, false, false>;
+    return tp ? (const void*)decode_step_kernel<false, true, false> : (const void*)decode_step_kernel<false, false, false>;
 }
 
 static int plan_fail(exl_decode_plan* p, int rc)
@@ -1176,6 +1313,12 @@ extern "C" int exl_decode_plan_create(const exl_decode_desc* d, exl_decode_plan*
     DeviceGuard guard(q0->device);
     const int H = q0->K, HQ = q0->N, I = d->mats[4]->N;
     if (d->head_dim != TILE || d->num_heads * TILE != HQ) return exl_set_err(EXL_ERR_ARG, "decode_plan: head_dim must be 128 and heads * 128 == q_proj width (%d heads, width %d)", d->num_heads, HQ);
+    const int kv_heads = d->num_kv_heads ? d->num_kv_heads : d->num_heads;         // 0: multi-head attention
+    if (kv_heads < 1 || kv_heads > d->num_heads || d->num_heads % kv_heads)
+        return exl_set_err(EXL_ERR_ARG, "decode_plan: num_kv_heads (%d) must divide num_heads (%d)", kv_heads, d->num_heads);
+    if (kv_heads != d->num_heads && d->tp_world > 1)
+        return exl_set_err(EXL_ERR_ARG, "decode_plan: grouped-query attention (%d heads over %d KV heads) under tensor parallelism is not supported by the fused step: use the per-op path", d->num_heads, kv_heads);
+    const int HKV = kv_heads * TILE;
     if (H % 512 || HQ % TILE || I % TILE) return exl_set_err(EXL_ERR_ARG, "decode_plan: widths must be multiples of 128 (hidden of 512): hidden %d attn %d inter %d", H, HQ, I);
     const int gs = q0->groupsize;
     int gs32 = gs / 32, sh = 0;
@@ -1185,7 +1328,7 @@ extern "C" int exl_decode_plan_create(const exl_decode_desc* d, exl_decode_plan*
     } else sh = 30;
     std::vector<LayerDesc> L((size_t)d->n_layers);
     bool any_act = false;
-    const int expectK[7] = {H, H, H, HQ, H, H, I}, expectN[7] = {HQ, HQ, HQ, H, I, I, H};
+    const int expectK[7] = {H, H, H, HQ, H, H, I}, expectN[7] = {HQ, HKV, HKV, H, I, I, H};      // k, v: kv_heads * 128 wide
     for (int l = 0; l < d->n_layers; l++) {
         memset(&L[l], 0, sizeof(LayerDesc));
         for (int i = 0; i < 7; i++) {
@@ -1206,7 +1349,8 @@ extern "C" int exl_decode_plan_create(const exl_decode_desc* d, exl_decode_plan*
     p->device = q0->device;
     StepArgs& a = p->args;
     memset(&a, 0, sizeof(a));
-    a.n_layers = d->n_layers; a.H = H; a.HQ = HQ; a.I = I; a.heads = d->num_heads; a.max_seq = d->max_seq_len; a.gshift = sh;
+    a.n_layers = d->n_layers; a.H = H; a.HQ = HQ; a.HKV = HKV; a.I = I; a.heads = d->num_heads; a.max_seq = d->max_seq_len; a.gshift = sh;
+    a.kv_heads = kv_heads; a.n_rep = d->num_heads / kv_heads;
     a.eps = d->rms_eps; a.sin = (const half*)d->sin; a.cos = (const half*)d->cos;
     a.final_norm = (const half*)d->final_norm; a.lm_head = (const half*)d->lm_head; a.vocab = d->lm_head ? d->vocab : 0;
     if (d->lm_head && (!d->final_norm || d->vocab % 4)) return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: lm_head needs final_norm and vocab %% 4 == 0"));
@@ -1216,7 +1360,7 @@ extern "C" int exl_decode_plan_create(const exl_decode_desc* d, exl_decode_plan*
         return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: act-order matrices under tensor parallelism are not supported by the fused step (o_proj needs the all-gathered attention output): use the per-op path"));
     int dev_smem = 0;
     cudaDeviceGetAttribute(&dev_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, p->device);
-    const size_t fixed = smem_fixed_bytes(H, HQ, I, any_act);
+    const size_t fixed = smem_fixed_bytes(H, HQ, I, any_act, a.n_rep);
     int depth = ring_depth_for((size_t)dev_smem, fixed);
     if (const char* e = getenv("EXL_DS_DEPTH")) { int v = atoi(e); if (v >= 1 && v < depth) depth = v; }
     if (depth < 2) return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: model too wide for the shared-memory plan (%d ring stages per pipeline)", depth));
@@ -1224,7 +1368,7 @@ extern "C" int exl_decode_plan_create(const exl_decode_desc* d, exl_decode_plan*
     a.depth = depth;
     p->smem = smem_dynamic_bytes(fixed, depth);
     if ((size_t)H * 2 > (size_t)a.spt_max * 256) return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: internal: head staging does not fit"));
-    const void* kfn = step_kernel_for(any_act, d->tp_world > 1);
+    const void* kfn = step_kernel_for(any_act, d->tp_world > 1, a.n_rep > 1);
     cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem);
     if (e != cudaSuccess) return plan_fail(p, exl_set_err(EXL_ERR_CUDA, "decode_plan: smem attribute (%zu B): %s", p->smem, cudaGetErrorString(e)));
     int per_sm = 0;
@@ -1232,11 +1376,11 @@ extern "C" int exl_decode_plan_create(const exl_decode_desc* d, exl_decode_plan*
     if (e != cudaSuccess || per_sm < 1) return plan_fail(p, exl_set_err(EXL_ERR_CUDA, "decode_plan: kernel does not fit an SM (smem %zu)", p->smem));
     p->grid = ds->num_sms;
     if (const char* eg = getenv("EXL_DS_GRID")) { int v = atoi(eg); if (v >= 1 && v <= ds->num_sms) p->grid = v; }
-    a.att_slots = att_slots_for(p->grid, d->num_heads);
+    a.att_slots = att_slots_for(p->grid, d->num_heads, kv_heads);
     // scratch: accumulators | attention partials | barrier
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
-    const size_t o_qkv = take((size_t)3 * HQ * 4), o_o = take((size_t)H * 4), o_gu = take((size_t)2 * I * 4), o_d = take((size_t)H * 4);
+    const size_t o_qkv = take((size_t)(HQ + 2 * HKV) * 4), o_o = take((size_t)H * 4), o_gu = take((size_t)2 * I * 4), o_d = take((size_t)H * 4);
     const size_t o_att = take((size_t)d->num_heads * a.att_slots * PART_LD * 4), o_bar = take(256), o_av = take((size_t)HQ * 2);
     const bool want_trace = getenv("EXL_DS_TRACE") != nullptr;
     const size_t o_trace = want_trace ? take((size_t)p->grid * TRACE_LAYERS * 24 * 8) : 0;
@@ -1340,7 +1484,7 @@ extern "C" int exl_decode_step(exl_decode_plan* p, const void* x_in, int past_le
     DeviceGuard guard(p->device);
     StepArgs a = p->args;
     a.x_in = (const half*)x_in; a.x_out = (half*)x_out; a.logits = (float*)logits; a.past_len = past_len;
-    if (att_needs_reset(a.heads, past_len, p->grid)) {
+    if (att_needs_reset(a.heads, a.kv_heads, past_len, p->grid)) {
         // short context: some CTAs inside a head's CTA range own no attention unit in this launch (stateless test, so a captured
         // CUDA graph -- past_len is baked into it -- replays the same decision)
         const int n = a.heads * a.att_slots * PART_LD;
@@ -1356,7 +1500,7 @@ extern "C" int exl_decode_step(exl_decode_plan* p, const void* x_in, int past_le
     cfg.gridDim = dim3((unsigned)p->grid); cfg.blockDim = dim3(DS_THREADS); cfg.dynamicSmemBytes = p->smem; cfg.stream = (cudaStream_t)stream_;
     cfg.attrs = at; cfg.numAttrs = 1;
     void* kargs[1] = {(void*)&a};
-    cudaError_t e = cudaLaunchKernelExC(&cfg, step_kernel_for(a.act != 0, a.tp_world > 1), kargs);
+    cudaError_t e = cudaLaunchKernelExC(&cfg, step_kernel_for(a.act != 0, a.tp_world > 1, a.n_rep > 1), kargs);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     if (e != cudaSuccess) return exl_set_err(EXL_ERR_CUDA, "launch of decode_step_kernel failed: %s (grid %d, smem %zu)", cudaGetErrorString(e), p->grid, p->smem);
     return EXL_OK;

@@ -6,6 +6,8 @@
 // shard and context length on the CPU -- a schedule mistake on the GPU is a trapped launch, so it is worth proving first.
 #pragma once
 #include <cstddef>
+#include <type_traits>
+#include <utility>
 
 #if defined(__CUDACC__)
 #define DS_HD __host__ __device__ __forceinline__
@@ -21,6 +23,7 @@ constexpr int STAGE_STRIDE = W_BYTES + 2048;     // ring stage: weights + scale 
 constexpr int PART_LD = 132;                     // attention partial: o[128], m, l, pad
 constexpr int MAX_DEPTH = 6;                     // ring stages per pipeline
 constexpr int ATT_CTAS_PER_HEAD = 7;             // at most this many CTAs share one head in the attention phase (when heads are few)
+constexpr int ATT_CTAS_PER_KV_HEAD = 16;         // the same cap under grouped-query attention, per KV head (a unit does n_rep heads' math)
 
 enum { PH_QKV = 0, PH_ATT = 1, PH_O = 2, PH_GU = 3, PH_DOWN = 4, PH_HEAD = 5 };
 
@@ -31,32 +34,67 @@ DS_HD int range_lo(long long n, int c, int pG) { return c >= pG ? (int)n : (int)
 // the CTA whose share contains item u (inverse of share_lo)
 DS_HD int cta_of(long long u, long long U, int G) { return (int)(((u + 1) * G - 1) / U); }
 
-// U: units; spt: K stages per tile; tpm: tiles per matrix (ATT: units per head); G: CTAs that take part in the phase
-struct Phase { int kind, U, spt, tpm, nmat, mat0, N, G; float* acc; };
+// U: units; spt: K stages per tile; tpm: tiles per matrix (ATT: units per KV head); tq: tiles of the first matrix (QKV: q is wider than
+// k and v under grouped-query attention; every other phase: tpm); G: CTAs that take part in the phase.  Tiles are numbered matrix by
+// matrix, so the phase accumulator of tile t starts at column t * TILE ([HQ | HKV | HKV] for QKV, [I | I] for GU).
+struct Phase { int kind, U, spt, tpm, tq, nmat, mat0, N, G; float* acc; };
 
-// A: anything with the fields H, HQ, I, heads, past_len, vocab, lm_head, acc_qkv, acc_o, acc_gu, acc_d (the kernel's StepArgs)
+// CTAs that may share one KV head's attention units
+DS_HD int att_cap(int heads, int kv_heads) { return kv_heads < heads ? ATT_CTAS_PER_KV_HEAD : ATT_CTAS_PER_HEAD; }
+
+// KV heads and k / v width of a shape: its kv_heads / HKV fields, or heads / HQ (multi-head attention) for a shape type that has none
+template <class A, class = void> struct has_kv_heads : std::false_type {};
+template <class A> struct has_kv_heads<A, std::void_t<decltype(std::declval<const A&>().kv_heads)>> : std::true_type {};
+template <class A> DS_HD int kv_heads_of(const A& a) { if constexpr (has_kv_heads<A>::value) return a.kv_heads; else return a.heads; }
+template <class A> DS_HD int hkv_of(const A& a) { if constexpr (has_kv_heads<A>::value) return a.HKV; else return a.HQ; }
+
+// A: anything with the fields H, HQ, I, heads, past_len, vocab, lm_head, acc_qkv, acc_o, acc_gu, acc_d, and for grouped-query
+// attention kv_heads and HKV (the kernel's StepArgs)
 template <class A>
 DS_HD Phase phase_of(const A& a, int kind, int grid)
 {
-    Phase p; p.kind = kind; p.acc = nullptr; p.G = grid; p.spt = 0; p.tpm = 0; p.nmat = 0; p.mat0 = 0; p.N = 0; p.U = 0;
+    Phase p; p.kind = kind; p.acc = nullptr; p.G = grid; p.spt = 0; p.tpm = 0; p.tq = 0; p.nmat = 0; p.mat0 = 0; p.N = 0; p.U = 0;
     if (kind == PH_QKV)       { p.spt = a.H / TILE;  p.N = a.HQ; p.nmat = 3; p.mat0 = 0; p.acc = a.acc_qkv; }
     else if (kind == PH_O)    { p.spt = a.HQ / TILE; p.N = a.H;  p.nmat = 1; p.mat0 = 3; p.acc = a.acc_o; }
     else if (kind == PH_GU)   { p.spt = a.H / TILE;  p.N = a.I;  p.nmat = 2; p.mat0 = 4; p.acc = a.acc_gu; }
     else if (kind == PH_DOWN) { p.spt = a.I / TILE;  p.N = a.H;  p.nmat = 1; p.mat0 = 6; p.acc = a.acc_d; }
     if (kind == PH_ATT) {
         const int nch = (a.past_len + 15) >> 4;
-        p.tpm = nch > 0 ? nch : 1;                          // units per head (one empty unit when there is no history)
-        p.U = a.heads * p.tpm;
+        p.tpm = nch > 0 ? nch : 1;                          // units per KV head (one empty unit when there is no history)
+        p.tq = p.tpm;
+        const int kvh = kv_heads_of(a);
+        p.U = kvh * p.tpm;
         // at most ~7 CTAs per head: the O prologue combines one partial per CTA and head (two rounds of 4 loads); with few heads
-        // per GPU (tensor parallel) the rest of the grid sits this phase out -- its bytes are small then
-        if (a.heads * ATT_CTAS_PER_HEAD < grid) p.G = a.heads * ATT_CTAS_PER_HEAD;
+        // per GPU (tensor parallel) the rest of the grid sits this phase out -- its bytes are small then.  Grouped-query attention:
+        // one unit carries the math of n_rep query heads, so up to 16 CTAs share a KV head (70B: 128 of 132 CTAs instead of 56)
+        const int cap = att_cap(a.heads, kvh);
+        if (kvh * cap < grid) p.G = kvh * cap;
     } else if (kind == PH_HEAD) {
         p.U = a.lm_head ? (int)(((long long)a.vocab * a.H * 2 + W_BYTES - 1) / W_BYTES) : 0;
     } else {
         p.tpm = p.N / TILE;
-        p.U = p.nmat * p.tpm * p.spt;
+        p.tq = p.tpm;
+        if (kind == PH_QKV) { p.tq = a.HQ / TILE; p.tpm = hkv_of(a) / TILE; }          // q, then k and v (as wide as q unless GQA)
+        p.U = (p.tq + (p.nmat - 1) * p.tpm) * p.spt;
     }
     return p;
+}
+// matrix (0 .. nmat - 1) of tile t of a GEMV phase, its first tile, and its tile count
+DS_HD int mat_of_tile(const Phase& p, int t) { return t < p.tq ? 0 : 1 + (t - p.tq) / p.tpm; }
+DS_HD int mat_tile0(const Phase& p, int mi) { return mi == 0 ? 0 : p.tq + (mi - 1) * p.tpm; }
+DS_HD int mat_tiles(const Phase& p, int mi) { return mi == 0 ? p.tq : p.tpm; }
+
+// Grouped-query attention scratch (decode_step.cu), aliased onto the x staging area, which is dead between the end of the QKV GEMV
+// and the O prologue: per (KV-head segment, query head of the group) 4 pipeline partials + the new token's partial and q in fp16;
+// per segment the new k and v rows in fp32.  Partials start at offset 0.
+DS_HD int gqa_qh_off(int n_rep) { return 2 * n_rep * 5 * PART_LD * 4; }
+DS_HD int gqa_kn_off(int n_rep) { return gqa_qh_off(n_rep) + 2 * n_rep * TILE * 2; }
+DS_HD int gqa_scratch_bytes(int n_rep) { return n_rep > 1 ? gqa_kn_off(n_rep) + 2 * 2 * TILE * 4 : 0; }
+// bytes of the x staging area (quantised x planes + segment table), at least the grouped-query attention scratch
+DS_HD int stage_area_bytes(int xstages, int n_rep)
+{
+    const int b = xstages * (256 + 32), g = gqa_scratch_bytes(n_rep);
+    return b > g ? b : ((g + 31) & ~31);
 }
 
 // ---- host side (exl_decode_plan_create / exl_decode_step) ----
@@ -64,32 +102,37 @@ DS_HD Phase phase_of(const A& a, int kind, int grid)
 // head own nothing, so the slot they would have written keeps whatever an EARLIER launch left there (a longer context fills
 // every slot) -- and the O prologue combines slots [0, c_hi - c_lo] of the head.  exl_decode_step resets the table to the
 // neutral partial (m = -inf, l = 0, o = 0) before such a launch.  With one unit per head (tpm == 1) a head has one slot: no gap.
-// tests/decode_sched_check.cpp proves: a gap exists only where this predicate holds.
-struct AttDims { int H, HQ, I, heads, past_len, vocab; const void* lm_head; float *acc_qkv, *acc_o, *acc_gu, *acc_d; };
-static inline bool att_needs_reset(int heads, int past_len, int grid)
+// tests/decode_sched_check.cpp (tests/decode_sched_check_gqa.cpp for GQA) proves: a gap exists only where this predicate holds.
+// Grouped-query attention: the same holds per KV head (every query head of the group has the CTA range of its KV head).
+struct AttDims { int H, HQ, HKV, I, heads, kv_heads, past_len, vocab; const void* lm_head; float *acc_qkv, *acc_o, *acc_gu, *acc_d; };
+static inline bool att_needs_reset(int heads, int kv_heads, int past_len, int grid)
 {
     AttDims a = {};
-    a.heads = heads; a.past_len = past_len;
+    a.heads = heads; a.kv_heads = kv_heads; a.past_len = past_len;
     const Phase p = phase_of(a, PH_ATT, grid);
     return p.U < p.G && p.tpm >= 2;
 }
+static inline bool att_needs_reset(int heads, int past_len, int grid) { return att_needs_reset(heads, heads, past_len, grid); }
 
-// slots of att_part per head: one per CTA that can hold a piece of the head (+ 2: a range may start and end inside the head)
-static inline int att_slots_for(int grid, int heads)
+// slots of att_part per query head: one per CTA that can hold a piece of its KV head (+ 2: a range may start and end inside the head)
+static inline int att_slots_for(int grid, int heads, int kv_heads)
 {
-    return (grid < ATT_CTAS_PER_HEAD * heads ? grid / heads : ATT_CTAS_PER_HEAD) + 2;
+    const int cap = att_cap(heads, kv_heads);
+    return (grid < cap * kv_heads ? grid / kv_heads : cap) + 2;
 }
+static inline int att_slots_for(int grid, int heads) { return att_slots_for(grid, heads, heads); }
 static inline int spt_max_for(int H, int HQ, int I)
 {
     int m = (H > I ? H : I) / TILE;
     return HQ / TILE > m ? HQ / TILE : m;
 }
 constexpr size_t SMEM_STATIC_ALLOWANCE = 2048;   // static __shared__ of the kernel (mbarriers, schedule tables): ptxas reports 1664 B
-// shared memory apart from the ring: alignment slack, x staging (+ a second slot of H / 128 stages with act-order), residual
-// stream, attention scratch (partials, q / new k / new v in fp32, q in fp16), norm weights, static variables
-static inline size_t smem_fixed_bytes(int H, int HQ, int I, bool act)
+// shared memory apart from the ring: alignment slack, x staging (+ a second slot of H / 128 stages with act-order; grouped-query
+// attention scratch shares it), residual stream, attention scratch (partials, q / new k / new v in fp32, q in fp16), norm weights,
+// static variables
+static inline size_t smem_fixed_bytes(int H, int HQ, int I, bool act, int n_rep = 1)
 {
-    return 1024 + (size_t)(spt_max_for(H, HQ, I) + (act ? H / TILE : 0)) * (256 + 32) + (size_t)H * 2
+    return 1024 + (size_t)stage_area_bytes(spt_max_for(H, HQ, I) + (act ? H / TILE : 0), n_rep) + (size_t)H * 2
          + (size_t)(2 * 17 * PART_LD + 6 * TILE) * 4 + (size_t)2 * TILE * 2 /* fp16 q */ + (size_t)H * 2 /* wnorm */ + SMEM_STATIC_ALLOWANCE;
 }
 // dynamic shared memory to request for `depth` ring stages per pipeline

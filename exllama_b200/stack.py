@@ -112,8 +112,9 @@ class Layer:
 
 class DecodeStack:
     def __init__(self, shape: LlamaShape, groupsize=128, act_order=False, device="cuda:0", max_seq=2048,
-                 layers=None, seed=0, tp_rank=0, tp_size=1, tp_group=None, with_head=True):
+                 layers=None, seed=0, tp_rank=0, tp_size=1, tp_group=None, with_head=True, batch=1):
         self.shape, self.groupsize, self.act_order = shape, groupsize, act_order
+        self.batch = batch                     # sequences the KV caches hold (and the fused plan may step at once)
         self.device = torch.device(device)
         self.dev_index = self.device.index or 0
         self.max_seq = max_seq
@@ -170,8 +171,8 @@ class DecodeStack:
             emb = torch.cat((freqs, freqs), dim=-1)
             self.sin = emb.sin()[None, None, :, :].half().contiguous()
             self.cos = emb.cos()[None, None, :, :].half().contiguous()
-            # KV cache [bsz, kv_heads_local, max_seq, head_dim] per layer (model.py:557-585)
-            self.key_cache = [torch.zeros((1, self.local_kv_heads, max_seq, shape.head_dim), dtype=torch.float16, device=self.device)
+            # KV cache [batch, kv_heads_local, max_seq, head_dim] per layer (model.py:557-585)
+            self.key_cache = [torch.zeros((batch, self.local_kv_heads, max_seq, shape.head_dim), dtype=torch.float16, device=self.device)
                               for _ in range(self.n_layers)]
             self.value_cache = [torch.zeros_like(self.key_cache[0]) for _ in range(self.n_layers)]
             # scratch, as model.py:897-917
@@ -190,28 +191,31 @@ class DecodeStack:
                    for l in self.layers)
 
     # ---- decode: fused path, rows == 1 (model.py:528-547) ----------------------------------------------------
-    def decode_step(self, hidden, past_len):
-        """hidden: [1, 1, hidden] fp16 on the device, updated in place layer by layer; returns logits [1, vocab]."""
+    def decode_step(self, hidden, past_len, seq=0):
+        """hidden: [1, 1, hidden] fp16 on the device, updated in place layer by layer; returns logits [1, vocab].
+        seq: the cache sequence this token belongs to (its rows [0, past_len) are attended, its row past_len is written)."""
         s, none = self.shape, self.none
         bsz, q_len = 1, hidden.shape[1]
         hq = self.local_heads * s.head_dim
         hkv = self.local_kv_heads * s.head_dim
+        key_cache = [kc[seq:seq + 1] for kc in self.key_cache]
+        value_cache = [vc[seq:seq + 1] for vc in self.value_cache]
         for i, L in enumerate(self.layers):
             q = torch.empty((bsz, q_len, hq), dtype=torch.float16, device=self.device)
             k = torch.empty((bsz, q_len, hkv), dtype=torch.float16, device=self.device)
             v = torch.empty_like(k)
             ext.q4_attn(hidden, L.ln1, s.eps, q, k, v, L.q.q4, L.k.q4, L.v.q4, self.sin, self.cos, q_len, past_len,
-                        self.local_heads, self.local_kv_heads, s.head_dim, self.key_cache[i], self.value_cache[i], self.max_seq,
+                        self.local_heads, self.local_kv_heads, s.head_dim, key_cache[i], value_cache[i], self.max_seq,
                         none, none, none, none, none, none, none)
             if self.fused_decode_attn and q_len == 1 and s.head_dim == 128:
                 # one kernel over the KV cache instead of the five torch launches below (csrc/decode_attn.cu)
                 attn = torch.empty_like(q)
-                ext.decode_attn(q, self.key_cache[i], self.value_cache[i], attn, self.local_heads, self.local_kv_heads,
+                ext.decode_attn(q, key_cache[i], value_cache[i], attn, self.local_heads, self.local_kv_heads,
                                 s.head_dim, past_len + 1, self.max_seq)
             else:
                 q = q.view(bsz, q_len, self.local_heads, s.head_dim).transpose(1, 2)
-                keys = repeat_kv(self.key_cache[i].narrow(2, 0, past_len + q_len), self.n_rep)
-                values = repeat_kv(self.value_cache[i].narrow(2, 0, past_len + q_len), self.n_rep)
+                keys = repeat_kv(key_cache[i].narrow(2, 0, past_len + q_len), self.n_rep)
+                values = repeat_kv(value_cache[i].narrow(2, 0, past_len + q_len), self.n_rep)
                 attn = torch.matmul(q, keys.transpose(2, 3))
                 attn /= math.sqrt(s.head_dim)
                 attn = torch.nn.functional.softmax(attn, dim=-1, dtype=torch.float16)
@@ -237,7 +241,7 @@ class DecodeStack:
         self.dplan = capi.DecodePlan(hs, [L.ln1 for L in self.layers], [L.ln2 for L in self.layers], self.key_cache, self.value_cache,
                                     self.sin, self.cos, self.local_heads, self.shape.head_dim, self.max_seq, self.shape.eps,
                                     final_norm=self.norm if head is not None else None, lm_head=head,
-                                    tp_rank=self.tp_rank, tp_world=self.tp_size, num_kv_heads=self.local_kv_heads)
+                                    tp_rank=self.tp_rank, tp_world=self.tp_size, num_kv_heads=self.local_kv_heads, max_batch=self.batch)
         if self.tp_size > 1:
             # exchange the cudaIpc handles of the regions the peers reduce into (acc_o, acc_d, cross-barrier counter)
             import torch.distributed as dist
@@ -245,8 +249,8 @@ class DecodeStack:
             dist.all_gather_object(handles, self.dplan.ipc_export(), group=self.tp_group)
             self.dplan.ipc_import(handles)
             dist.barrier(self.tp_group)
-        self._plan_xout = torch.empty(self.shape.hidden, dtype=torch.float16, device=self.device)
-        self._plan_logits = torch.empty((1, self.shape.vocab), dtype=torch.float32, device=self.device) if head is not None else None
+        self._plan_xout = torch.empty((self.batch, self.shape.hidden) if self.batch > 1 else self.shape.hidden, dtype=torch.float16, device=self.device)
+        self._plan_logits = torch.empty((self.batch, self.shape.vocab), dtype=torch.float32, device=self.device) if head is not None else None
         return self.dplan
 
     def decode_step_fused(self, hidden, past_len):
@@ -254,6 +258,17 @@ class DecodeStack:
         the final pre-norm hidden state is left in self._plan_xout."""
         self.dplan.step(hidden, past_len, x_out=self._plan_xout, logits=self._plan_logits)
         return self._plan_logits if self._plan_logits is not None else self._plan_xout
+
+    def decode_step_fused_batch(self, hidden, past_lens):
+        """One token for each of bsz = len(past_lens) <= batch sequences in one launch: hidden [bsz, 1, hidden] fp16 (read only),
+        sequence b at context past_lens[b] of cache sequence b.  Returns logits [bsz, vocab] fp32 (or the final hidden states
+        without a head); the final pre-norm hidden states are left in self._plan_xout[:bsz]."""
+        bsz = len(past_lens)
+        assert hidden.shape[0] == bsz and hidden.is_contiguous(), (hidden.shape, bsz)
+        xo = self._plan_xout.view(-1, self.shape.hidden)
+        lg = self._plan_logits
+        self.dplan.step_batch(hidden, past_lens, x_out=xo, logits=lg)
+        return lg[:bsz] if lg is not None else xo[:bsz]
 
     def _o_input(self, attn_local):
         """o_proj input of this rank: its own heads' output, or -- act-order + TP -- the rows of its group range out of the

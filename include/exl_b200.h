@@ -180,7 +180,8 @@ typedef struct exl_decode_desc {
     const exl_q4_matrix* const* mats;   /* [n_layers * 7]: q, k, v, o, gate, up, down of each layer (handles from exl_make_q4) */
     const void* const* ln1;              /* [n_layers] input_layernorm weight, half [hidden] */
     const void* const* ln2;              /* [n_layers] post_attention_layernorm weight */
-    void* const* key_cache;              /* [n_layers] half [num_kv_heads, max_seq_len, head_dim] (model.py:557-585) */
+    void* const* key_cache;              /* [n_layers] half [max_batch, num_kv_heads, max_seq_len, head_dim] (model.py:557-585; max_batch 1
+                                            unless the plan comes from exl_decode_plan_create_batch) */
     void* const* value_cache;
     const void* sin; const void* cos;    /* half [max_seq_len, head_dim] (model.py:864-877) */
     const void* final_norm;              /* half [hidden] or NULL */
@@ -196,6 +197,12 @@ typedef struct exl_decode_desc {
 } exl_decode_desc;
 
 int exl_decode_plan_create(const exl_decode_desc* desc, exl_decode_plan** out_plan);
+/* Batched decode: a plan whose steps carry 1 .. max_batch (<= 4) sequences, each at its own context, through the same weight
+   stream.  The caches hold max_batch sequences ([max_batch, num_kv_heads, max_seq_len, head_dim], ExLlamaCache(batch_size=...),
+   model.py:559-577).  Not with act-order matrices or tensor parallelism; max_batch must fit the model (shared memory, and
+   max_batch * num_heads -- num_kv_heads under grouped-query attention -- <= SMs); otherwise EXL_ERR_ARG naming what fits.
+   exl_decode_plan_create(d, out) is exl_decode_plan_create_batch(d, 1, out). */
+int exl_decode_plan_create_batch(const exl_decode_desc* desc, int max_batch, exl_decode_plan** out_plan);
 int exl_decode_plan_destroy(exl_decode_plan* plan);
 /* Tensor parallel set-up: export this rank's 64-byte cudaIpc handle, exchange (e.g. through torch.distributed), import all of
    them (world x 64 bytes in rank order) on every rank before the first exl_decode_step; every rank must then call
@@ -212,6 +219,12 @@ int exl_decode_plan_trace(exl_decode_plan* plan, unsigned long long* out_host, i
    writes at past_len.  x_out (optional) receives the final hidden state before the final norm, logits float [vocab]
    (required iff the plan has an lm_head).  CUDA-graph capturable; successive calls need no host synchronisation. */
 int exl_decode_step(exl_decode_plan* plan, const void* x_in, int past_len, void* x_out, void* logits, void* stream);
+/* One token for each of bsz (1 .. the plan's max_batch) sequences: x_in half [bsz][hidden]; sequence b attends over rows
+   [0, past_len_host[b]) of cache sequence b and writes its new row there (sequences >= bsz are not touched); x_out half
+   [bsz][hidden], logits float [bsz][vocab].  The past_len values are read on the host (baked into a CUDA-graph capture).
+   exl_decode_step is this call with bsz 1 on sequence 0. */
+int exl_decode_step_batch(exl_decode_plan* plan, const void* x_in, int bsz, const int* past_len_host, void* x_out, void* logits,
+                          void* stream);
 
 /* --- tensor-parallel variants (new functionality; the reference has no tensor parallelism, SURVEY.md 8e) ----- */
 

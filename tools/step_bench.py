@@ -1,7 +1,9 @@
 #!/usr/bin/env python
 """Time the whole-token persistent kernel (csrc/decode_step.cu) next to the per-op path on the synthetic stack.
 Accepts the SHAPES names and the grouped-query attention ones (GQA_SHAPES, e.g. 70b); the line records the GPU and its power limit.
-    python tools/step_bench.py [--model 7b] [--ctx 1920] [--seq 2048] [--groupsize 128] [--act-order] [--layers N] [--reps 20]"""
+--batch N times one launch for N sequences, all at --ctx (aggregate tok/s = N tokens per launch; bytes = weights + head + N x K/V);
+the per-op arm then times sequence 0 alone.
+    python tools/step_bench.py [--model 7b] [--ctx 1920] [--seq 2048] [--groupsize 128] [--act-order] [--layers N] [--reps 20] [--batch N]"""
 import argparse, json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -12,12 +14,12 @@ from exllama_b200.stack import GQA_SHAPES, SHAPES, DecodeStack, _Arena
 MIN_WINDOW_S = 1.2          # timed window per arm
 
 
-def device_bytes(shape, layers, groupsize, seq):
+def device_bytes(shape, layers, groupsize, seq, batch=1):
     """What DecodeStack allocates on the device, roughly: q4 tensors, lm_head, KV caches, prepare_buffers scratch."""
     h, hq, hkv, i = shape.hidden, shape.heads * shape.head_dim, shape.kv_heads * shape.head_dim, shape.inter
     per_layer = (_Arena.q4_bytes(h, hq, groupsize) + 2 * _Arena.q4_bytes(h, hkv, groupsize) + _Arena.q4_bytes(hq, h, groupsize) +
                  2 * _Arena.q4_bytes(h, i, groupsize) + _Arena.q4_bytes(i, h, groupsize))
-    kv = 2 * layers * seq * hkv * 2
+    kv = 2 * layers * seq * hkv * 2 * batch
     scratch = seq * i * 2 + h * i * 2 + (1 << 20)
     return per_layer * layers + shape.vocab * h * 2 + kv + scratch
 
@@ -29,21 +31,25 @@ def main():
     ap.add_argument("--act-order", action="store_true", help="act-order (g_idx) matrices")
     ap.add_argument("--reps", type=int, default=20, help="minimum timed steps per arm (more if the window would be under 1.2 s)")
     ap.add_argument("--no-per-op", action="store_true")
+    ap.add_argument("--batch", type=int, default=1, help="sequences per launch (1..4, as far as the model fits)")
     args = ap.parse_args()
     shapes = {**SHAPES, **GQA_SHAPES}
     if args.model not in shapes:
         sys.exit(f"unknown model {args.model!r}; one of {sorted(shapes)}")
     shape = shapes[args.model]
     layers = args.layers if args.layers is not None else shape.layers
-    need = device_bytes(shape, layers, args.groupsize, args.seq)
+    need = device_bytes(shape, layers, args.groupsize, args.seq, args.batch)
     free, total = torch.cuda.mem_get_info()
     if need > free * 0.95:
         sys.exit(f"{args.model}: about {need / 1e9:.1f} GB needed, {free / 1e9:.1f} GB of {total / 1e9:.1f} GB free on this GPU; use --layers")
-    st = DecodeStack(shape, groupsize=args.groupsize, act_order=args.act_order, device="cuda:0", max_seq=args.seq, layers=args.layers)
+    st = DecodeStack(shape, groupsize=args.groupsize, act_order=args.act_order, device="cuda:0", max_seq=args.seq, layers=args.layers,
+                     batch=args.batch)
     for kc, vc in zip(st.key_cache, st.value_cache):
         kc.normal_(0, 0.5); vc.normal_(0, 0.5)
     st.make_plan()
-    x = (torch.randn((1, 1, shape.hidden), device="cuda") * 0.5).half()
+    nb = args.batch
+    xb = (torch.randn((nb, 1, shape.hidden), device="cuda") * 0.5).half()
+    x = xb[:1]
 
     def timed(fn):
         for _ in range(3): fn()
@@ -65,12 +71,16 @@ def main():
     res = {"tool": "tools/step_bench.py", "model": args.model, "ctx": args.ctx, "seq": args.seq, "groupsize": args.groupsize,
            "act_order": args.act_order, "layers": len(st.layers), "heads": shape.heads, "kv_heads": shape.kv_heads,
            "gpu": torch.cuda.get_device_name(0), "power_limit_w": power_limit(torch.cuda.current_device()), "plan": st.dplan.info()}
-    ms, reps = timed(lambda: st.decode_step_fused(x, args.ctx))
+    if nb > 1:
+        res["batch"] = nb
+        ms, reps = timed(lambda: st.decode_step_fused_batch(xb, [args.ctx] * nb))
+    else:
+        ms, reps = timed(lambda: st.decode_step_fused(x, args.ctx))
     wbytes = st.q4_weight_bytes_per_token() + shape.vocab * shape.hidden * 2
-    kv = 2 * len(st.layers) * args.ctx * shape.kv_heads * shape.head_dim * 2          # K and V rows read once per KV head
-    res["fused_ms"] = round(ms, 4); res["fused_tok_s"] = round(1000 / ms, 1); res["fused_reps"] = reps; res["bytes"] = wbytes + kv
+    kv = nb * 2 * len(st.layers) * args.ctx * shape.kv_heads * shape.head_dim * 2     # K and V rows read once per KV head and sequence
+    res["fused_ms"] = round(ms, 4); res["fused_tok_s"] = round(nb * 1000 / ms, 1); res["fused_reps"] = reps; res["bytes"] = wbytes + kv
     res["kv_bytes"] = kv; res["fused_GBps"] = round((wbytes + kv) / ms / 1e6, 1)
-    lf = st._plan_logits.clone()
+    lf = st._plan_logits[:1].clone()
     if not args.no_per_op:
         h = x.clone()
         def per_op():

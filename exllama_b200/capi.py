@@ -53,6 +53,7 @@ SIGNATURES = {
     "exl_q4_matmul_host": (i32, [vp, i32, vp, vp, vp, vp, vp]),
     "exl_decode_plan_create": (i32, [vp, C.POINTER(vp)]),
     "exl_decode_plan_create_batch": (i32, [vp, i32, C.POINTER(vp)]),
+    "exl_decode_plan_create_lora": (i32, [vp, i32, vp, C.POINTER(vp)]),
     "exl_decode_plan_destroy": (i32, [vp]),
     "exl_decode_plan_info": (i32, [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]),
     "exl_decode_step": (i32, [vp, vp, i32, vp, vp, vp]),
@@ -226,16 +227,22 @@ class _DecodeDesc(C.Structure):
                 ("tp_rank", i32), ("tp_world", i32), ("num_kv_heads", i32)]
 
 
+class _DecodeLora(C.Structure):
+    """struct exl_decode_lora (include/exl_b200.h)"""
+    _fields_ = [("n_layers", i32), ("a", C.POINTER(vp)), ("b", C.POINTER(vp)), ("rank", C.POINTER(i32))]
+
+
 class DecodePlan:
     """exl_decode_plan: the whole decode token as one persistent kernel (csrc/decode_step.cu).
 
     handles: per layer the 7 Q4 handles (q, k, v, o, gate, up, down) as integers / c_void_p; every tensor passed here is
     borrowed and must outlive the plan.  num_kv_heads (grouped-query attention, default num_heads): k_proj / v_proj are
     num_kv_heads * head_dim wide; single GPU only.  max_batch (1..4): sequences a step_batch() may carry; the caches are then
-    [max_batch, num_kv_heads, max_seq_len, head_dim]; single GPU, no act-order."""
+    [max_batch, num_kv_heads, max_seq_len, head_dim]; single GPU, no act-order.  lora: per layer None or a 7-tuple (q, k, v, o,
+    gate, up, down) of None or (A half [in, r], B half [r, out] already scaled by alpha / r), lora.py's layout; single GPU."""
 
     def __init__(self, handles, ln1, ln2, key_cache, value_cache, sin, cos, num_heads, head_dim, max_seq_len, eps,
-                 final_norm=None, lm_head=None, tp_rank=0, tp_world=1, num_kv_heads=None, max_batch=1):
+                 final_norm=None, lm_head=None, tp_rank=0, tp_world=1, num_kv_heads=None, max_batch=1, lora=None):
         n = len(handles)
         self._keep = (ln1, ln2, key_cache, value_cache, sin, cos, final_norm, lm_head)
         flat = []
@@ -261,7 +268,28 @@ class DecodePlan:
         self.tp_world = tp_world
         self.max_batch = max_batch
         self.handle = vp()
-        check(lib().exl_decode_plan_create_batch(C.byref(d), max_batch, C.byref(self.handle)))
+        if lora is None:
+            check(lib().exl_decode_plan_create_batch(C.byref(d), max_batch, C.byref(self.handle)))
+            return
+        assert len(lora) == n, (len(lora), n)
+        pa, pb, rk, keep = [], [], [], []
+        for layer in lora:
+            mats = layer if layer is not None else (None,) * 7
+            assert len(mats) == 7
+            for ab in mats:
+                if ab is None:
+                    pa.append(None); pb.append(None); rk.append(0)
+                else:
+                    A, B = ab
+                    keep += [A, B]
+                    pa.append(A.data_ptr()); pb.append(B.data_ptr()); rk.append(A.shape[1])
+        self._lora_keep = keep
+        self._lora_arrays = ((vp * (7 * n))(*pa), (vp * (7 * n))(*pb), (i32 * (7 * n))(*rk))
+        lo = _DecodeLora()
+        lo.n_layers = n
+        lo.a, lo.b = (C.cast(x, C.POINTER(vp)) for x in self._lora_arrays[:2])
+        lo.rank = C.cast(self._lora_arrays[2], C.POINTER(i32))
+        check(lib().exl_decode_plan_create_lora(C.byref(d), max_batch, C.byref(lo), C.byref(self.handle)))
 
     def ipc_export(self) -> bytes:
         buf = (C.c_ubyte * 64)()

@@ -76,7 +76,7 @@ int exl_own_scratch(ExlDevice* ds, int role, int64_t numel, half** out)
 extern "C" {
 
 const char* exl_last_error(void) { return t_err; }
-int exl_version(void) { return 102; }             // 101: exl_decode_desc.num_kv_heads; 102: batched decode plans and steps
+int exl_version(void) { return 103; }             // 101: exl_decode_desc.num_kv_heads; 102: batched decode plans and steps; 103: LoRA plans
 int64_t exl_launch_count(void) { return g_launches.load(); }
 const char* exl_last_q4_path(void) { return g_last_q4_path; }
 

@@ -36,6 +36,9 @@
 //    IMMAs serve every sequence.  Sequence b's two x planes ride in B columns 2b, 2b + 1, so lane t of an MMA quad ends up holding
 //    sequence t's result; ATT runs over virtual heads (sequence, head) with each sequence's own context and cache rows; the head
 //    dots every lm_head stage with every sequence.  Only the K/V bytes grow with the batch.
+//  * LoRA adapters (template flag LORA, one GPU): an adapted phase gets an LA step after its prologue (t = x . A over (matrix, K stage)
+//    units, fp32 red.add into L2, one grid barrier), and the CTA owning K stage 0 of an adapted tile adds fp16(t) . B to it after the
+//    GEMV (decode_step_sched.h: lora_*).
 //
 // Restrictions (checked on the host; anything else uses the per-op kernels): head_dim 128, heads % kv_heads == 0 (grouped-query
 // attention only without tensor parallelism), groupsize 32 * 2^n (or one group), widths multiples of 128, act-order only without
@@ -73,6 +76,9 @@ struct alignas(64) LayerDesc
     const half* ln1; const half* ln2;
     half* kc; half* vc;                // [max_batch, kv_heads, max_seq, 128]
 };
+
+// one projection's LoRA adapter: A [K, rank] and B [rank, N] fp16 row-major (B already scaled by alpha / rank); rank 0 = none
+struct LoraMat { const half* a; const half* b; int rank; int t_off; };
 
 struct StepArgs
 {
@@ -113,6 +119,9 @@ struct StepArgs
     int bsz;                           // sequences of this launch, 1 .. max_batch of the plan
     int xst;                           // compacted x staging stages per sequence (decode_step_sched.h: batch_xstages)
     int past_lens[MAX_BATCH];          // context of each sequence
+    // LoRA adapters (LORA kernels only; the others read none of these): [n_layers * 7] matrices' adapters, and the fp32 t = x . A
+    // accumulators in L2 (matrix of rank r at t_off: [max_batch][r]), zeroed at launch start
+    const LoraMat* lora; float* lora_t; int lora_t4;              // lora_t4: floats of lora_t / 4
 };
 
 // ------------------------------------------------------------------------------------------------------------ helpers
@@ -288,8 +297,9 @@ __device__ __forceinline__ void grid_barrier(unsigned long long* ctr, unsigned l
 // ACT: act-order matrices present; TP: tensor parallel; GQA: grouped-query attention (kv_heads < heads, single GPU); BATCH: a plan
 // for more than one sequence (neither ACT nor TP).  Compile-time so that the common kernel (none of them) carries none of their
 // address arithmetic, branches or code (the runtime-flag version of the same source was 10 % slower on the plain 7B step; a runtime
-// n_rep branch around the attention phase made ptxas spill in it).  Without BATCH, nb below is the constant 1.
-template <bool ACT, bool TP, bool GQA, bool BATCH>
+// n_rep branch around the attention phase made ptxas spill in it).  Without BATCH, nb below is the constant 1.  LORA: a plan with
+// LoRA adapters (single GPU; any of the others but TP): the LA steps and B terms below.
+template <bool ACT, bool TP, bool GQA, bool BATCH, bool LORA = false>
 __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid_constant__ StepArgs a)
 {
     extern __shared__ __align__(128) unsigned char smem[];
@@ -456,6 +466,9 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
     // ---- launch start: all accumulators and the logits to zero (robust against an aborted previous launch), then barrier ----
     zero_share(a.acc_qkv, ZR_QKV); zero_share(a.acc_o, ZR_H); zero_share(a.acc_gu, ZR_GU); zero_share(a.acc_d, ZR_H);
     if (a.logits) zero_share(a.logits, ZR_LOGITS);
+    if constexpr (LORA)
+        for (int i = share_lo(a.lora_t4, cta, G) + tid; i < share_lo(a.lora_t4, cta + 1, G); i += DS_CONSUMERS)
+            reinterpret_cast<float4*>(a.lora_t)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int i = tid; i < nb * a.H / 8; i += DS_CONSUMERS)
         reinterpret_cast<uint4*>(xres)[i] = __ldg(reinterpret_cast<const uint4*>(a.x_in) + i);
 
@@ -794,6 +807,85 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         else gemv_t(std::integral_constant<int, 1>{}, p, u0, u1);
     };
 
+    // ---- LoRA (LORA kernels only).  LA step of an adapted phase: t[b][j] += x_b[k] * A[k, j] over this CTA's (matrix, K stage) units
+    // (decode_step_sched.h), x_b being sequence b's phase input in the checkpoint's input order -- never gathered through an x_map: the
+    // rows of A are in that order -- as make_get(b)(k8) yields it, 8 fp16 values at a time.  fp32 products and sums, fp32 red.add into
+    // t in L2.  Returns whether the phase is adapted: the caller then runs a grid barrier, after which t is complete.
+    auto lora_a = [&](int l, const Phase& p, auto make_get) -> bool {
+        const LoraMat* lm = a.lora + l * 7 + p.mat0;
+        int js[3] = {0, 0, 0}, na = 0;
+        for (int m = 0; m < p.nmat; m++) if (lm[m].rank > 0) js[na++] = m;
+        if (na == 0) return false;
+        float* lx = parts;                                   // [nb][128] x of the unit's K stage (the attention partials are free here)
+        float* lt = parts + MAX_BATCH * TILE;                // [nb][rank] this unit's share of t
+        const int U = lora_units(na, p.spt);
+        for (int v = share_lo(U, cta, G); v < share_lo(U, cta + 1, G); v++) {
+            const int s = v % p.spt;
+            const LoraMat m = lm[js[v / p.spt]];
+            for (int i = tid; i < nb * 16; i += DS_CONSUMERS) {
+                const int b = i >> 4, r = i & 15;
+                const uint4 hv = make_get(b)(s * 16 + r);
+                const half2* h = reinterpret_cast<const half2*>(&hv);
+                #pragma unroll
+                for (int q = 0; q < 4; q++) { const float2 f = __half22float2(h[q]); lx[b * TILE + r * 8 + 2 * q] = f.x; lx[b * TILE + r * 8 + 2 * q + 1] = f.y; }
+            }
+            for (int i = tid; i < nb * m.rank; i += DS_CONSUMERS) lt[i] = 0.f;
+            consumer_sync();
+            const int nkg = DS_CONSUMERS / m.rank;           // k groups: thread (kg, j) takes rows kg, kg + nkg, ... of column j
+            if (tid < nkg * m.rank) {
+                const int j = tid % m.rank, kg = tid / m.rank;
+                const half* ap = m.a + (size_t)s * TILE * m.rank + j;
+                float acc[MAX_BATCH] = {0.f, 0.f, 0.f, 0.f};
+                for (int k = kg; k < TILE; k += nkg) {
+                    const float w = __half2float(__ldg(ap + (size_t)k * m.rank));
+                    #pragma unroll
+                    for (int b = 0; b < MAX_BATCH; b++) if (b < nb) acc[b] = fmaf(lx[b * TILE + k], w, acc[b]);
+                }
+                #pragma unroll
+                for (int b = 0; b < MAX_BATCH; b++) if (b < nb) atomicAdd(lt + b * m.rank + j, acc[b]);
+            }
+            consumer_sync();
+            for (int i = tid; i < nb * m.rank; i += DS_CONSUMERS) atomicAdd(a.lora_t + m.t_off + i, lt[i]);     // t: [b][rank]
+            consumer_sync();                                  // lx / lt are reused by the next unit
+        }
+        return true;
+    };
+    // B term, after the GEMV of the phase: every tile of an adapted matrix whose K stage 0 this CTA owns gets
+    // acc[b][tile columns] += sum_j fp16(t[b][j]) * B[j, columns], in fp32 (t rounded to fp16 where the reference rounds lora_temp)
+    auto lora_b = [&](int l, const Phase& p, int u0, int u1) {
+        if (u1 <= u0) return;
+        const LoraMat* lm = a.lora + l * 7 + p.mat0;
+        const size_t acc_ld = (size_t)(p.tq + (p.nmat - 1) * p.tpm) * TILE;      // accumulator row of a sequence
+        const int c = tid & (TILE - 1), jq = tid >> 7;                          // column of the tile, quarter of the rank
+        for (int tile = lora_b_first(p, u0); tile * p.spt < u1; tile++) {
+            const int mi = mat_of_tile(p, tile);
+            const LoraMat m = lm[mi];
+            if (m.rank == 0) continue;
+            const int n = mat_tiles(p, mi) * TILE;
+            const half* bp = m.b + (size_t)(tile - mat_tile0(p, mi)) * TILE + c;
+            for (int b = 0; b < nb; b++) {
+                const float* tp = a.lora_t + m.t_off + b * m.rank;
+                float sum = 0.f;
+                for (int j = jq; j < m.rank; j += DS_CONSUMERS / TILE)
+                    sum = fmaf(__half2float(__float2half_rn(__ldcg(tp + j))), __half2float(__ldg(bp + (size_t)j * n)), sum);
+                atomicAdd(p.acc + b * acc_ld + (size_t)tile * TILE + c, sum);
+            }
+        }
+    };
+    // LA inputs: sequence b's residual stream normalised with its row factor and the norm weights nw (as norm_get, un-gathered)
+    auto lora_norm_get = [&](const half* nw, int b, float rmf) {
+        const uint4* xr = reinterpret_cast<const uint4*>(xres + (size_t)b * a.H);
+        return [=](int k8) -> uint4 {
+            uint4 xv = xr[k8];
+            const uint4 wv = __ldg(reinterpret_cast<const uint4*>(nw) + k8);
+            const half2 rm2 = __float2half2_rn(rmf);
+            half2* h = reinterpret_cast<half2*>(&xv); const half2* w2 = reinterpret_cast<const half2*>(&wv);
+            #pragma unroll
+            for (int i = 0; i < 4; i++) h[i] = __hmul2(__hmul2(h[i], rm2), w2[i]);
+            return xv;
+        };
+    };
+
     // tensor parallel: after the local barrier, this CTA's share of the rank's reduced partial goes into every peer's slot [tp_rank]
     // as {value, epoch} pairs (8-byte stores; two pairs per 16-byte store are fine: each pair is validated on its own)
     auto push_partial = [&](const float* acc, uint2* const* push, unsigned epoch, int l, int ev) {
@@ -1000,8 +1092,12 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             else stage_phase(p, u0, u1, [&](int m) { return norm_get_map(L->ln1, rm, L->xmap[m]); });
             }
             consumer_sync();
+            if constexpr (LORA) {
+                if (lora_a(l, p, [&](int b) { return lora_norm_get(L->ln1, b, BATCH ? rm_of(b) : rm); })) grid_barrier(a.bar, target, (unsigned)G, tid);
+            }
             stamp(l, 1);
             gemv(p, u0, u1);
+            if constexpr (LORA) lora_b(l, p, u0, u1);
             jbase += u1 - u0;
             stamp(l, 2);
         }
@@ -1240,8 +1336,16 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
                 });
             }
             consumer_sync();
+            if constexpr (LORA) {
+                // un-gathered o_proj input: act-order has it in attn_vec already, otherwise the softmax-combine yields it
+                bool adapted;
+                if constexpr (ACT) adapted = lora_a(l, p, [&](int) { return [&](int k8) -> uint4 { return __ldcg(reinterpret_cast<const uint4*>(a.attn_vec) + k8); }; });
+                else adapted = lora_a(l, p, [&](int b) { return [&, b](int k8) -> uint4 { return combine8(b * a.heads + (k8 >> 4), (k8 & 15) * 8); }; });
+                if (adapted) grid_barrier(a.bar, target, (unsigned)G, tid);
+            }
             stamp(l, 6);
             gemv(p, u0, u1);
+            if constexpr (LORA) lora_b(l, p, u0, u1);
             jbase += u1 - u0;
             preload_norm(L->ln2, phase_of(a, PH_GU, G, nb));
             stamp(l, 7);
@@ -1263,8 +1367,12 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             else stage_phase(p, u0, u1, [&](int m) { return norm_get_map(L->ln2, rm, L->xmap[m]); });
             }
             consumer_sync();
+            if constexpr (LORA) {
+                if (lora_a(l, p, [&](int b) { return lora_norm_get(L->ln2, b, BATCH ? rm_of(b) : rm); })) grid_barrier(a.bar, target, (unsigned)G, tid);
+            }
             stamp(l, 9);
             gemv(p, u0, u1);
+            if constexpr (LORA) lora_b(l, p, u0, u1);
             jbase += u1 - u0;
             stamp(l, 10);
         }
@@ -1305,8 +1413,22 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
                 });
             }
             consumer_sync();
+            if constexpr (LORA) {
+                // silu(gate) * up of sequence b, un-gathered
+                auto act_get = [&](int b) {
+                    return [&, b](int k8) -> uint4 {
+                        const float* gu = a.acc_gu + (size_t)b * 2 * a.I;
+                        uint4 r; half* hh = reinterpret_cast<half*>(&r);
+                        #pragma unroll
+                        for (int i = 0; i < 8; i++) hh[i] = __hmul(silu_h(__float2half_rn(__ldcg(gu + k8 * 8 + i))), __float2half_rn(__ldcg(gu + a.I + k8 * 8 + i)));
+                        return r;
+                    };
+                };
+                if (lora_a(l, p, act_get)) grid_barrier(a.bar, target, (unsigned)G, tid);
+            }
             stamp(l, 12);
             gemv(p, u0, u1);
+            if constexpr (LORA) lora_b(l, p, u0, u1);
             jbase += u1 - u0;
             if (l + 1 < a.n_layers) preload_norm(a.layers[l + 1].ln1, phase_of(a, PH_QKV, G, nb));
             stamp(l, 13);
@@ -1454,10 +1576,17 @@ struct exl_decode_plan
     size_t smem = 0;
     int grid = 0;
     int max_batch = 1;                          // sequences a step may carry (> 1: the BATCH kernels)
+    LoraMat* d_lora = nullptr;                  // LoRA plans (the LORA kernels): [n_layers * 7] adapters
+    long long lora_barriers = 0;                // their extra grid barriers per step
 };
 
-static const void* step_kernel_for(bool act, bool tp, bool gqa, bool batch)
+static const void* step_kernel_for(bool act, bool tp, bool gqa, bool batch, bool lora = false)
 {
+    if (lora) {                                                                     // never under TP; a batch without act-order
+        if (batch) return gqa ? (const void*)decode_step_kernel<false, false, true, true, true> : (const void*)decode_step_kernel<false, false, false, true, true>;
+        if (gqa) return act ? (const void*)decode_step_kernel<true, false, true, false, true> : (const void*)decode_step_kernel<false, false, true, false, true>;
+        return act ? (const void*)decode_step_kernel<true, false, false, false, true> : (const void*)decode_step_kernel<false, false, false, false, true>;
+    }
     if (batch) return gqa ? (const void*)decode_step_kernel<false, false, true, true> : (const void*)decode_step_kernel<false, false, false, true>;   // neither act-order nor TP
     if (gqa) return act ? (const void*)decode_step_kernel<true, false, true, false> : (const void*)decode_step_kernel<false, false, true, false>;     // no GQA under TP
     if (act) return tp ? (const void*)decode_step_kernel<true, true, false, false> : (const void*)decode_step_kernel<true, false, false, false>;
@@ -1471,6 +1600,7 @@ static int plan_fail(exl_decode_plan* p, int rc)
         if (p->d_layers) cudaFree(p->d_layers);
         if (p->d_scratch) cudaFree(p->d_scratch);
         if (p->d_shared) cudaFree(p->d_shared);
+        if (p->d_lora) cudaFree(p->d_lora);
         delete p;
     }
     return rc;
@@ -1481,7 +1611,41 @@ extern "C" int exl_decode_plan_create(const exl_decode_desc* d, exl_decode_plan*
     return exl_decode_plan_create_batch(d, 1, out);
 }
 
+static int plan_create(const exl_decode_desc* d, int max_batch, const exl_decode_lora* lora, exl_decode_plan** out);
+
 extern "C" int exl_decode_plan_create_batch(const exl_decode_desc* d, int max_batch, exl_decode_plan** out)
+{
+    return plan_create(d, max_batch, nullptr, out);
+}
+
+extern "C" int exl_decode_plan_create_lora(const exl_decode_desc* d, int max_batch, const exl_decode_lora* lora, exl_decode_plan** out)
+{
+    if (!d || !out) return exl_set_err(EXL_ERR_ARG, "decode_plan: NULL argument");
+    if (!lora) return plan_create(d, max_batch, nullptr, out);
+    *out = nullptr;
+    if (lora->n_layers != d->n_layers)
+        return exl_set_err(EXL_ERR_ARG, "decode_plan_lora: the adapter has %d layers, the model %d: give one entry per layer (rank 0 where there is none)", lora->n_layers, d->n_layers);
+    if (d->n_layers < 1 || d->n_layers > MAX_LAYERS || !lora->rank) return exl_set_err(EXL_ERR_ARG, "decode_plan_lora: bad layer count %d or NULL rank array", d->n_layers);
+    bool any = false;
+    for (int i = 0; i < 7 * d->n_layers; i++) any = any || lora->rank[i] != 0;
+    if (!any) return plan_create(d, max_batch, nullptr, out);                  // no adapter: exactly the plan without one
+    if (d->tp_world > 1)
+        return exl_set_err(EXL_ERR_ARG, "decode_plan_lora: LoRA adapters under tensor parallelism are not supported by the fused step: use the per-op path");
+    if (!lora->a || !lora->b) return exl_set_err(EXL_ERR_ARG, "decode_plan_lora: NULL A or B array: use the per-op path for this adapter");
+    for (int i = 0; i < 7 * d->n_layers; i++) {
+        const int r = lora->rank[i], l = i / 7, m = i % 7;
+        if (r == 0) continue;
+        if (!lora_rank_ok(r))
+            return exl_set_err(EXL_ERR_ARG, "decode_plan_lora: layer %d matrix %d has rank %d; the fused step takes multiples of 8 up to %d: use the per-op path", l, m, r, LORA_MAX_RANK);
+        if (!lora->a[i] || !lora->b[i])
+            return exl_set_err(EXL_ERR_ARG, "decode_plan_lora: layer %d matrix %d has rank %d but a NULL A or B: use the per-op path", l, m, r);
+        if (((uintptr_t)lora->a[i] | (uintptr_t)lora->b[i]) & 15)
+            return exl_set_err(EXL_ERR_ARG, "decode_plan_lora: layer %d matrix %d: A and B must be 16-byte aligned for the fused step: use the per-op path", l, m);
+    }
+    return plan_create(d, max_batch, lora, out);
+}
+
+static int plan_create(const exl_decode_desc* d, int max_batch, const exl_decode_lora* lora, exl_decode_plan** out)
 {
     if (!d || !out) return exl_set_err(EXL_ERR_ARG, "decode_plan: NULL argument");
     *out = nullptr;
@@ -1563,7 +1727,7 @@ extern "C" int exl_decode_plan_create_batch(const exl_decode_desc* d, int max_ba
     a.depth = depth;
     p->smem = smem_dynamic_bytes(fixed, depth);
     if ((size_t)H * 2 > (size_t)a.spt_max * 256) return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: internal: head staging does not fit"));
-    const void* kfn = step_kernel_for(any_act, d->tp_world > 1, a.n_rep > 1, max_batch > 1);
+    const void* kfn = step_kernel_for(any_act, d->tp_world > 1, a.n_rep > 1, max_batch > 1, lora != nullptr);
     cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem);
     if (e != cudaSuccess) return plan_fail(p, exl_set_err(EXL_ERR_CUDA, "decode_plan: smem attribute (%zu B): %s", p->smem, cudaGetErrorString(e)));
     int per_sm = 0;
@@ -1578,6 +1742,16 @@ extern "C" int exl_decode_plan_create_batch(const exl_decode_desc* d, int max_ba
     const size_t o_att = take(mb * d->num_heads * a.att_slots * PART_LD * 4), o_bar = take(256), o_av = take((size_t)HQ * 2);
     const bool want_trace = getenv("EXL_DS_TRACE") != nullptr;
     const size_t o_trace = want_trace ? take((size_t)p->grid * TRACE_LAYERS * 24 * 8) : 0;
+    // LoRA: t accumulators, [max_batch][rank] per adapted matrix
+    std::vector<LoraMat> lm(lora ? (size_t)d->n_layers * 7 : 0);
+    size_t t_floats = 0;
+    for (size_t i = 0; i < lm.size(); i++) {
+        lm[i].rank = lora->rank[i];
+        lm[i].a = lm[i].rank ? (const half*)lora->a[i] : nullptr; lm[i].b = lm[i].rank ? (const half*)lora->b[i] : nullptr;
+        lm[i].t_off = (int)t_floats;
+        t_floats += mb * (size_t)lm[i].rank;
+    }
+    const size_t o_lt = lora ? take(t_floats * 4) : 0;
     const int W = d->tp_world > 1 ? d->tp_world : 1;
     p->shared_o = 0; p->shared_d = (((size_t)W * H * 8) + 255) & ~(size_t)255; p->shared_bar = 2 * p->shared_d;
     const size_t shared_bytes = p->shared_bar + 256;
@@ -1603,6 +1777,14 @@ extern "C" int exl_decode_plan_create_batch(const exl_decode_desc* d, int max_ba
     a.att_part = (float*)(p->d_scratch + o_att); a.bar = (unsigned long long*)(p->d_scratch + o_bar);
     if (const char* ed = getenv("EXL_DS_DEBUG")) a.debug = atoi(ed);
     a.trace = want_trace ? (unsigned long long*)(p->d_scratch + o_trace) : nullptr;
+    if (lora) {
+        static_assert(MAX_BATCH * (TILE + LORA_MAX_RANK) <= LORA_SCRATCH_ROOM, "LA scratch (lora_scratch_floats) exceeds the attention partial area");
+        if (cudaMalloc(&p->d_lora, sizeof(LoraMat) * lm.size()) != cudaSuccess ||
+            cudaMemcpy(p->d_lora, lm.data(), sizeof(LoraMat) * lm.size(), cudaMemcpyHostToDevice) != cudaSuccess)
+            return plan_fail(p, exl_set_err(EXL_ERR_CUDA, "decode_plan: LoRA table upload failed"));
+        a.lora = p->d_lora; a.lora_t = (float*)(p->d_scratch + o_lt); a.lora_t4 = (int)(t_floats / 4);
+        p->lora_barriers = lora_barriers(lora->rank, d->n_layers);
+    }
     *out = p;
     return EXL_OK;
 }
@@ -1653,7 +1835,8 @@ extern "C" int exl_decode_plan_info(const exl_decode_plan* p, int* grid, int* ri
 {
     if (!p) return exl_set_err(EXL_ERR_STATE, "decode_plan_info: NULL plan");
     if (grid) *grid = p->grid; if (ring_stages) *ring_stages = 4 * p->args.depth; if (smem_bytes) *smem_bytes = (int64_t)p->smem;
-    if (barriers_per_step) *barriers_per_step = 1 + (5 + (p->args.act ? 1 : 0) + (p->args.tp_world > 1 ? (p->args.tp_reduce ? 4 : 2) : 0)) * (int64_t)p->args.n_layers;
+    if (barriers_per_step) *barriers_per_step = 1 + (5 + (p->args.act ? 1 : 0) + (p->args.tp_world > 1 ? (p->args.tp_reduce ? 4 : 2) : 0)) * (int64_t)p->args.n_layers
+                                                           + p->lora_barriers;
     return EXL_OK;
 }
 
@@ -1711,7 +1894,7 @@ extern "C" int exl_decode_step_batch(exl_decode_plan* p, const void* x_in, int b
     cfg.gridDim = dim3((unsigned)p->grid); cfg.blockDim = dim3(DS_THREADS); cfg.dynamicSmemBytes = p->smem; cfg.stream = (cudaStream_t)stream_;
     cfg.attrs = at; cfg.numAttrs = 1;
     void* kargs[1] = {(void*)&a};
-    cudaError_t e = cudaLaunchKernelExC(&cfg, step_kernel_for(a.act != 0, a.tp_world > 1, a.n_rep > 1, p->max_batch > 1), kargs);
+    cudaError_t e = cudaLaunchKernelExC(&cfg, step_kernel_for(a.act != 0, a.tp_world > 1, a.n_rep > 1, p->max_batch > 1, a.lora != nullptr), kargs);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     if (e != cudaSuccess) return exl_set_err(EXL_ERR_CUDA, "launch of decode_step_kernel failed: %s (grid %d, smem %zu)", cudaGetErrorString(e), p->grid, p->smem);
     return EXL_OK;

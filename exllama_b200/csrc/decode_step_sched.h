@@ -185,4 +185,34 @@ static inline int max_batch_for(int H, int HQ, int I, int heads, int kv_heads, b
     return best;
 }
 
+// ---- LoRA adapters (exl_decode_plan_create_lora) ----
+// An adapted phase (any of its matrices has rank > 0) gets one extra step after its prologue, LA: units (adapted matrix j of the phase,
+// 128-row K stage s), numbered j * spt + s and cut into G contiguous shares.  The CTA of a unit dots that K stage of x with the 128 rows
+// of A and adds the result into t[b][rank] in L2; one grid barrier then makes t complete.  In the GEMV the B term of a tile of an
+// adapted matrix is added by exactly one CTA: the one that owns the tile's K stage 0.  A and B are read from global memory by the
+// consumers (no ring stage, no shared memory beyond the attention partial area, which is free outside ATT).
+constexpr int LORA_MAX_RANK = 128;
+DS_HD bool lora_rank_ok(int r) { return r >= 0 && r <= LORA_MAX_RANK && r % 8 == 0; }
+DS_HD int lora_units(int n_adapted, int spt) { return n_adapted * spt; }
+// the CTA that adds the B term of tile `tile` of a GEMV phase
+DS_HD int lora_b_cta(const Phase& p, int tile) { return cta_of((long long)tile * p.spt, p.U, p.G); }
+// first tile whose K stage 0 lies in the unit range [u0, u1) of a CTA (the B-term tiles are [first, last] with last = (u1 - 1) / spt)
+DS_HD int lora_b_first(const Phase& p, int u0) { return (u0 + p.spt - 1) / p.spt; }
+// fp32 floats of the LA step's shared scratch: x of one K stage and the partial t, per sequence (it lives in the attention partials)
+DS_HD int lora_scratch_floats(int max_batch, int max_rank) { return max_batch * (TILE + max_rank); }
+constexpr int LORA_SCRATCH_ROOM = 2 * 17 * PART_LD;
+// phase of matrix m (q k v o gate up down)
+DS_HD int lora_phase_of_mat(int m) { return m < 3 ? PH_QKV : (m == 3 ? PH_O : (m < 6 ? PH_GU : PH_DOWN)); }
+// extra grid barriers per step: one per adapted phase of every layer; rank: [n_layers * 7]
+static inline long long lora_barriers(const int* rank, int n_layers)
+{
+    long long n = 0;
+    for (int l = 0; l < n_layers; l++) {
+        bool ph[6] = {false, false, false, false, false, false};
+        for (int m = 0; m < 7; m++) if (rank[l * 7 + m] > 0) ph[lora_phase_of_mat(m)] = true;
+        n += (int)ph[PH_QKV] + (int)ph[PH_O] + (int)ph[PH_GU] + (int)ph[PH_DOWN];
+    }
+    return n;
+}
+
 } // namespace ds_sched

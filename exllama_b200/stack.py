@@ -102,8 +102,11 @@ class Q4Linear:
     def nbytes(self):
         return self.qweight.numel() * 4 + self.qzeros.numel() * 4 + self.scales.numel() * 2
 
-    def forward(self, x):
-        return cuda_ext.ext_q4_matmul(x, self.q4, self.width)
+    def forward(self, x, lora=None):
+        """x @ W (+ (x @ A) @ B with lora = (A, B), as Ex4bitLinear.forward passes an adapter, model.py:207-217)."""
+        if lora is None:
+            return cuda_ext.ext_q4_matmul(x, self.q4, self.width)
+        return cuda_ext.ext_q4_matmul(x, self.q4, self.width, lora[0], lora[1])
 
 
 class Layer:
@@ -183,6 +186,47 @@ class DecodeStack:
             self.temp_dq = torch.zeros((1, max_dq), dtype=torch.float16, device=self.device)
             ext.prepare_buffers(self.device, self.temp_state, self.temp_mlp, self.temp_zeros_float, self.temp_dq)
         self.none = cuda_ext.none_tensor
+        self.lora = None                       # per layer None or {projection name: (A [in, r], B [r, out] scaled)}, see add_lora
+
+    # ---- LoRA adapter (lora.py's layout: A transposed to [in, r], B [r, out] pre-scaled by alpha / r) ----------------------------
+    PROJ = ("q", "k", "v", "o", "gate", "up", "down")
+
+    def add_lora(self, rank, targets=("q", "v"), layers=None, alpha=None, seed=0):
+        """Synthesise one adapter of rank `rank` on the projections `targets` (names of PROJ, or "all") of `layers` (default every
+        layer) and attach it to every path of the stack (decode_step, prefill, make_plan).  Zero-mean Gaussian A ~ N(0, 1 / in) and
+        B ~ N(0, (0.2 / sqrt(r))^2), then B *= alpha / r as lora.py does (alpha defaults to r): the LoRA term is then about half the
+        rms of the projection's own output (synth_q4_device's gain is ~0.4) whatever the rank, and it has no DC gain a deep stack
+        could blow up through.  alpha scales the term as it does in PEFT: alpha = 2 r doubles it."""
+        if targets == "all":
+            targets = self.PROJ
+        assert all(t in self.PROJ for t in targets), targets
+        alpha = float(rank if alpha is None else alpha)
+        g = torch.Generator(device=self.device)
+        g.manual_seed(seed * 7717 + 5)
+        lora = self.lora or [None] * self.n_layers
+        for i in (range(self.n_layers) if layers is None else layers):
+            L = self.layers[i]
+            ad = dict(lora[i] or {})
+            for t in targets:
+                lin = getattr(L, t)
+                A = (torch.randn((lin.height, rank), device=self.device, generator=g) / math.sqrt(lin.height)).half()
+                B = (torch.randn((rank, lin.width), device=self.device, generator=g) * (0.2 / math.sqrt(rank)) * (alpha / rank)).half()
+                ad[t] = (A.contiguous(), B.contiguous())
+            lora[i] = ad
+        self.lora = lora
+        return lora
+
+    def _lora_of(self, i, name):
+        """(A, B) of projection `name` of layer i, or (none, none)."""
+        ad = self.lora[i] if self.lora is not None else None
+        if not ad or name not in ad:
+            return self.none, self.none
+        return ad[name]
+
+    def _lora_temp(self, i, names, rows):
+        """lora_temp as model.py:246-252 / 335-341 size it: [1, rows * the largest rank of the call], or none_tensor."""
+        r = max([self._lora_of(i, n)[0].shape[1] for n in names if self._lora_of(i, n)[0] is not self.none] + [0])
+        return torch.empty((1, rows * r), dtype=torch.float16, device=self.device) if r else self.none
 
     # ---- bookkeeping for rooflines -------------------------------------------------------------------------
     def q4_weight_bytes_per_token(self):
@@ -204,9 +248,12 @@ class DecodeStack:
             q = torch.empty((bsz, q_len, hq), dtype=torch.float16, device=self.device)
             k = torch.empty((bsz, q_len, hkv), dtype=torch.float16, device=self.device)
             v = torch.empty_like(k)
+            # LoRA tensors (or none) and lora_temp as ExLlamaAttention.fused passes them (model.py:322-341)
+            (q_a, q_b), (k_a, k_b), (v_a, v_b), (o_a, o_b) = (self._lora_of(i, n) for n in ("q", "k", "v", "o"))
+            lt_attn = self._lora_temp(i, ("q", "k", "v", "o"), bsz * q_len)
             ext.q4_attn(hidden, L.ln1, s.eps, q, k, v, L.q.q4, L.k.q4, L.v.q4, self.sin, self.cos, q_len, past_len,
                         self.local_heads, self.local_kv_heads, s.head_dim, key_cache[i], value_cache[i], self.max_seq,
-                        none, none, none, none, none, none, none)
+                        q_a, q_b, k_a, k_b, v_a, v_b, lt_attn)
             if self.fused_decode_attn and q_len == 1 and s.head_dim == 128:
                 # one kernel over the KV cache instead of the five torch launches below (csrc/decode_attn.cu)
                 attn = torch.empty_like(q)
@@ -222,9 +269,12 @@ class DecodeStack:
                 attn = torch.matmul(attn, values).transpose(1, 2).reshape(bsz, q_len, hq)
             x2 = hidden.view(-1, s.hidden)
             if self.tp_size == 1:
-                ext.q4_attn_2(x2, attn.view(-1, hq), L.o.q4, none, none, none)
-                ext.q4_mlp(x2, L.ln2, s.eps, L.gate.q4, L.up.q4, L.down.q4, none, none, none, none, none, none, none)
+                ext.q4_attn_2(x2, attn.view(-1, hq), L.o.q4, o_a, o_b, lt_attn)
+                (g_a, g_b), (u_a, u_b), (d_a, d_b) = (self._lora_of(i, n) for n in ("gate", "up", "down"))
+                ext.q4_mlp(x2, L.ln2, s.eps, L.gate.q4, L.up.q4, L.down.q4, g_a, g_b, u_a, u_b, d_a, d_b,
+                           self._lora_temp(i, ("gate", "up", "down"), bsz * q_len))
             else:
+                assert self.lora is None, "LoRA under tensor parallelism is not implemented"
                 tpmod.row_parallel_residual(ext, x2, self._o_input(attn.view(-1, hq)), L.o.q4, self.tp_rank, self.tp_group)
                 tpmod.mlp_tp(ext, cuda_ext, x2, L, s.eps, self.tp_rank, self.tp_group)
         if self.lm_head is None:
@@ -241,7 +291,8 @@ class DecodeStack:
         self.dplan = capi.DecodePlan(hs, [L.ln1 for L in self.layers], [L.ln2 for L in self.layers], self.key_cache, self.value_cache,
                                     self.sin, self.cos, self.local_heads, self.shape.head_dim, self.max_seq, self.shape.eps,
                                     final_norm=self.norm if head is not None else None, lm_head=head,
-                                    tp_rank=self.tp_rank, tp_world=self.tp_size, num_kv_heads=self.local_kv_heads, max_batch=self.batch)
+                                    tp_rank=self.tp_rank, tp_world=self.tp_size, num_kv_heads=self.local_kv_heads, max_batch=self.batch,
+                                    lora=self._plan_lora())
         if self.tp_size > 1:
             # exchange the cudaIpc handles of the regions the peers reduce into (acc_o, acc_d, cross-barrier counter)
             import torch.distributed as dist
@@ -252,6 +303,12 @@ class DecodeStack:
         self._plan_xout = torch.empty((self.batch, self.shape.hidden) if self.batch > 1 else self.shape.hidden, dtype=torch.float16, device=self.device)
         self._plan_logits = torch.empty((self.batch, self.shape.vocab), dtype=torch.float32, device=self.device) if head is not None else None
         return self.dplan
+
+    def _plan_lora(self):
+        """The adapter as DecodePlan takes it: per layer None or a 7-tuple of (A, B) or None; None without an adapter."""
+        if self.lora is None:
+            return None
+        return [None if not ad else tuple(ad.get(n) for n in self.PROJ) for ad in self.lora]
 
     def decode_step_fused(self, hidden, past_len):
         """hidden: [1, 1, hidden] fp16 (read only).  Returns logits [1, vocab] fp32 (or the final hidden state without a head);
@@ -284,16 +341,17 @@ class DecodeStack:
         bsz, q_len, _ = hidden.shape
         hq = self.local_heads * s.head_dim
         kvh = self.local_kv_heads
+        ad = lambda i, n: (self.lora[i] or {}).get(n) if self.lora is not None else None      # (A, B) or None
         for i, L in enumerate(self.layers):
             residual = hidden
             x = cuda_ext.ext_rms_norm(hidden, L.ln1, s.eps)
-            q = L.q.forward(x)
-            k = L.k.forward(x)
+            q = L.q.forward(x, ad(i, "q"))
+            k = L.k.forward(x, ad(i, "k"))
             ext.rope_(q, self.sin, self.cos, past_len, self.local_heads, s.head_dim)
             ext.rope_(k, self.sin, self.cos, past_len, kvh, s.head_dim)
             q = q.view(bsz, q_len, self.local_heads, s.head_dim).transpose(1, 2)
             k = k.view(bsz, q_len, kvh, s.head_dim).transpose(1, 2)
-            v = L.v.forward(x).view(bsz, q_len, kvh, s.head_dim).transpose(1, 2)
+            v = L.v.forward(x, ad(i, "v")).view(bsz, q_len, kvh, s.head_dim).transpose(1, 2)
             self.key_cache[i].narrow(2, past_len, q_len).copy_(k)
             self.value_cache[i].narrow(2, past_len, q_len).copy_(v)
             keys = repeat_kv(self.key_cache[i].narrow(2, 0, past_len + q_len), self.n_rep)
@@ -302,15 +360,15 @@ class DecodeStack:
                 raise NotImplementedError("chunked prefill with past is outside the benchmarked path")
             attn = torch.nn.functional.scaled_dot_product_attention(q, keys, values, attn_mask=None, is_causal=True)
             attn = attn.transpose(1, 2).reshape(bsz, q_len, hq)
-            o = L.o.forward(self._o_input(attn.view(-1, hq)).view(bsz, q_len, hq))
+            o = L.o.forward(self._o_input(attn.view(-1, hq)).view(bsz, q_len, hq), ad(i, "o"))
             if self.tp_size > 1:
                 tpmod.all_reduce(o, self.tp_group)
             hidden = residual + o
             residual = hidden
             x = cuda_ext.ext_rms_norm(hidden, L.ln2, s.eps)
-            y = torch.nn.functional.silu(L.gate.forward(x))
-            y *= L.up.forward(x)
-            y = L.down.forward(y)
+            y = torch.nn.functional.silu(L.gate.forward(x, ad(i, "gate")))
+            y *= L.up.forward(x, ad(i, "up"))
+            y = L.down.forward(y, ad(i, "down"))
             if self.tp_size > 1:
                 tpmod.all_reduce(y, self.tp_group)
             hidden = residual + y

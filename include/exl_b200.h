@@ -203,6 +203,21 @@ int exl_decode_plan_create(const exl_decode_desc* desc, exl_decode_plan** out_pl
    max_batch * num_heads -- num_kv_heads under grouped-query attention -- <= SMs); otherwise EXL_ERR_ARG naming what fits.
    exl_decode_plan_create(d, out) is exl_decode_plan_create_batch(d, 1, out). */
 int exl_decode_plan_create_batch(const exl_decode_desc* desc, int max_batch, exl_decode_plan** out_plan);
+/* LoRA adapters (model.py's `lora` argument, lora.py): each of the 7 projections of each layer may carry an adapter; the step adds
+   (x . A) . B to that projection's output, as exl_q4_matmul_lora does, with x . A rounded to fp16 (the reference's lora_temp) and the
+   product with B accumulated in fp32 into the projection (the reference's second fp16 rounding, of (x . A) . B, is skipped).  Works in
+   every single-GPU configuration exl_decode_plan_create_batch accepts (multi-head and grouped-query attention, 1 .. max_batch
+   sequences with the same adapter, act-order at max_batch 1).  A and B are borrowed like every other pointer of the plan; another
+   adapter needs another plan.  lora == NULL or every rank 0 gives exactly exl_decode_plan_create_batch's plan.  EXL_ERR_ARG (naming the
+   per-op path) for: tp_world > 1, a rank that is not a multiple of 8 in 8 .. 128, A or B not 16-byte aligned, n_layers != desc's, a
+   rank > 0 with a NULL A or B. */
+typedef struct exl_decode_lora {
+    int n_layers;                 /* must equal desc->n_layers */
+    const void* const* a;         /* [n_layers * 7] half [K, rank] (lora.py layout: A transposed) or NULL */
+    const void* const* b;         /* [n_layers * 7] half [rank, N], already scaled by alpha / rank, or NULL */
+    const int* rank;              /* [n_layers * 7], host; 0 = no adapter on that projection */
+} exl_decode_lora;
+int exl_decode_plan_create_lora(const exl_decode_desc* desc, int max_batch, const exl_decode_lora* lora, exl_decode_plan** out_plan);
 int exl_decode_plan_destroy(exl_decode_plan* plan);
 /* Tensor parallel set-up: export this rank's 64-byte cudaIpc handle, exchange (e.g. through torch.distributed), import all of
    them (world x 64 bytes in rank order) on every rank before the first exl_decode_step; every rank must then call

@@ -3,7 +3,10 @@
 Accepts the SHAPES names and the grouped-query attention ones (GQA_SHAPES, e.g. 70b); the line records the GPU and its power limit.
 --batch N times one launch for N sequences, all at --ctx (aggregate tok/s = N tokens per launch; bytes = weights + head + N x K/V);
 the per-op arm then times sequence 0 alone.
-    python tools/step_bench.py [--model 7b] [--ctx 1920] [--seq 2048] [--groupsize 128] [--act-order] [--layers N] [--reps 20] [--batch N]"""
+--lora-rank R attaches a synthetic LoRA adapter of rank R (DecodeStack.add_lora) to q and v (--lora-targets qv) or to all seven
+projections (all); both arms then run it.
+    python tools/step_bench.py [--model 7b] [--ctx 1920] [--seq 2048] [--groupsize 128] [--act-order] [--layers N] [--reps 20] [--batch N]
+                               [--lora-rank R] [--lora-targets qv|all]"""
 import argparse, json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -32,6 +35,8 @@ def main():
     ap.add_argument("--reps", type=int, default=20, help="minimum timed steps per arm (more if the window would be under 1.2 s)")
     ap.add_argument("--no-per-op", action="store_true")
     ap.add_argument("--batch", type=int, default=1, help="sequences per launch (1..4, as far as the model fits)")
+    ap.add_argument("--lora-rank", type=int, default=0, help="rank of a synthetic LoRA adapter (0: none)")
+    ap.add_argument("--lora-targets", choices=["qv", "all"], default="qv", help="projections the adapter covers")
     args = ap.parse_args()
     shapes = {**SHAPES, **GQA_SHAPES}
     if args.model not in shapes:
@@ -46,6 +51,8 @@ def main():
                      batch=args.batch)
     for kc, vc in zip(st.key_cache, st.value_cache):
         kc.normal_(0, 0.5); vc.normal_(0, 0.5)
+    if args.lora_rank:
+        st.add_lora(args.lora_rank, targets=("q", "v") if args.lora_targets == "qv" else "all")
     st.make_plan()
     nb = args.batch
     xb = (torch.randn((nb, 1, shape.hidden), device="cuda") * 0.5).half()
@@ -70,7 +77,8 @@ def main():
         return a.elapsed_time(b) / reps, reps
     res = {"tool": "tools/step_bench.py", "model": args.model, "ctx": args.ctx, "seq": args.seq, "groupsize": args.groupsize,
            "act_order": args.act_order, "layers": len(st.layers), "heads": shape.heads, "kv_heads": shape.kv_heads,
-           "gpu": torch.cuda.get_device_name(0), "power_limit_w": power_limit(torch.cuda.current_device()), "plan": st.dplan.info()}
+           "gpu": torch.cuda.get_device_name(0), "power_limit_w": power_limit(torch.cuda.current_device()), "plan": st.dplan.info(),
+           "lora_rank": args.lora_rank, "lora_targets": args.lora_targets if args.lora_rank else None}
     if nb > 1:
         res["batch"] = nb
         ms, reps = timed(lambda: st.decode_step_fused_batch(xb, [args.ctx] * nb))

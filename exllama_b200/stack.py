@@ -337,12 +337,17 @@ class DecodeStack:
 
     # ---- prefill: unfused path (model.py:532-550) --------------------------------------------------------------
     def prefill(self, hidden, past_len=0, last_only=True):
+        """hidden: [bsz, q_len, hidden] fp16, bsz <= batch; sequence b fills rows [past_len, past_len + q_len) of cache sequence b.
+        Returns logits [bsz, vocab] of the last position (last_only) or [bsz * q_len, vocab]."""
         s = self.shape
         bsz, q_len, _ = hidden.shape
+        if bsz > self.batch:
+            raise ValueError(f"prefill of {bsz} sequences into caches that hold {self.batch} (DecodeStack(..., batch=))")
         hq = self.local_heads * s.head_dim
         kvh = self.local_kv_heads
         ad = lambda i, n: (self.lora[i] or {}).get(n) if self.lora is not None else None      # (A, B) or None
         for i, L in enumerate(self.layers):
+            key_cache, value_cache = self.key_cache[i][:bsz], self.value_cache[i][:bsz]
             residual = hidden
             x = cuda_ext.ext_rms_norm(hidden, L.ln1, s.eps)
             q = L.q.forward(x, ad(i, "q"))
@@ -352,10 +357,10 @@ class DecodeStack:
             q = q.view(bsz, q_len, self.local_heads, s.head_dim).transpose(1, 2)
             k = k.view(bsz, q_len, kvh, s.head_dim).transpose(1, 2)
             v = L.v.forward(x, ad(i, "v")).view(bsz, q_len, kvh, s.head_dim).transpose(1, 2)
-            self.key_cache[i].narrow(2, past_len, q_len).copy_(k)
-            self.value_cache[i].narrow(2, past_len, q_len).copy_(v)
-            keys = repeat_kv(self.key_cache[i].narrow(2, 0, past_len + q_len), self.n_rep)
-            values = repeat_kv(self.value_cache[i].narrow(2, 0, past_len + q_len), self.n_rep)
+            key_cache.narrow(2, past_len, q_len).copy_(k)
+            value_cache.narrow(2, past_len, q_len).copy_(v)
+            keys = repeat_kv(key_cache.narrow(2, 0, past_len + q_len), self.n_rep)
+            values = repeat_kv(value_cache.narrow(2, 0, past_len + q_len), self.n_rep)
             if past_len > 0:
                 raise NotImplementedError("chunked prefill with past is outside the benchmarked path")
             attn = torch.nn.functional.scaled_dot_product_attention(q, keys, values, attn_mask=None, is_causal=True)

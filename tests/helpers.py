@@ -44,6 +44,61 @@ def golden_cols(n, seed, k=512):
     return np.sort(np.random.default_rng(seed).choice(n, k, replace=False))
 
 
+def _np(t):
+    return t.cpu().numpy()
+
+
+def adapter_of(st, i, name):
+    """(A, B) of projection `name` of layer i of a DecodeStack, or None."""
+    return (st.lora[i] or {}).get(name) if st.lora is not None else None
+
+
+def oracle_mm(oracle, xin, lin, ab=None, acc=None, recons=False):
+    """x . W of a stack projection in float64 (act-order: the x gather of make_q4's sequential layout), accumulated onto acc, with an
+    adapter (A, B): acc + fp16(fp16(x . A) . B) as q4_matmul_lora and the per-op blocks compose it.
+
+    recons=True contracts against the fp16-rounded reconstructed weights (what the wgmma GEMM's B operand holds, bit-identical to
+    reconstruct_kernel).  Those weights come from oracle.reconstruct_f16 once and are contracted in float64 by numpy: the same exact
+    sum as oracle.q4_matmul_f64(..., recons=True), which re-dequantises every weight for every row and is too slow for a prefill."""
+    xm = None if lin.g_idx is None else oracle.make_x_map(lin.g_idx.numpy(), lin.qzeros.shape[0])
+    if ab is not None:
+        t = oracle.half_matmul_f64(xin, _np(ab[0])).astype(np.float16)
+        acc = oracle.half_matmul_f64(t, _np(ab[1]), acc_in=acc).astype(np.float16)
+    if not recons:
+        return oracle.q4_matmul_f64(xin, _np(lin.qweight), _np(lin.qzeros), _np(lin.scales), xm, acc)
+    w = oracle.reconstruct_f16(_np(lin.qweight), _np(lin.qzeros), _np(lin.scales)).astype(np.float64)
+    xg = np.asarray(xin, np.float64) if xm is None else np.asarray(xin, np.float64)[:, xm]
+    out = xg @ w
+    return out if acc is None else out + np.asarray(acc, np.float64)
+
+
+def oracle_decode_step(oracle, st, snap, x, past, seq=0):
+    """float64/fp16 restatement of one decode token of a DecodeStack (grouped-query attention, cache sequence `seq`, the stack's
+    adapter) on the cache snapshot `snap` (per layer (key_cache, value_cache) tensors): (final hidden fp16, logits float64, new k/v
+    rows per layer)."""
+    s = st.shape
+    hd, heads, kvh = s.head_dim, s.heads, s.kv_heads
+    sin = st.sin.view(-1, hd).cpu().numpy(); cos = st.cos.view(-1, hd).cpu().numpy()
+    x = x.reshape(1, s.hidden).copy()
+    rows = []
+    for i, L in enumerate(st.layers):
+        xn, _ = oracle.rms_norm(x, _np(L.ln1), s.eps)
+        q, k, v = (oracle_mm(oracle, xn, getattr(L, n), adapter_of(st, i, n)).astype(np.float16) for n in ("q", "k", "v"))
+        q = oracle.rope(q.reshape(1, heads, hd), sin, cos, 1, heads, hd, heads, past).reshape(-1)
+        k = oracle.rope(k.reshape(1, kvh, hd), sin, cos, 1, kvh, hd, kvh, past).reshape(kvh, hd)
+        kc = _np(snap[i][0][seq]).copy(); vc = _np(snap[i][1][seq]).copy()
+        kc[:, past] = k; vc[:, past] = v.reshape(kvh, hd)
+        rows.append((k.copy(), v.reshape(kvh, hd).copy()))
+        attn = oracle.decode_attn_f64(q, kc, vc, heads, kvh, hd, past + 1, st.max_seq).astype(np.float16).reshape(1, -1)
+        x = oracle_mm(oracle, attn, L.o, adapter_of(st, i, "o"), acc=x).astype(np.float16)
+        xn, _ = oracle.rms_norm(x, _np(L.ln2), s.eps)
+        act = oracle.silu_mul(oracle_mm(oracle, xn, L.gate, adapter_of(st, i, "gate")).astype(np.float16),
+                              oracle_mm(oracle, xn, L.up, adapter_of(st, i, "up")).astype(np.float16))
+        x = oracle_mm(oracle, act, L.down, adapter_of(st, i, "down"), acc=x).astype(np.float16)
+    hn, _ = oracle.rms_norm(x, _np(st.norm), s.eps)
+    return x, hn.astype(np.float64) @ _np(st.lm_head).astype(np.float64).T, rows
+
+
 def to_cuda(*arrays):
     import torch
     out = []

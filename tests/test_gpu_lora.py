@@ -11,7 +11,7 @@ adapter on q and v shows in the logits even when the softmax over a long synthet
 import numpy as np
 import pytest
 
-from helpers import assert_close_ref64
+from helpers import assert_close_ref64, oracle_decode_step, oracle_mm
 
 pytestmark = pytest.mark.gpu
 
@@ -47,45 +47,6 @@ def _restore(st, snap):
 
 def _np(t):
     return t.cpu().numpy()
-
-
-def _mm(oracle, xin, lin, ab=None, acc=None):
-    """x . W of a stack projection in float64 (act-order: the x gather of make_q4's sequential layout), accumulated onto acc, with an
-    adapter (A, B): acc + fp16(fp16(x . A) . B) as q4_matmul_lora and the per-op blocks compose it."""
-    xm = None if lin.g_idx is None else oracle.make_x_map(lin.g_idx.numpy(), lin.qzeros.shape[0])
-    if ab is not None:
-        t = oracle.half_matmul_f64(xin, _np(ab[0])).astype(np.float16)
-        acc = oracle.half_matmul_f64(t, _np(ab[1]), acc_in=acc).astype(np.float16)
-    return oracle.q4_matmul_f64(xin, _np(lin.qweight), _np(lin.qzeros), _np(lin.scales), xm, acc)
-
-
-def _ab(st, i, name):
-    return (st.lora[i] or {}).get(name) if st.lora is not None else None
-
-
-def _oracle_step(oracle, st, snap, x, past, seq=0):
-    """float64/fp16 restatement of one decode token with the stack's adapter: (final hidden fp16, logits float64, new k/v rows)."""
-    s = st.shape
-    hd, heads, kvh = s.head_dim, s.heads, s.kv_heads
-    sin = st.sin.view(-1, hd).cpu().numpy(); cos = st.cos.view(-1, hd).cpu().numpy()
-    x = x.reshape(1, s.hidden).copy()
-    rows = []
-    for i, L in enumerate(st.layers):
-        xn, _ = oracle.rms_norm(x, _np(L.ln1), s.eps)
-        q, k, v = (_mm(oracle, xn, getattr(L, n), _ab(st, i, n)).astype(np.float16) for n in ("q", "k", "v"))
-        q = oracle.rope(q.reshape(1, heads, hd), sin, cos, 1, heads, hd, heads, past).reshape(-1)
-        k = oracle.rope(k.reshape(1, kvh, hd), sin, cos, 1, kvh, hd, kvh, past).reshape(kvh, hd)
-        kc = _np(snap[i][0][seq]).copy(); vc = _np(snap[i][1][seq]).copy()
-        kc[:, past] = k; vc[:, past] = v.reshape(kvh, hd)
-        rows.append((k.copy(), v.reshape(kvh, hd).copy()))
-        attn = oracle.decode_attn_f64(q, kc, vc, heads, kvh, hd, past + 1, st.max_seq).astype(np.float16).reshape(1, -1)
-        x = _mm(oracle, attn, L.o, _ab(st, i, "o"), acc=x).astype(np.float16)
-        xn, _ = oracle.rms_norm(x, _np(L.ln2), s.eps)
-        act = oracle.silu_mul(_mm(oracle, xn, L.gate, _ab(st, i, "gate")).astype(np.float16),
-                              _mm(oracle, xn, L.up, _ab(st, i, "up")).astype(np.float16))
-        x = _mm(oracle, act, L.down, _ab(st, i, "down"), acc=x).astype(np.float16)
-    hn, _ = oracle.rms_norm(x, _np(st.norm), s.eps)
-    return x, hn.astype(np.float64) @ _np(st.lm_head).astype(np.float64).T, rows
 
 
 def _per_op(st, snap, xs, pasts):
@@ -130,7 +91,7 @@ def _check_step(oracle, st, xs, pasts, what):
     torch.cuda.synchronize()
     got_x = st._plan_xout.view(-1, st.shape.hidden)[:bsz].cpu().numpy()
     for b in range(bsz):
-        want_x, want_logits, rows = _oracle_step(oracle, st, snap, _np(xs[b]), pasts[b], b)
+        want_x, want_logits, rows = oracle_decode_step(oracle, st, snap, _np(xs[b]), pasts[b], b)
         w = f"{what} seq {b} (ctx {pasts[b]})"
         assert_close_ref64(got_x[b], want_x.reshape(-1).astype(np.float64), rel=1e-2, rms=1e-2, what=f"{w} final hidden vs oracle")
         assert_close_ref64(logits[b], want_logits.reshape(-1), rel=1.5e-2, rms=1.5e-2, what=f"{w} logits vs oracle")
@@ -174,7 +135,7 @@ def test_per_op_blocks_vs_oracle(oracle, rank, act, kv):
                 st.max_seq, *ab("q"), *ab("k"), *ab("v"), lt)
     sin = st.sin.view(-1, hd).cpu().numpy(); cos = st.cos.view(-1, hd).cpu().numpy()
     xn, _ = oracle.rms_norm(x0, _np(L.ln1), s.eps)
-    wq, wk, wv = (_mm(oracle, xn, getattr(L, n), ab(n)).astype(np.float16) for n in ("q", "k", "v"))
+    wq, wk, wv = (oracle_mm(oracle, xn, getattr(L, n), ab(n)).astype(np.float16) for n in ("q", "k", "v"))
     wq = oracle.rope(wq.reshape(1, heads, hd), sin, cos, 1, heads, hd, heads, past).reshape(-1)
     wk = oracle.rope(wk.reshape(1, kv, hd), sin, cos, 1, kv, hd, kv, past).reshape(-1)
     tol = dict(rel=6e-3, rms=6e-3)
@@ -188,14 +149,14 @@ def test_per_op_blocks_vs_oracle(oracle, rank, act, kv):
     attn = (torch.randn((1, heads * hd), device="cuda") * 0.5).half()
     x2 = x.view(1, -1).clone()
     ext.q4_attn_2(x2, attn, L.o.q4, *ab("o"), lt)
-    want = _mm(oracle, _np(attn), L.o, ab("o"), acc=x0)
+    want = oracle_mm(oracle, _np(attn), L.o, ab("o"), acc=x0)
     assert_close_ref64(_np(x2), want, what="q4_attn_2", **tol)
     # q4_mlp: x += down(silu(gate(n)) * up(n)), every projection with its adapter
     x3 = x.view(1, -1).clone()
     ext.q4_mlp(x3, L.ln2, s.eps, L.gate.q4, L.up.q4, L.down.q4, *ab("gate"), *ab("up"), *ab("down"), lt)
     xn, _ = oracle.rms_norm(x0, _np(L.ln2), s.eps)
-    a = oracle.silu_mul(_mm(oracle, xn, L.gate, ab("gate")).astype(np.float16), _mm(oracle, xn, L.up, ab("up")).astype(np.float16))
-    want = _mm(oracle, a, L.down, ab("down"), acc=x0)
+    a = oracle.silu_mul(oracle_mm(oracle, xn, L.gate, ab("gate")).astype(np.float16), oracle_mm(oracle, xn, L.up, ab("up")).astype(np.float16))
+    want = oracle_mm(oracle, a, L.down, ab("down"), acc=x0)
     assert_close_ref64(_np(x3), want, what="q4_mlp", **tol)
     st.close()
 

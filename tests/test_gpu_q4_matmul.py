@@ -153,7 +153,30 @@ def test_skinny_unsupported_groupsize_takes_general_route(oracle, M, K, N, gs, a
 TC_CASES = [(128, 1024, 512, 128, False), (200, 2048, 384, 32, True), (1, 512, 128, 64, False), (77, 4096, 1152, 128, True),
             (384, 1024, 1024, 1024, False), (130, 2816, 96, 128, False),
             # M > 128 and ceil(M / 256) * ceil(N / 128) >= SMs / 2: the 256-row (MT = 2) tiles, with a partial last M tile
-            (300, 1024, 8448, 128, False), (260, 512, 8448, 32, True)]
+            (300, 1024, 8448, 128, False), (260, 512, 8448, 32, True),
+            # either side of the 128- and 256-row tile edges at 66 column tiles: MT = 1 up to M = 128, MT = 2 above; at M = 129 the
+            # second 128-row sub-tile holds one row, at M = 257 the last CTA's first sub-tile holds one row and its second none
+            (127, 256, 8448, 128, False), (128, 256, 8448, 32, True), (129, 256, 8448, 128, False),
+            (255, 256, 8448, 32, False), (256, 256, 8448, 128, True), (257, 256, 8448, 32, False),
+            # 32 column tiles: 2 x 32 = 64 row-pair tiles < 66 (half of 132 SMs) at M = 512, 3 x 32 = 96 at 513: MT flips from 1 to 2
+            (512, 256, 4096, 128, False), (513, 256, 4096, 32, True)]
+
+
+def _tc_mt(M, N, sms):
+    """Rows per CTA of the wgmma GEMM over 128 (exl_tc_gemm_launch's tile choice): 2 when M > 128 and 256-row tiles still give at
+    least half a CTA per SM."""
+    return 2 if M > 128 and (M + 255) // 256 * ((N + 127) // 128) >= sms // 2 else 1
+
+
+def test_tc_cases_cover_both_tile_heights():
+    """TC_CASES runs both instantiations of q4_gemm_tc_kernel (MT = 1 and MT = 2) on the card the suite runs on, and M = 512 / 513 at
+    N = 4096 sit on either side of the switch."""
+    import torch
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    assert {_tc_mt(M, N, sms) for M, _, N, _, _ in TC_CASES} == {1, 2}, sms
+    if sms == 132:
+        assert (_tc_mt(512, 4096, sms), _tc_mt(513, 4096, sms)) == (1, 2)
+        assert [_tc_mt(M, 8448, sms) for M in (127, 128, 129, 255, 256, 257)] == [1, 1, 2, 2, 2, 2]
 
 
 @pytest.mark.parametrize("M,K,N,gs,act", TC_CASES)
@@ -168,15 +191,30 @@ def test_tcgen05_gemm_vs_ref64(oracle, M, K, N, gs, act):
     out = capi.q4_matmul(to_cuda(x), q4, force_path=2)
     torch.cuda.synchronize()
     assert capi.last_q4_path() == "tc_gemm"
-    if N >= 8192:
-        assert M > 128 and (M + 255) // 256 * ((N + 127) // 128) >= torch.cuda.get_device_properties(0).multi_processor_count // 2
+    mt = _tc_mt(M, N, torch.cuda.get_device_properties(0).multi_processor_count)
     ref = oracle.ref64_with_act_order(x, qw, qz, sc, g_idx, recons=True)
-    assert_close_ref64(out.cpu().numpy(), ref, what=f"tc_gemm M{M} K{K} N{N} g{gs} act{act}")
+    assert_close_ref64(out.cpu().numpy(), ref, what=f"tc_gemm M{M} K{K} N{N} g{gs} act{act} MT{mt}")
     res = oracle.synth_x(M, N, seed=99)
     out2 = to_cuda(res.copy())
     capi.q4_matmul(to_cuda(x), q4, out=out2, no_zero=True, force_path=2)
     ref2 = oracle.ref64_with_act_order(x, qw, qz, sc, g_idx, acc_in=res, recons=True)
-    assert_close_ref64(out2.cpu().numpy(), ref2, what="tc_gemm accumulate")
+    assert_close_ref64(out2.cpu().numpy(), ref2, what=f"tc_gemm accumulate MT{mt}")
+
+
+@pytest.mark.parametrize("M,path", [(48, "skinny_mma"), (49, "tc_gemm")])
+def test_auto_route_threshold(oracle, M, path):
+    """force_path=0: M = 48 is the last M of the repeated skinny passes, M = 49 the first of the wgmma GEMM."""
+    import torch
+    from exllama_b200 import capi
+    K, N, gs = 1024, 512, 128
+    qw, qz, sc, g_idx = _mk(oracle, K, N, gs, True, seed=M)
+    x = oracle.synth_x(M, K, seed=M + 1)
+    q4 = _q4(capi, qw, qz, sc, g_idx)
+    out = capi.q4_matmul(to_cuda(x), q4)
+    torch.cuda.synchronize()
+    assert capi.last_q4_path() == path
+    ref = oracle.ref64_with_act_order(x, qw, qz, sc, g_idx, recons=path == "tc_gemm")
+    assert_close_ref64(out.cpu().numpy(), ref, what=f"auto route M{M}")
 
 
 def test_reconstruct_bit_exact(oracle):

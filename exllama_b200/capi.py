@@ -41,6 +41,7 @@ SIGNATURES = {
     "exl_q4_mlp": (i32, [vp, vp, f32, vp, vp, vp, i32, i32] + [vp, vp, i32] * 3 + [vp, i32, vp]),
     "exl_tp_status": (i32, [i32, C.POINTER(C.c_uint)]),
     "exl_decode_attn": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
+    "exl_prefill_attn": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]),
     "exl_q4_attn_2_tp": (i32, [vp, vp, vp, i32, i32, vp]),
     "exl_tp_workspace_alloc": (i32, [i32, C.POINTER(vp), vp]),
     "exl_tp_workspace_open": (i32, [i32, vp, C.POINTER(vp)]),
@@ -203,6 +204,18 @@ def decode_attn(q, key_cache, value_cache, num_heads, num_kv_heads, head_dim, se
     import torch
     out = torch.empty_like(q)
     check(lib().exl_decode_attn(_ptr(q), _ptr(key_cache), _ptr(value_cache), _ptr(out), num_heads, num_kv_heads, head_dim, seq_len, max_seq_len, _stream()))
+    return out
+
+
+def prefill_attn(q, key_cache, value_cache, num_heads, num_kv_heads, head_dim, past_len, max_seq_len, out=None):
+    """q half [bsz, q_len, num_heads, head_dim] -> out half [bsz, q_len, num_heads * head_dim]: causal attention of the chunk at
+    positions [past_len, past_len + q_len) over cache rows [0, past_len + t] (include/exl_b200.h exl_prefill_attn)."""
+    import torch
+    bsz, q_len = q.shape[0], q.shape[1]
+    if out is None:
+        out = torch.empty((bsz, q_len, num_heads * head_dim), dtype=torch.float16, device=q.device)
+    check(lib().exl_prefill_attn(_ptr(q), _ptr(key_cache), _ptr(value_cache), _ptr(out), bsz, q_len, num_heads, num_kv_heads, head_dim,
+                                 past_len, max_seq_len, _stream()))
     return out
 
 

@@ -76,7 +76,8 @@ int exl_own_scratch(ExlDevice* ds, int role, int64_t numel, half** out)
 extern "C" {
 
 const char* exl_last_error(void) { return t_err; }
-int exl_version(void) { return 103; }             // 101: exl_decode_desc.num_kv_heads; 102: batched decode plans and steps; 103: LoRA plans
+int exl_version(void) { return 104; }             // 101: exl_decode_desc.num_kv_heads; 102: batched decode plans and steps; 103: LoRA plans;
+                                                  // 104: exl_prefill_attn
 int64_t exl_launch_count(void) { return g_launches.load(); }
 const char* exl_last_q4_path(void) { return g_last_q4_path; }
 
@@ -576,6 +577,13 @@ int exl_decode_attn(const void* q, const void* key_cache, const void* value_cach
 {
     return exl_decode_attn_launch((const half*)q, (const half*)key_cache, (const half*)value_cache, (half*)out, num_heads, num_kv_heads,
                                   head_dim, seq_len, max_seq_len, 1.0f / sqrtf((float)head_dim), (cudaStream_t)stream);
+}
+
+int exl_prefill_attn(const void* q, const void* key_cache, const void* value_cache, void* out, int bsz, int q_len, int num_heads,
+                     int num_kv_heads, int head_dim, int past_len, int max_seq_len, void* stream)
+{
+    return exl_prefill_attn_launch((const half*)q, (const half*)key_cache, (const half*)value_cache, (half*)out, bsz, q_len, num_heads,
+                                   num_kv_heads, head_dim, past_len, max_seq_len, (cudaStream_t)stream);
 }
 
 int exl_q4_matmul_host(const void* x_host, int M, const exl_q4_matrix* w, void* out_host, void* d_x, void* d_out, void* stream_)

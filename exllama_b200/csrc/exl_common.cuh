@@ -157,6 +157,10 @@ int exl_column_remap_launch(const half* x, half* x_new, int M, int K, const uint
 int exl_decode_attn_launch(const half* q, const half* kc, const half* vc, half* out, int heads, int kv_heads, int head_dim,
                            int seq, int max_seq, float scale, cudaStream_t stream);
 
+// prefill_attn.cu
+int exl_prefill_attn_launch(const half* q, const half* kc, const half* vc, half* out, int bsz, int q_len, int heads, int kv_heads,
+                            int head_dim, int past_len, int max_seq, cudaStream_t stream);
+
 // half_matmul.cu
 int exl_half_matmul_cublas_launch(ExlDevice* ds, const half* x, const half* w, half* out, int M, int K, int N, bool no_zero, cudaStream_t stream);
 int exl_half_matmul_custom_launch(const half* x, const half* w, half* out, int M, int K, int N, cudaStream_t stream);

@@ -265,6 +265,27 @@ void decode_attn(torch::Tensor q, torch::Tensor key_cache, torch::Tensor value_c
                              head_dim, seq_len, max_seq_len, cur_stream()));
 }
 
+// causal attention of a chunk over the KV cache: q [bsz, q_len, heads(*hd) ...] -> out [bsz, q_len, heads*hd]; caches are the bsz
+// sequences [bsz, kv_heads, max_seq_len, hd] the chunk belongs to
+void prefill_attn(torch::Tensor q, torch::Tensor key_cache, torch::Tensor value_cache, torch::Tensor out, int num_heads,
+                  int num_kv_heads, int head_dim, int past_len, int max_seq_len)
+{
+    CHECK_DTYPE(q, kHalf); CHECK_DTYPE(key_cache, kHalf); CHECK_DTYPE(value_cache, kHalf); CHECK_DTYPE(out, kHalf);
+    TORCH_CHECK(q.dim() >= 2, "prefill_attn: q must be [bsz, q_len, ...]");
+    const int64_t bsz = q.size(0), q_len = q.size(1);
+    const int64_t tok = (int64_t)num_heads * head_dim;
+    TORCH_CHECK(q.is_contiguous() && q.numel() == bsz * q_len * tok, "prefill_attn: q must be contiguous [bsz, q_len, num_heads, head_dim]");
+    TORCH_CHECK(out.is_contiguous() && out.numel() == q.numel(), "prefill_attn: out must be contiguous [bsz, q_len, num_heads * head_dim]");
+    const int64_t cache = bsz * num_kv_heads * (int64_t)max_seq_len * head_dim;
+    TORCH_CHECK(key_cache.is_contiguous() && value_cache.is_contiguous() && key_cache.numel() == cache && value_cache.numel() == cache,
+                "prefill_attn: caches must be contiguous [bsz, num_kv_heads, max_seq_len, head_dim]");
+    TORCH_CHECK(key_cache.device() == q.device() && value_cache.device() == q.device() && out.device() == q.device(),
+                "prefill_attn: tensors on different devices");
+    const at::cuda::OptionalCUDAGuard device_guard(q.device());
+    EXL_CALL(exl_prefill_attn(q.data_ptr(), key_cache.data_ptr(), value_cache.data_ptr(), out.data_ptr(), (int)bsz, (int)q_len,
+                              num_heads, num_kv_heads, head_dim, past_len, max_seq_len, cur_stream()));
+}
+
 // fused projection + peer-memory all-reduce
 pybind11::tuple tp_workspace_alloc(int device)
 {
@@ -326,6 +347,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m)
     m.def("q4_attn_2_tp", &q4_attn_2_tp, "q4_attn_2_tp");
     m.def("q4_mlp_tp", &q4_mlp_tp, "q4_mlp_tp");
     m.def("decode_attn", &decode_attn, "decode_attn");
+    m.def("prefill_attn", &prefill_attn, "prefill_attn");
     m.def("tp_status", [](int device) { unsigned t = 0; EXL_CALL(exl_tp_status(device, &t)); return (int)t; }, "tp_status");
     m.def("tp_workspace_alloc", &tp_workspace_alloc, "tp_workspace_alloc");
     m.def("tp_workspace_open", &tp_workspace_open, "tp_workspace_open");

@@ -336,35 +336,48 @@ class DecodeStack:
         return full.index_select(1, self.o_rows)
 
     # ---- prefill: unfused path (model.py:532-550) --------------------------------------------------------------
-    def prefill(self, hidden, past_len=0, last_only=True):
-        """hidden: [bsz, q_len, hidden] fp16, bsz <= batch; sequence b fills rows [past_len, past_len + q_len) of cache sequence b.
-        Returns logits [bsz, vocab] of the last position (last_only) or [bsz * q_len, vocab]."""
+    def prefill(self, hidden, past_len=0, last_only=True, seq=0):
+        """hidden: [bsz, q_len, hidden] fp16; sequence b fills rows [past_len, past_len + q_len) of cache sequence seq + b and attends
+        rows [0, past_len + t] of it (a prompt chunk, or a follow-up turn appended to a live cache).  Returns logits [bsz, vocab] of
+        the last position (last_only) or [bsz * q_len, vocab].  At past_len 0 attention is torch's causal SDPA (model.py's
+        prompt path); at past_len > 0 it is csrc/prefill_attn.cu over the cache in place."""
         s = self.shape
         bsz, q_len, _ = hidden.shape
         if bsz > self.batch:
             raise ValueError(f"prefill of {bsz} sequences into caches that hold {self.batch} (DecodeStack(..., batch=))")
+        if seq < 0 or seq + bsz > self.batch:
+            raise ValueError(f"prefill of {bsz} sequences into cache sequences [{seq}, {seq + bsz}): the caches hold [0, {self.batch})")
+        if past_len < 0 or past_len + q_len > self.max_seq:
+            raise ValueError(f"prefill of {q_len} tokens at past_len {past_len}: rows [{past_len}, {past_len + q_len}) do not fit "
+                             f"max_seq {self.max_seq}")
+        if past_len > 0 and self.tp_size > 1:
+            raise NotImplementedError("prefill at past_len > 0 under tensor parallelism is not implemented")
         hq = self.local_heads * s.head_dim
         kvh = self.local_kv_heads
         ad = lambda i, n: (self.lora[i] or {}).get(n) if self.lora is not None else None      # (A, B) or None
         for i, L in enumerate(self.layers):
-            key_cache, value_cache = self.key_cache[i][:bsz], self.value_cache[i][:bsz]
+            key_cache, value_cache = self.key_cache[i][seq:seq + bsz], self.value_cache[i][seq:seq + bsz]
             residual = hidden
             x = cuda_ext.ext_rms_norm(hidden, L.ln1, s.eps)
             q = L.q.forward(x, ad(i, "q"))
             k = L.k.forward(x, ad(i, "k"))
             ext.rope_(q, self.sin, self.cos, past_len, self.local_heads, s.head_dim)
             ext.rope_(k, self.sin, self.cos, past_len, kvh, s.head_dim)
-            q = q.view(bsz, q_len, self.local_heads, s.head_dim).transpose(1, 2)
             k = k.view(bsz, q_len, kvh, s.head_dim).transpose(1, 2)
             v = L.v.forward(x, ad(i, "v")).view(bsz, q_len, kvh, s.head_dim).transpose(1, 2)
             key_cache.narrow(2, past_len, q_len).copy_(k)
             value_cache.narrow(2, past_len, q_len).copy_(v)
-            keys = repeat_kv(key_cache.narrow(2, 0, past_len + q_len), self.n_rep)
-            values = repeat_kv(value_cache.narrow(2, 0, past_len + q_len), self.n_rep)
             if past_len > 0:
-                raise NotImplementedError("chunked prefill with past is outside the benchmarked path")
-            attn = torch.nn.functional.scaled_dot_product_attention(q, keys, values, attn_mask=None, is_causal=True)
-            attn = attn.transpose(1, 2).reshape(bsz, q_len, hq)
+                # one kernel over the cache in place instead of repeat_kv + the additive mask + SDPA (csrc/prefill_attn.cu): q stays
+                # [bsz, q_len, heads, hd] as rope_ left it, and the output is already o_proj's input layout
+                attn = torch.empty((bsz, q_len, hq), dtype=torch.float16, device=self.device)
+                ext.prefill_attn(q, key_cache, value_cache, attn, self.local_heads, kvh, s.head_dim, past_len, self.max_seq)
+            else:
+                q = q.view(bsz, q_len, self.local_heads, s.head_dim).transpose(1, 2)
+                keys = repeat_kv(key_cache.narrow(2, 0, past_len + q_len), self.n_rep)
+                values = repeat_kv(value_cache.narrow(2, 0, past_len + q_len), self.n_rep)
+                attn = torch.nn.functional.scaled_dot_product_attention(q, keys, values, attn_mask=None, is_causal=True)
+                attn = attn.transpose(1, 2).reshape(bsz, q_len, hq)
             o = L.o.forward(self._o_input(attn.view(-1, hq)).view(bsz, q_len, hq), ad(i, "o"))
             if self.tp_size > 1:
                 tpmod.all_reduce(o, self.tp_group)

@@ -163,6 +163,28 @@ int exl_q4_mlp(void* x, const void* rms_norm_weight, float epsilon,
 int exl_decode_attn(const void* q, const void* key_cache, const void* value_cache, void* out,
                     int num_heads, int num_kv_heads, int head_dim, int seq_len, int max_seq_len, void* stream);
 
+/* Causal attention of a chunk of q_len new tokens over the KV cache, read in place (exllama_b200/csrc/prefill_attn.cu).  Replaces
+   repeat_kv + the additive causal mask + scaled_dot_product_attention of ExLlamaAttention.forward (model.py:447-493, mask
+   model.py:1016-1018), at any past_len.  Token t of sequence b sits at absolute position past_len + t and attends rows
+   [0, past_len + t] of its cache sequence:
+     out[b, t, h, :] = softmax_j(q[b, t, h] . K[b, kvh(h), j] / sqrt(128)) . V[b, kvh(h), j],  j in [0, past_len + t],
+     kvh(h) = h / (num_heads / num_kv_heads)
+   Layouts (fp16, contiguous):
+     q           [bsz, q_len, num_heads, 128]   the q projection after rope, as prefill holds it
+     out         [bsz, q_len, num_heads * 128]  o_proj's input
+     key_cache / value_cache  the first of bsz consecutive sequences of a [*, num_kv_heads, max_seq_len, 128] cache (a caller may
+                 pass sequence seq's slice of a larger cache)
+   Preconditions: cache rows [past_len, past_len + q_len) of the bsz sequences already hold this chunk's k / v.
+   Guarantees: reads only cache rows [0, past_len + q_len) of the bsz sequences (rows past them may hold anything, NaN
+   included); writes only out; no programmatic dependent launch, so ordinary stream order is all it needs; no atomics, so two
+   launches give bitwise equal results.  Scores, softmax and accumulators are fp32, P is rounded to fp16 for the P . V product,
+   the output is rounded to fp16 once.
+   EXL_ERR_ARG (the message names the value) for head_dim != 128, num_kv_heads not dividing num_heads, bsz < 1, q_len < 1,
+   past_len < 0, past_len + q_len > max_seq_len, or a NULL pointer. */
+int exl_prefill_attn(const void* q, const void* key_cache, const void* value_cache, void* out,
+                     int bsz, int q_len, int num_heads, int num_kv_heads, int head_dim,
+                     int past_len, int max_seq_len, void* stream);
+
 /* --- whole decode step as ONE persistent kernel (SURVEY.md 8f-4 "host loop"; 8f-2 lm_head + final norm) ------------- */
 
 /* Everything ExLlama.forward does for one new token of one sequence (model.py:1053-1077: per layer ExLlamaAttention.fused

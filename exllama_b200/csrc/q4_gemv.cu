@@ -17,11 +17,15 @@
 //  * the contraction runs on the integer tensor cores (mma.sync m16n8k32 u8 x s8/u8 -> s32, SASS IMMA.16832) with
 //    the *nibbles as the A operand straight from registers* (two ops per 8 weights: w & 0x0f0f0f0f, (w >> 4) & ...)
 //    and the <= 8 activation rows as the n = 8 operand, so the unpack costs 3/8 instruction per weight and the cost
-//    is independent of M for M <= 8.  x is carried per quantisation group as a 16-bit integer with its own scale
+//    is independent of M for M <= 8.  x is carried per segment (below) as a 16-bit integer with its own scale
 //    (two byte planes), the zero point becomes one multiply per group (zp * sum x_q), and everything inside a
 //    group is exact integer arithmetic; groups are combined in fp32 with the fp16 group scales.
-//    Quantising x to 16 bits per group costs < 1e-4 of the output rms -- below the fp16 rounding of the result
-//    (the reference accumulates in fp16, matrix.cuh:87-133).
+//    A segment of x is the quantisation group, cut at each 128-k ring stage (groups of 256 k and more, or a single group), so an
+//    outlier channel coarsens at most 128 k of x, as in decode_step.cu.  Rounding x to 16 bits moves each x by at most half a
+//    step, absmax(segment) / 65534, so an output moves by at most sum_k absmax(segment of k) / 65534 * |w_kn| plus fp32 and its
+//    final fp16 rounding (tests/helpers.py quant_error_bound, proved against an emulation of this kernel in
+//    tests/test_quant_bound.py, checked on the GPU in test_gpu_quant_edges.py).  On Gaussian x that worst case is ~1e-3 of the
+//    output rms at K = 1024, and the actual error (a sum of independent roundings) stays below 1e-4 of it.
 //  * split-K without global memory: one thread-block CLUSTER owns one 128-column tile; its CS CTAs take contiguous
 //    K slices and the leader sums the CS partials out of its own shared memory, where the peers deposited them
 //    through DSMEM with st.async (the stores complete transaction bytes on an mbarrier of the leader, so no
@@ -57,7 +61,7 @@ constexpr int STAGE_BYTES = WN * BOX_BYTES;  // 8 KB
 constexpr int NST = GV_NST;
 static_assert(NST % 2 == 0, "the two k-warp groups alternate ring stages");
 constexpr int RED_LD = GV_TILE_N + 4;
-constexpr int GMAXC = GV_GMAXC;                  // max quantisation groups staged per chunk
+constexpr int GMAXC = GV_GMAXC;                  // max quantisation groups / x segments staged per chunk
 constexpr int SC_ROW = GV_TILE_N * 2;      // bytes of scales per group row in smem
 constexpr int ZQ_ROW = GV_TILE_N / 2;      // bytes of packed zeros per group row in smem (raw, as TMA delivers them)
 constexpr int SEG_BYTES = GMAXC * GV_MAXM * 16;  // per (segment, token): {sum of x_q over even ring stages, over odd ring stages, x scale, -}
@@ -171,7 +175,7 @@ struct Accum
     uint32_t zp4;        // segment's zero points + 1, one byte per column
     int sxq[2];          // per token (2t, 2t+1): sum of x_q over the part of the segment this k-warp accumulates
     float sxs[2];        // per token: x scale of the segment
-    int cur_grp;
+    int cur_grp;         // key of the open segment (unit >> segment shift), -1: none
     bool fresh;          // integer accumulators are logically zero: the next MMA starts from C = 0
 };
 
@@ -187,15 +191,15 @@ __device__ __forceinline__ void seg_flush(Accum& A)
     A.fresh = true;
 }
 
-__device__ __forceinline__ void group_switch(Accum& A, int grp, int g_lo, uint32_t sc_addr, uint32_t zq_addr, uint32_t seg_addr,
+// key: the new segment; gl: its group's row of the staged scales / zeros; sl: its row of the segment table
+__device__ __forceinline__ void group_switch(Accum& A, int key, int gl, int sl, uint32_t sc_addr, uint32_t zq_addr, uint32_t seg_addr,
                                              int lane_col, int t, int par)
 {
     if (A.cur_grp >= 0) seg_flush(A);
-    const int gl = grp - g_lo;
     uint2 sc; uint32_t zw; uint4 s0, s1;
     asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(sc.x), "=r"(sc.y) : "r"(sc_addr + gl * SC_ROW + lane_col * 2));
     asm volatile("ld.shared.u32 %0, [%1];" : "=r"(zw) : "r"(zq_addr + gl * ZQ_ROW + (lane_col >> 3) * 4));
-    const uint32_t ea = seg_addr + (gl * GV_MAXM + 2 * t) * 16;
+    const uint32_t ea = seg_addr + (sl * GV_MAXM + 2 * t) * 16;
     asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(s0.x), "=r"(s0.y), "=r"(s0.z), "=r"(s0.w) : "r"(ea));
     asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(s1.x), "=r"(s1.y), "=r"(s1.z), "=r"(s1.w) : "r"(ea + 16));
     const half2 s01 = *reinterpret_cast<const half2*>(&sc.x);
@@ -206,7 +210,7 @@ __device__ __forceinline__ void group_switch(Accum& A, int grp, int g_lo, uint32
     A.zp4 = ((z4 & 0xfu) | ((z4 & 0xf0u) << 4) | ((z4 & 0xf00u) << 8) | ((z4 & 0xf000u) << 12)) + 0x01010101u;
     A.sxq[0] = (int)(par ? s0.y : s0.x); A.sxs[0] = __uint_as_float(s0.z);
     A.sxq[1] = (int)(par ? s1.y : s1.x); A.sxs[1] = __uint_as_float(s1.z);
-    A.cur_grp = grp;
+    A.cur_grp = key;
 }
 
 // Quantise one staged k8-row (8 halves, natural order) with scale 1/inv: returns sum of x_q and the packed byte planes
@@ -329,6 +333,9 @@ __global__ void __launch_bounds__(THREADS, GV_MINB) q4_gemv_kernel(const __grid_
     const int item = blockIdx.x / cs;
     constexpr int NSUB = (EPI == GV_EPI_SILU_MUL) ? 2 : 1;
     const int k8_lim = K >> 3;
+    // x segments: a unit (4 k8-rows = 32 k) belongs to segment unit >> sshift and to group unit >> gs_shift32; a segment is the
+    // group when the group fits a ring stage (32, 64, 128 k), else one stage of it (4 units)
+    const int sshift = min(a.gs_shift32, 2), gdiff = a.gs_shift32 - sshift;
     const int sg0 = rank * spt / cs, sg1 = (rank + 1) * spt / cs;       // this CTA's K slice, in ring stages
 
     if (tid == 0) {
@@ -426,6 +433,7 @@ __global__ void __launch_bounds__(THREADS, GV_MINB) q4_gemv_kernel(const __grid_
             const int c1 = min(sg1, c0 + a.chunk_stages);
             const int g_lo = a.groups == 1 ? 0 : ((c0 * 4) >> a.gs_shift32);
             const int g_hi = a.groups == 1 ? 0 : min(a.groups - 1, ((c1 * 4 - 1) >> a.gs_shift32));
+            const int s_lo = (c0 * 4) >> sshift;                 // first segment of the chunk (segments of 4 << sshift k8-rows)
 
             consumer_sync();                 // previous chunk / sub-tile finished with sc_s, zq_s, xs, red
             // ---- scales / zeros of groups [g_lo, g_hi] for this tile's columns: TMA bulk copies onto sc_bar ----
@@ -517,67 +525,36 @@ __global__ void __launch_bounds__(THREADS, GV_MINB) q4_gemv_kernel(const __grid_
             };
             // ---- quantise each (token, segment) of x to 16-bit integers with its own scale ----
             if (!reuse_x) {
-                const int nseg = g_hi - g_lo + 1;
-                const int rows_lo = c0 * STAGE_ROWS, rows_hi = min(c1 * STAGE_ROWS, k8_lim);
+                // a segment is rpg (4, 8 or 16) consecutive rows inside one ring stage -- the quantisation group, cut at the stage for
+                // groups of 256 k and more (and for a single group), so one outlier coarsens at most 128 k of x: one thread per row,
+                // max / sum over the segment with width-rpg shuffles (nrows and the thread count are multiples of rpg)
+                const int nseg = ((c1 * 4 - 1) >> sshift) - s_lo + 1;
                 const int nrows = (c1 - c0) * STAGE_ROWS;
-                const int rpg = a.groups > 1 ? (4 << a.gs_shift32) : (1 << 30);       // k8-rows per quantisation group
+                const int rpg = 4 << sshift;                                             // k8-rows per segment
                 uint4* table = reinterpret_cast<uint4*>(seg_s);
                 for (int idx = tid; idx < nseg * (GV_MAXM - M); idx += CONSUMERS)       // unused tokens: scale 0
                     table[(idx / (GV_MAXM - M)) * GV_MAXM + M + idx % (GV_MAXM - M)] = make_uint4(0, 0, 0, 0);
-                if (rpg <= STAGE_ROWS) {
-                    // a segment is rpg (4, 8 or 16) consecutive rows inside one ring stage: one thread per row,
-                    // max / sum over the segment with width-rpg shuffles (nrows and the thread count are multiples of rpg)
-                    for (int base = 0; base < M * nrows; base += CONSUMERS) {
-                        const int idx = base + tid;
-                        const bool act = idx < M * nrows;
-                        const int m = act ? idx / nrows : 0, rr = act ? idx - m * nrows : 0;
-                        uint4* rp = reinterpret_cast<uint4*>(xs + (size_t)m * a.xs_stride + (size_t)rr * 16);
-                        const uint4 hv = act ? stage_row(m, rr) : make_uint4(0, 0, 0, 0);      // straight from registers: no fp16 round trip
-                        float mx = row_absmax(hv);
-                        for (int o = rpg >> 1; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-                        uint4 q;
-                        int sum = quantise_row(hv, mx > 0.f ? 32767.0f / mx : 0.f, q);
-                        for (int o = rpg >> 1; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-                        if (act) {
-                            *rp = q;
-                            const int r = rows_lo + rr;                       // absolute k8-row
-                            if ((r & (rpg - 1)) == 0) {
-                                const int gi = r / rpg - g_lo;
-                                const int par = (r / STAGE_ROWS - sg0) & 1;             // parity of the stage inside this CTA's slice
-                                table[gi * GV_MAXM + m] = make_uint4(par ? 0u : (uint32_t)sum, par ? (uint32_t)sum : 0u,
-                                                                     __float_as_uint(mx * (1.0f / 32767.0f)), 0u);
-                            }
+                const int rows_lo = c0 * STAGE_ROWS;
+                for (int base = 0; base < M * nrows; base += CONSUMERS) {
+                    const int idx = base + tid;
+                    const bool act = idx < M * nrows;
+                    const int m = act ? idx / nrows : 0, rr = act ? idx - m * nrows : 0;
+                    uint4* rp = reinterpret_cast<uint4*>(xs + (size_t)m * a.xs_stride + (size_t)rr * 16);
+                    const uint4 hv = act ? stage_row(m, rr) : make_uint4(0, 0, 0, 0);      // straight from registers: no fp16 round trip
+                    float mx = row_absmax(hv);
+                    for (int o = rpg >> 1; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+                    uint4 q;
+                    int sum = quantise_row(hv, mx > 0.f ? 32767.0f / mx : 0.f, q);
+                    for (int o = rpg >> 1; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+                    if (act) {
+                        *rp = q;
+                        const int r = rows_lo + rr;                       // absolute k8-row
+                        if ((r & (rpg - 1)) == 0) {
+                            const int si = r / rpg - s_lo;
+                            const int par = (r / STAGE_ROWS - sg0) & 1;             // parity of the stage inside this CTA's slice
+                            table[si * GV_MAXM + m] = make_uint4(par ? 0u : (uint32_t)sum, par ? (uint32_t)sum : 0u,
+                                                                 __float_as_uint(mx * (1.0f / 32767.0f)), 0u);
                         }
-                    }
-                } else {
-                    // large groups (groupsize >= 256 or a single group): stage fp16 first, then one warp per (segment, token)
-                    for (int idx = tid; idx < M * nrows; idx += CONSUMERS) {
-                        const int m = idx / nrows, j = idx - m * nrows;
-                        *reinterpret_cast<uint4*>(xs + (size_t)m * a.xs_stride + (size_t)j * 16) = stage_row(m, j);
-                    }
-                    consumer_sync();
-                    for (int task = warp; task < nseg * M; task += CONSUMERS / 32) {
-                        const int gi = task / M, m = task - gi * M;
-                        int r_lo = rows_lo, r_hi = rows_hi;
-                        if (a.groups > 1) { r_lo = max(rows_lo, (g_lo + gi) * rpg); r_hi = min(rows_hi, (g_lo + gi + 1) * rpg); }
-                        unsigned char* xrow_p = xs + (size_t)m * a.xs_stride;
-                        float mx = 0.f;
-                        for (int r = r_lo + lane; r < r_hi; r += 32)
-                            mx = fmaxf(mx, row_absmax(*reinterpret_cast<const uint4*>(xrow_p + (size_t)(r - rows_lo) * 16)));
-                        #pragma unroll
-                        for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-                        const float inv = mx > 0.f ? 32767.0f / mx : 0.f;
-                        int sum0 = 0, sum1 = 0;
-                        for (int r = r_lo + lane; r < r_hi; r += 32) {
-                            uint4* rp = reinterpret_cast<uint4*>(xrow_p + (size_t)(r - rows_lo) * 16);
-                            uint4 q;
-                            const int sm = quantise_row(*rp, inv, q);
-                            *rp = q;
-                            if ((r / STAGE_ROWS - sg0) & 1) sum1 += sm; else sum0 += sm;
-                        }
-                        #pragma unroll
-                        for (int o = 16; o > 0; o >>= 1) { sum0 += __shfl_xor_sync(0xffffffffu, sum0, o); sum1 += __shfl_xor_sync(0xffffffffu, sum1, o); }
-                        if (lane == 0) table[gi * GV_MAXM + m] = make_uint4((uint32_t)sum0, (uint32_t)sum1, __float_as_uint(mx * (1.0f / 32767.0f)), 0u);
                     }
                 }
             }
@@ -602,19 +579,19 @@ __global__ void __launch_bounds__(THREADS, GV_MINB) q4_gemv_kernel(const __grid_
             int slot = (jbase + (sg - sg0)) % NST;
             uint32_t phase = (uint32_t)((jbase + (sg - sg0)) / NST) & 1u;
             uint32_t xb = xa0 + (uint32_t)(sg - c0) * (STAGE_ROWS * 16);
+            #define GV_SEG_SWITCH(U_)                                                                  \
+                const int key = (u0 + U_) >> sshift;                                                   \
+                if (key != A.cur_grp) group_switch(A, key, (key >> gdiff) - g_lo, key - s_lo, sc_a, zq_a, seg_a, lane_col, t, rel_par);
             #define GV_UNIT_CHECKED(U_, W_, X_)                                                        \
                 if (((u0 + U_) * 4 + 4) <= k8_lim) {                                                   \
-                    const int grp = (u0 + U_) >> a.gs_shift32;                                         \
-                    if (grp != A.cur_grp) group_switch(A, grp, g_lo, sc_a, zq_a, seg_a, lane_col, t, rel_par); \
+                    GV_SEG_SWITCH(U_)                                                                  \
                     unit_mma(A, W_, X_);                                                               \
                 }
             #define GV_UNIT_FAST(U_, W_, X_)                                                           \
                 {                                                                                      \
-                    const int grp = (u0 + U_) >> gshift;                                               \
-                    if (grp != A.cur_grp) group_switch(A, grp, g_lo, sc_a, zq_a, seg_a, lane_col, t, rel_par); \
+                    GV_SEG_SWITCH(U_)                                                                  \
                     unit_mma(A, W_, X_);                                                               \
                 }
-            const int gshift = a.gs_shift32;
             for (; sg < c1; sg += 2) {
                 mbar_wait_a(full0 + slot * 8, phase);
                 if (!skip_math) {
@@ -647,6 +624,7 @@ __global__ void __launch_bounds__(THREADS, GV_MINB) q4_gemv_kernel(const __grid_
                 slot += 2;
                 if (slot >= NST) { slot -= NST; phase ^= 1u; }
             }
+            #undef GV_SEG_SWITCH
             #undef GV_UNIT_CHECKED
             #undef GV_UNIT_FAST
             // x scales are per (segment, chunk): close the open segment before the staging buffers are recycled
@@ -931,9 +909,11 @@ int exl_gemv_launch(ExlDevice* ds, const half* x, int M, const exl_q4_matrix* co
     }
     a.num_mats = num_mats;
     a.no_zero = no_zero ? 1 : 0;
-    // staging chunk: M * chunk_k * 2 bytes of x <= XS_BUDGET, and at most GMAXC quantisation groups
+    // staging chunk: M * chunk_k * 2 bytes of x <= XS_BUDGET, and fewer than GMAXC x segments (a segment is the group, at most one
+    // 128-k stage of it)
     int chunk_k = XS_BUDGET / (2 * M);
-    if (w0->groups > 1) { int gk = (GMAXC - 1) * w0->groupsize; if (gk < chunk_k) chunk_k = gk; }
+    const int seg_k = (w0->groups > 1 && w0->groupsize < STAGE_K) ? w0->groupsize : STAGE_K;
+    if ((GMAXC - 1) * seg_k < chunk_k) chunk_k = (GMAXC - 1) * seg_k;
     int chunk_stages = chunk_k / STAGE_K;
     if (chunk_stages < 1) return exl_set_err(EXL_ERR_ARG, "q4_gemv: cannot stage a chunk (groupsize %d)", w0->groupsize);
     if (chunk_stages > a.spt) chunk_stages = a.spt;

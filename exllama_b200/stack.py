@@ -53,7 +53,7 @@ class _Arena:
 
     @staticmethod
     def q4_bytes(K, N, groupsize):
-        G = K // groupsize
+        G = 1 if groupsize is None else K // groupsize
         r = lambda b: (b + 255) & ~255
         return r(K // 8 * N * 4) + r(G * (N // 8) * 4) + r(G * N * 2)
 
@@ -64,7 +64,7 @@ def synth_q4_device(K, N, groupsize, device, gen, act_order=False, scale_lo=None
     symmetric weight groups.  A mean offset of even one quantisation step gives every matrix a DC gain of ~scale * K >> 1 and a
     deep synthetic stack then blows up through its DC mode -- measured: 33B overflowed fp16 within a few layers), and scales sized
     for a per-layer gain below one whatever K is (std(q - z) ~ 4.6, so gain = 4.6 * mean(scale) * sqrt(K) ~ 0.4)."""
-    G = K // groupsize
+    G = 1 if groupsize is None else K // groupsize
     if scale_hi is None:
         scale_hi = 2.3e-3 * (4096.0 / K) ** 0.5
     if scale_lo is None:
@@ -86,7 +86,7 @@ def synth_q4_device(K, N, groupsize, device, gen, act_order=False, scale_lo=None
     if act_order:
         perm = torch.randperm(K, device=device, generator=gen)
         g_idx = torch.empty(K, dtype=torch.int32, device=device)
-        g_idx[perm] = (torch.arange(K, device=device) // groupsize).int()
+        g_idx[perm] = 0 if groupsize is None else (torch.arange(K, device=device) // groupsize).int()
         g_idx = g_idx.cpu()
     return qweight, qzeros, scales, g_idx
 
@@ -131,7 +131,10 @@ class DecodeStack:
         self.o_rows = None
         if shape.kv_heads != shape.heads and tp_size > 1:
             raise NotImplementedError("grouped-query attention under tensor parallelism (KV-head sharding) is not implemented")
-        plan = tpmod.plan_shards(shape.hidden, shape.inter, shape.heads, shape.head_dim, groupsize, tp_size)
+        if groupsize is None and tp_size > 1:
+            raise NotImplementedError("one quantisation group per matrix (groupsize None) under tensor parallelism is not implemented")
+        # groupsize None: one group per matrix, so a single rank's plan takes the whole intermediate width as one unit
+        plan = tpmod.plan_shards(shape.hidden, shape.inter, shape.heads, shape.head_dim, groupsize or shape.inter, tp_size)
         self.plan = plan
         h = shape.hidden
         self.local_heads = plan.heads[tp_rank]

@@ -99,6 +99,208 @@ def oracle_decode_step(oracle, st, snap, x, past, seq=0):
     return x, hn.astype(np.float64) @ _np(st.lm_head).astype(np.float64).T, rows
 
 
+def q4_column_sample(qweight, qzeros, scales, cols):
+    """(qweight, qzeros, scales) of the output columns `cols` (whole groups of 8, ascending): an exact restriction of the matrix, so
+    the float64 oracle can check a sample of a matrix too wide to contract in full."""
+    cols = np.asarray(cols)
+    G = qzeros.shape[0]
+    sub_qw = np.ascontiguousarray(qweight[:, cols]); sub_sc = np.ascontiguousarray(scales[:, cols])
+    zfull = ((qzeros.view(np.uint32)[:, :, None] >> (np.arange(8, dtype=np.uint32) * 4)[None, None]) & 0xF).reshape(G, -1)
+    zsub = zfull[:, cols].reshape(G, -1, 8)
+    sub_qz = (zsub.astype(np.uint32) << (np.arange(8, dtype=np.uint32) * 4)).sum(-1).astype(np.uint32).view(np.int32)
+    return sub_qw, np.ascontiguousarray(sub_qz), sub_sc
+
+
+def sample_cols(N, groups8, seed=0):
+    """`groups8` whole 8-column groups of an N-wide output (all columns when that covers N), ascending."""
+    if groups8 * 8 >= N:
+        return np.arange(N)
+    c = np.sort(np.random.default_rng(seed).choice(N // 8, groups8, replace=False)) * 8
+    return (c[:, None] + np.arange(8)[None]).reshape(-1)
+
+
+# ---------------------------------------------------------------------------------------------------------------------------------
+# x quantisation of the decode GEMVs: an error bound, and the inputs that stress it
+#
+# q4_gemv_kernel (q4_gemv.cu) and decode_step_kernel (decode_step.cu) carry x as a 16-bit integer per quantisation segment:
+#     x_q = rn(x * Q / absmax(segment)),   x ~ x_q * absmax / Q,   Q = 32767 (q4_gemv) or 32639 (decode_step: the high byte
+#     (x_q + 128) >> 8 must fit in s8),
+# and contract x_q with the 4-bit weights exactly in int32.  In both kernels a segment lies inside one quantisation group and one
+# aligned 128-k ring stage.  Which segments a launch uses (q4_gemv also cuts them at its staging chunk and cluster slice) is the
+# launch's business; the bound below takes the largest window a segment can have, so it holds for any split.
+# ---------------------------------------------------------------------------------------------------------------------------------
+
+QUANT_Q = {"gemv": 32767, "step": 32639}
+STAGE_K = 128
+FP16_TINY = 2.0 ** -24            # smallest fp16 subnormal
+# The fp32 term.  Every fp32 rounding on the way to an output -- Q / absmax and x * (Q / absmax), the x scale absmax * (1/Q), scale
+# * x scale, (float)val and the fma of each segment, then the k-warp, cluster and atomic sums of the partials -- is a relative error
+# of at most 2^-24 of a partial no larger than (1 + 2^-22) sum_k |x_k w_kn|.  A segment costs at most 4 of them plus one addition,
+# an output sees at most one segment per window plus one per 128-k stage where a chunk or a cluster slice cuts a window, and fewer
+# than QUANT_C more in the k-warp / cluster / atomic reductions: n_fp32 = 5 * (windows + K / 128) + QUANT_C roundings in all.
+QUANT_C = 16
+
+
+def quant_windows(K, groups):
+    """Window index of every k (gathered order): the largest range of k one quantisation segment may cover, the group
+    intersected with the aligned 128-k stage."""
+    return np.arange(K) // min(K // groups, STAGE_K)
+
+
+def quant_error_bound(oracle, x, qweight, qzeros, scales, x_map=None, kind="gemv"):
+    """(B, ref64): a float64 bound B[m, n] >= |kernel - ref64| of one decode GEMV, and ref64 itself.
+
+    qweight is in the sequential layout make_q4 leaves (groups contiguous in k, oracle.make_sequential) and x is gathered through
+    x_map before the contraction, as the kernels do.
+
+        B = (1 + 2^-10) * ( sum_k A(k) / (2Q) |w_kn|  +  n_fp32 2^-24 sum_k |x_mk w_kn| )  +  2^-11 |ref|  +  2^-24
+
+    A(k) = absmax of x over the window of k (quant_windows): rounding x to the 16-bit grid costs at most half a step A / Q per
+    element.  n_fp32 (QUANT_C's comment) is 5 (K / min(gs, 128) + K / 128) + 16: about K / 5 at groups of 32, K / 13 from
+    groups of 128 up.  2^-11 |ref| + 2^-24 is the final fp16 rounding (relative for normal results,
+    absolute below 2^-14), and 1 + 2^-10 lets that rounding act on the error itself."""
+    assert kind in QUANT_Q
+    xg = np.asarray(x, np.float16).astype(np.float64)
+    if x_map is not None:
+        xg = xg[:, np.asarray(x_map, np.int64)]
+    W = oracle.dequant_f64(qweight, qzeros, scales)
+    ref = xg @ W
+    M, K = xg.shape
+    win = quant_windows(K, qzeros.shape[0])
+    starts = np.flatnonzero(np.r_[True, win[1:] != win[:-1]])
+    A = np.maximum.reduceat(np.abs(xg), starts, axis=1)[:, win]
+    aw = np.abs(W)
+    t1 = (A / (2.0 * QUANT_Q[kind])) @ aw
+    n_fp32 = 5 * (win[-1] + 1 + -(-K // STAGE_K)) + QUANT_C
+    t2 = n_fp32 * 2.0 ** -24 * (np.abs(xg) @ aw)
+    return (1 + 2.0 ** -10) * (t1 + t2) + 2.0 ** -11 * np.abs(ref) + FP16_TINY, ref
+
+
+def assert_within_bound(got_f16, bound, ref, what=""):
+    got = np.asarray(got_f16, np.float64)
+    assert np.isfinite(got).all(), f"{what}: non-finite output"
+    err = np.abs(got - ref)
+    bad = err > bound
+    i = np.unravel_index(np.argmax(err / bound), err.shape)
+    assert not bad.any(), (f"{what}: {bad.sum()} / {bad.size} outside the quantisation bound; worst at {i}: err {err[i]:.4g} > "
+                           f"bound {bound[i]:.4g} (ref {ref[i]:.4g})")
+    return float((err / bound).max())
+
+
+# ---- weights ----------------------------------------------------------------------------------------------------------------------
+
+def pack_q4(nib, znib, scales, g_idx=None):
+    """nibbles q [K, N] and stored zero nibbles z [G, N] (0..15) -> GPTQ (qweight [K/8, N], qzeros [G, N/8], scales, g_idx)."""
+    K, N = nib.shape
+    sh = np.arange(8, dtype=np.uint32) * 4
+    qw = (nib.astype(np.uint32).reshape(K // 8, 8, N) << sh[None, :, None]).sum(1, dtype=np.uint32).view(np.int32)
+    G, Nz = znib.shape
+    qz = (znib.astype(np.uint32).reshape(G, Nz // 8, 8) << sh[None, None, :]).sum(-1, dtype=np.uint32).view(np.int32)
+    return np.ascontiguousarray(qw), np.ascontiguousarray(qz), np.asarray(scales, np.float16), g_idx
+
+
+def _groups(K, gs):
+    return 1 if gs is None else K // gs
+
+
+def _g_idx(K, gs, act, rng):
+    if not act:
+        return None
+    g = np.zeros(K, np.int32) if gs is None else (np.arange(K) // gs).astype(np.int32)
+    return g[rng.permutation(K)]
+
+
+def synth_q4_ckpt(K, N, gs, act=False, seed=0, cols=None, scale=1.0, quiet_rows=(), quiet_frac=0.9, g_idx=None):
+    """Checkpoint-like GPTQ tensors (gs None = one group): stored zero nibbles 7 or 8, nibbles a discretised normal (sd 2.5)
+    around z + 1 clipped to 0..15, scales log-uniform over two decades (x `scale`) with 1 % of the columns at 30x.
+    cols: only these columns get checkpoint-like nibbles (the rest uniform), so a sampled-column check of a very wide matrix stays
+    cheap.  quiet_rows: k (original order) whose weights are exactly 0 (q = z + 1) in `quiet_frac` of the columns -- an outlier
+    channel the layer mostly ignores.  g_idx: use this act-order permutation (matrices that share one x order, e.g. q / k / v)."""
+    rng = np.random.default_rng(seed)
+    G = _groups(K, gs)
+    znib = rng.integers(7, 9, size=(G, N))
+    sc = 10.0 ** rng.uniform(-3.5, -1.5, size=(G, N)) * scale
+    sc[:, rng.random(N) < 0.01] *= 30
+    cols = np.arange(N) if cols is None else np.asarray(cols)
+    g_idx = _g_idx(K, gs, act, rng) if g_idx is None else g_idx
+    grp = (np.zeros(K, np.int64) if gs is None else np.arange(K) // gs) if g_idx is None else g_idx.astype(np.int64)
+    zc = znib[:, cols][grp] + 1
+    nc = np.clip(np.rint(zc + 2.5 * rng.standard_normal((K, len(cols)))), 0, 15)
+    for k in quiet_rows:
+        quiet = rng.random(len(cols)) < quiet_frac
+        nc[k, quiet] = zc[k, quiet]
+    qw_c, qz, sc16, _ = pack_q4(nc.astype(np.uint8), znib, sc.astype(np.float16))
+    if len(cols) == N:
+        return qw_c, qz, sc16, g_idx
+    qw = rng.integers(0, 2**32, size=(K // 8, N), dtype=np.uint32).view(np.int32)
+    qw[:, cols] = qw_c
+    return qw, qz, sc16, g_idx
+
+
+def synth_q4_saturated(K, N, gs, sign=-1, scales=None, act=False, seed=0):
+    """Every weight at the end of the 4-bit range: sign -1 = nibble 0 with zero nibble 15 (q - z - 1 = -16), sign +1 = nibble 15
+    with zero nibble 0 (q - z - 1 = +14).  The packed words are built directly (all nibbles equal), so 70B widths stay cheap."""
+    rng = np.random.default_rng(seed)
+    G = _groups(K, gs)
+    wq, wz = (0, -1) if sign < 0 else (-1, 0)                       # -1 = 0xffffffff: eight nibbles of 15
+    if scales is None:
+        scales = 10.0 ** rng.uniform(-3, -2, size=(G, N))
+    return (np.full((K // 8, N), wq, np.int32), np.full((G, N // 8), wz, np.int32), np.asarray(scales, np.float16),
+            _g_idx(K, gs, act, rng))
+
+
+# ---- activations ------------------------------------------------------------------------------------------------------------------
+
+def outlier_channels(K, gs, variant):
+    """Channels for the outlier generator (gs None = one group): variant 0 = the first k of a group, stage and chunk; 1 = the last k
+    of a group and the first of the next stage; 2 = three channels in one group; 3 = the last k of the first 8192-k staging chunk
+    and the last k of the matrix; 4 = one channel inside a group, one in another group."""
+    g = K if gs is None else gs
+    c = {0: [0],
+         1: [g - 1, min(K - 1, 128 if g > 128 else g)],
+         2: [min(g - 1, 5), min(g - 1, 77), min(g - 1, 126)],
+         3: [min(K, 8192) - 1, K - 1],
+         4: [g // 3, min(K - 1, g + g // 2 + 1)]}[variant]
+    return sorted(set(c))
+
+
+X_KINDS = ("gauss", "outlier64", "outlier1000", "silu", "zeros", "const", "big", "subnormal")
+
+
+def gen_x(kind, M, K, seed=0, channels=(0,), gs=None):
+    """Seeded fp16 activations [M, K] for the quantisation edges:
+    gauss: standard normal;  outlier64 / outlier1000: standard normal with `channels` at +-64 / +-1000 (signs alternate by row);
+    silu: silu(g) * u with g ~ N(1, 1.5), u ~ N(0.3, 1) (sign-biased, as the input of down_proj);  zeros: row 0 all zero (M > 1) and,
+    in the last row, an all-zero group (the group of k = 0 when gs is None: the first 128 k);  const: every row constant (its own
+    value), so every x_q is +-Q and quantisation is exact;  big: N(0, 100) with absmax 60000 (pair it with weights scaled down so
+    the output stays finite);  subnormal: random fp16 subnormals."""
+    rng = np.random.default_rng(seed)
+    x = rng.standard_normal((M, K))
+    if kind.startswith("outlier"):
+        mag = float(kind[len("outlier"):])
+        for m in range(M):
+            for j, c in enumerate(channels):
+                x[m, c] = mag * (1 if (m + j) % 2 == 0 else -1)
+    elif kind == "silu":
+        g = 1 + 1.5 * x
+        x = g / (1 + np.exp(-g)) * (0.3 + rng.standard_normal((M, K)))
+    elif kind == "zeros":
+        if M > 1:
+            x[0] = 0
+        w = 128 if gs is None else gs
+        x[M - 1, :w] = 0
+    elif kind == "const":
+        x = np.repeat(rng.choice([-1, 1], M)[:, None] * rng.uniform(0.1, 3, (M, 1)), K, axis=1)
+    elif kind == "big":
+        x = 100 * x
+        x[np.arange(M), rng.integers(0, K, M)] = 60000 * rng.choice([-1, 1], M)
+    elif kind == "subnormal":
+        x = rng.integers(-1023, 1024, (M, K)) * 2.0 ** -24
+    else:
+        assert kind == "gauss", kind
+    return x.astype(np.float16)
+
+
 def to_cuda(*arrays):
     import torch
     out = []

@@ -6,7 +6,7 @@ import os
 import numpy as np
 import pytest
 
-from helpers import GOLDEN, assert_close_ref64, golden_cols, to_cuda
+from helpers import GOLDEN, assert_close_ref64, golden_cols, q4_column_sample, sample_cols, to_cuda
 
 pytestmark = pytest.mark.gpu
 
@@ -98,14 +98,10 @@ def test_full_size_7b_shapes_linearity(oracle):
         y1 = capi.q4_matmul(to_cuda(x1), q4).float(); y2 = capi.q4_matmul(to_cuda(x2), q4).float()
         ys = capi.q4_matmul(to_cuda(xs), q4).float()
         # xs was rounded to fp16: compare against W applied to the rounded sum via the column sample instead
-        cols = np.sort(np.random.default_rng(0).choice(N // 8, 24, replace=False)) * 8
-        cols = (cols[:, None] + np.arange(8)[None]).reshape(-1)
-        sub_qw = np.ascontiguousarray(qw[:, cols]); sub_sc = np.ascontiguousarray(sc[:, cols])
-        zfull = ((qz.view(np.uint32)[:, :, None] >> (np.arange(8, dtype=np.uint32) * 4)[None, None]) & 0xF).reshape(K // gs, N)
-        zsub = zfull[:, cols].reshape(K // gs, -1, 8)
-        sub_qz = (zsub.astype(np.uint32) << (np.arange(8, dtype=np.uint32) * 4)).sum(-1).astype(np.uint32).view(np.int32)
+        cols = sample_cols(N, 24, seed=0)
+        sub = q4_column_sample(qw, qz, sc, cols)
         for xv, yv in ((x1, y1), (x2, y2), (xs, ys)):
-            ref = oracle.q4_matmul_f64(xv, sub_qw, sub_qz, sub_sc)
+            ref = oracle.q4_matmul_f64(xv, *sub)
             assert_close_ref64(yv.cpu().numpy()[:, cols], ref, what=f"col-sample K{K} N{N}")
         rms = float(ys.pow(2).mean().sqrt())
         assert float((y1 + y2 - ys).abs().max()) <= 0.02 * rms + 4e-3 * float(ys.abs().max())

@@ -15,6 +15,20 @@ _lib = None
 
 vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_int64, C.c_float
 
+
+class ExlRagged(C.Structure):
+    """exl_ragged: n_seq sequences, host arrays of q_len, past_len and cache_seq."""
+    _fields_ = [("n_seq", i32), ("q_len", C.POINTER(i32)), ("past_len", C.POINTER(i32)), ("cache_seq", C.POINTER(i32))]
+
+
+def ragged(q_lens, past_lens, cache_seqs):
+    """An ExlRagged over host copies of the three lists (the arrays stay alive with the returned structure)."""
+    n = len(q_lens)
+    arrs = [(i32 * n)(*[int(v) for v in a]) for a in (q_lens, past_lens, cache_seqs)]
+    r = ExlRagged(n, *[C.cast(a, C.POINTER(i32)) for a in arrs])
+    r._keep = arrs
+    return r
+
 # name -> (restype, argtypes); mirrors include/exl_b200.h one to one
 SIGNATURES = {
     "exl_last_error": (C.c_char_p, []),
@@ -42,6 +56,8 @@ SIGNATURES = {
     "exl_tp_status": (i32, [i32, C.POINTER(C.c_uint)]),
     "exl_decode_attn": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, vp]),
     "exl_prefill_attn": (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp]),
+    "exl_prefill_attn_ragged": (i32, [vp, vp, vp, vp, C.POINTER(ExlRagged), i32, i32, i32, i32, i32, vp]),
+    "exl_rope_cache_ragged": (i32, [vp, vp, vp, vp, vp, vp, vp, C.POINTER(ExlRagged), i32, i32, i32, i32, i32, vp]),
     "exl_q4_attn_2_tp": (i32, [vp, vp, vp, i32, i32, vp]),
     "exl_tp_workspace_alloc": (i32, [i32, C.POINTER(vp), vp]),
     "exl_tp_workspace_open": (i32, [i32, vp, C.POINTER(vp)]),
@@ -217,6 +233,29 @@ def prefill_attn(q, key_cache, value_cache, num_heads, num_kv_heads, head_dim, p
     check(lib().exl_prefill_attn(_ptr(q), _ptr(key_cache), _ptr(value_cache), _ptr(out), bsz, q_len, num_heads, num_kv_heads, head_dim,
                                  past_len, max_seq_len, _stream()))
     return out
+
+
+def prefill_attn_ragged(q, key_cache, value_cache, q_lens, past_lens, cache_seqs, num_heads, num_kv_heads, head_dim, max_seq_len,
+                        out=None):
+    """q half [T, num_heads, head_dim] (the sequences' tokens packed in order) -> out half [T, num_heads * head_dim]: causal
+    attention of sequence i's tokens at positions [past_lens[i], past_lens[i] + q_lens[i]) over cache sequence cache_seqs[i] of
+    caches [num_cache_seqs, num_kv_heads, max_seq_len, head_dim] (include/exl_b200.h exl_prefill_attn_ragged)."""
+    import torch
+    if out is None:
+        out = torch.empty((q.shape[0], num_heads * head_dim), dtype=torch.float16, device=q.device)
+    r = ragged(q_lens, past_lens, cache_seqs)
+    check(lib().exl_prefill_attn_ragged(_ptr(q), _ptr(key_cache), _ptr(value_cache), _ptr(out), C.byref(r), key_cache.shape[0],
+                                        num_heads, num_kv_heads, head_dim, max_seq_len, _stream()))
+    return out
+
+
+def rope_cache_ragged(q, k, v, key_cache, value_cache, sin, cos, q_lens, past_lens, cache_seqs, num_heads, num_kv_heads, head_dim,
+                      max_seq_len):
+    """Rope q [T, num_heads, head_dim] and k [T, num_kv_heads, head_dim] in place at each token's position and write k and v into
+    rows past_lens[i] + t of cache sequence cache_seqs[i] (include/exl_b200.h exl_rope_cache_ragged)."""
+    r = ragged(q_lens, past_lens, cache_seqs)
+    check(lib().exl_rope_cache_ragged(_ptr(q), _ptr(k), _ptr(v), _ptr(key_cache), _ptr(value_cache), _ptr(sin), _ptr(cos), C.byref(r),
+                                      key_cache.shape[0], num_heads, num_kv_heads, head_dim, max_seq_len, _stream()))
 
 
 def prepare_buffers(device, temp_state, temp_mlp, temp_zeros_float, temp_dq):

@@ -76,8 +76,8 @@ int exl_own_scratch(ExlDevice* ds, int role, int64_t numel, half** out)
 extern "C" {
 
 const char* exl_last_error(void) { return t_err; }
-int exl_version(void) { return 104; }             // 101: exl_decode_desc.num_kv_heads; 102: batched decode plans and steps; 103: LoRA plans;
-                                                  // 104: exl_prefill_attn
+int exl_version(void) { return 105; }             // 101: exl_decode_desc.num_kv_heads; 102: batched decode plans and steps; 103: LoRA plans;
+                                                  // 104: exl_prefill_attn; 105: exl_prefill_attn_ragged, exl_rope_cache_ragged
 int64_t exl_launch_count(void) { return g_launches.load(); }
 const char* exl_last_q4_path(void) { return g_last_q4_path; }
 
@@ -584,6 +584,22 @@ int exl_prefill_attn(const void* q, const void* key_cache, const void* value_cac
 {
     return exl_prefill_attn_launch((const half*)q, (const half*)key_cache, (const half*)value_cache, (half*)out, bsz, q_len, num_heads,
                                    num_kv_heads, head_dim, past_len, max_seq_len, (cudaStream_t)stream);
+}
+
+int exl_prefill_attn_ragged(const void* q, const void* key_cache, const void* value_cache, void* out, const exl_ragged* r,
+                            int num_cache_seqs, int num_heads, int num_kv_heads, int head_dim, int max_seq_len, void* stream)
+{
+    return exl_prefill_attn_ragged_launch((const half*)q, (const half*)key_cache, (const half*)value_cache, (half*)out, r, num_cache_seqs,
+                                          num_heads, num_kv_heads, head_dim, max_seq_len, (cudaStream_t)stream);
+}
+
+int exl_rope_cache_ragged(void* q, void* k, const void* v, void* key_cache, void* value_cache, const void* sin, const void* cos,
+                          const exl_ragged* r, int num_cache_seqs, int num_heads, int num_kv_heads, int head_dim,
+                          int max_seq_len, void* stream)
+{
+    return exl_rope_cache_ragged_launch((half*)q, (half*)k, (const half*)v, (half*)key_cache, (half*)value_cache, (const half*)sin,
+                                        (const half*)cos, r, num_cache_seqs, num_heads, num_kv_heads, head_dim, max_seq_len,
+                                        (cudaStream_t)stream);
 }
 
 int exl_q4_matmul_host(const void* x_host, int M, const exl_q4_matrix* w, void* out_host, void* d_x, void* d_out, void* stream_)

@@ -46,8 +46,24 @@ __global__ void __launch_bounds__(256) rms_norm_kernel(const half* __restrict__ 
     for (int i = nv * 8 + tid; i < dim; i += 256) orow[i] = __hmul(__hmul(xr[i], rm), w[i]);
 }
 
-// rotate-half RoPE in place, half2 per thread (rope.cu:48-67):
-//   l' = hfma(l, cos_l, hmul(r, -sin_l));   r' = hfma(r, cos_r, hmul(l, sin_r)),  pos = past_len + row / num_heads
+// rotate-half RoPE of half2 pair c2 of one head row at position pos (rope.cu:48-67):
+//   l' = hfma(l, cos_l, hmul(r, -sin_l));   r' = hfma(r, cos_r, hmul(l, sin_r))
+__device__ __forceinline__ void rope_rotate(half2& l, half2& r, const half* __restrict__ sin, const half* __restrict__ cos, int pos,
+                                            int c2, int head_dim)
+{
+    const int half_dim = head_dim / 2;
+    const half2 cl = reinterpret_cast<const half2*>(cos + (size_t)pos * head_dim)[c2];
+    const half2 cr = reinterpret_cast<const half2*>(cos + (size_t)pos * head_dim + half_dim)[c2];
+    half2 sl = reinterpret_cast<const half2*>(sin + (size_t)pos * head_dim)[c2];
+    const half2 sr = reinterpret_cast<const half2*>(sin + (size_t)pos * head_dim + half_dim)[c2];
+    sl = __hneg2(sl);
+    const half2 ls = __hmul2(r, sl);
+    const half2 rs = __hmul2(l, sr);
+    l = __hfma2(l, cl, ls);
+    r = __hfma2(r, cr, rs);
+}
+
+// rotate-half RoPE in place, half2 per thread, pos = past_len + row / num_heads
 __global__ void __launch_bounds__(256) rope_kernel(half* __restrict__ x, const half* __restrict__ sin, const half* __restrict__ cos,
                                                    int rows_per_batch, int head_dim, int num_heads, int past_len, long long total_pairs)
 {
@@ -58,19 +74,50 @@ __global__ void __launch_bounds__(256) rope_kernel(half* __restrict__ x, const h
     const int c2 = (int)(idx - rowg * hd4);
     const int row = (int)(rowg % rows_per_batch);
     const int pos = past_len + row / num_heads;
-    const int half_dim = head_dim / 2;
     half2* xl = reinterpret_cast<half2*>(x + rowg * head_dim) + c2;
-    half2* xr = reinterpret_cast<half2*>(x + rowg * head_dim + half_dim) + c2;
-    const half2 cl = reinterpret_cast<const half2*>(cos + (size_t)pos * head_dim)[c2];
-    const half2 cr = reinterpret_cast<const half2*>(cos + (size_t)pos * head_dim + half_dim)[c2];
-    half2 sl = reinterpret_cast<const half2*>(sin + (size_t)pos * head_dim)[c2];
-    const half2 sr = reinterpret_cast<const half2*>(sin + (size_t)pos * head_dim + half_dim)[c2];
-    sl = __hneg2(sl);
-    const half2 l = *xl, r = *xr;
-    const half2 ls = __hmul2(r, sl);
-    const half2 rs = __hmul2(l, sr);
-    *xl = __hfma2(l, cl, ls);
-    *xr = __hfma2(r, cr, rs);
+    half2* xr = reinterpret_cast<half2*>(x + rowg * head_dim + head_dim / 2) + c2;
+    half2 l = *xl, r = *xr;
+    rope_rotate(l, r, sin, cos, pos, c2, head_dim);
+    *xl = l;
+    *xr = r;
+}
+
+// the sequences of a ragged batch in packed token order: sequence s owns token rows [tok0[s], tok0[s + 1])
+struct RopeRagged { int n; int tok0[EXL_RAGGED_MAX_SEQ + 1]; int past[EXL_RAGGED_MAX_SEQ]; int cache[EXL_RAGGED_MAX_SEQ]; };
+
+// One CTA per token t of sequence s, at position pos = past[s] + t - tok0[s]: rope every q head and k head of the token in place
+// (rope_rotate, as rope_kernel), and write the roped k row and the v row into row pos of cache sequence cache[s].
+__global__ void __launch_bounds__(256) rope_cache_ragged_kernel(half* __restrict__ q, half* __restrict__ k, const half* __restrict__ v,
+                                                                half* __restrict__ kc, half* __restrict__ vc,
+                                                                const half* __restrict__ sin, const half* __restrict__ cos,
+                                                                const __grid_constant__ RopeRagged rr, int heads, int kv_heads, int max_seq)
+{
+    constexpr int HD = 128, HD4 = HD / 4;
+    const int t = blockIdx.x;
+    int s = 0;
+    while (s + 1 < rr.n && t >= rr.tok0[s + 1]) s++;
+    const int pos = rr.past[s] + t - rr.tok0[s];
+    const int pairs = (heads + kv_heads) * HD4;
+    for (int i = threadIdx.x; i < pairs; i += blockDim.x) {
+        const int h = i / HD4, c2 = i - h * HD4;
+        const bool is_k = h >= heads;
+        half2* row = reinterpret_cast<half2*>(is_k ? k + ((size_t)t * kv_heads + (h - heads)) * HD : q + ((size_t)t * heads + h) * HD);
+        half2 l = row[c2], r = row[HD4 + c2];
+        rope_rotate(l, r, sin, cos, pos, c2, HD);
+        row[c2] = l;
+        row[HD4 + c2] = r;
+        if (is_k) {
+            const int kh = h - heads;
+            const size_t dst = (((size_t)rr.cache[s] * kv_heads + kh) * max_seq + pos) * HD;
+            const half2* vrow = reinterpret_cast<const half2*>(v + ((size_t)t * kv_heads + kh) * HD);
+            half2* kd = reinterpret_cast<half2*>(kc + dst);
+            half2* vd = reinterpret_cast<half2*>(vc + dst);
+            kd[c2] = l;
+            kd[HD4 + c2] = r;
+            vd[c2] = vrow[c2];
+            vd[HD4 + c2] = vrow[HD4 + c2];
+        }
+    }
 }
 
 __device__ __forceinline__ half2 silu2(half2 x)
@@ -139,6 +186,32 @@ int exl_rope_launch(half* x, const half* sin, const half* cos, int bsz, int rows
     if (head_dim % 4 != 0) return exl_set_err(EXL_ERR_ARG, "rope: head_dim %d must be a multiple of 4", head_dim);
     rope_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(x, sin, cos, rows_per_batch, head_dim, num_heads, past_len, total);
     EXL_CHECK_LAUNCH("rope_kernel");
+    return EXL_OK;
+}
+
+int exl_rope_cache_ragged_launch(half* q, half* k, const half* v, half* kc, half* vc, const half* sin, const half* cos,
+                                 const exl_ragged* r, int num_cache_seqs, int heads, int kv_heads, int head_dim, int max_seq,
+                                 cudaStream_t stream)
+{
+    const char* who = "rope_cache_ragged";
+    if (!q || !k || !v || !kc || !vc || !sin || !cos)
+        return exl_set_err(EXL_ERR_ARG, "%s: NULL pointer (q %p, k %p, v %p, key_cache %p, value_cache %p, sin %p, cos %p)", who,
+                           (void*)q, (void*)k, (const void*)v, (void*)kc, (void*)vc, (const void*)sin, (const void*)cos);
+    if (head_dim != 128) return exl_set_err(EXL_ERR_ARG, "%s: head_dim %d != 128", who, head_dim);
+    if (heads < 1 || kv_heads < 1 || heads % kv_heads != 0)
+        return exl_set_err(EXL_ERR_ARG, "%s: num_kv_heads %d does not divide num_heads %d", who, kv_heads, heads);
+    if (const int rc = exl_ragged_validate(r, num_cache_seqs, max_seq, who)) return rc;
+    RopeRagged rr;
+    rr.n = r->n_seq;
+    long long T = 0;
+    for (int i = 0; i < r->n_seq; i++) {
+        rr.tok0[i] = (int)T; rr.past[i] = r->past_len[i]; rr.cache[i] = r->cache_seq[i];
+        T += r->q_len[i];
+    }
+    if (T > 0x7fffffffLL) return exl_set_err(EXL_ERR_ARG, "%s: %lld tokens (at most 2^31 - 1)", who, T);
+    rr.tok0[r->n_seq] = (int)T;
+    rope_cache_ragged_kernel<<<(unsigned)T, 256, 0, stream>>>(q, k, v, kc, vc, sin, cos, rr, heads, kv_heads, max_seq);
+    EXL_CHECK_LAUNCH("rope_cache_ragged_kernel");
     return EXL_OK;
 }
 

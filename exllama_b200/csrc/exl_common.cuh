@@ -149,6 +149,9 @@ bool exl_tc_gemm_supported(const exl_q4_matrix* w, int M);
 // elementwise.cu
 int exl_rms_norm_launch(const half* x, const half* w, half* out, float eps, int rows, int dim, cudaStream_t stream);
 int exl_rope_launch(half* x, const half* sin, const half* cos, int bsz, int rows_per_batch, int head_dim, int num_heads, int past_len, cudaStream_t stream);
+int exl_rope_cache_ragged_launch(half* q, half* k, const half* v, half* kc, half* vc, const half* sin, const half* cos,
+                                 const exl_ragged* r, int num_cache_seqs, int heads, int kv_heads, int head_dim, int max_seq,
+                                 cudaStream_t stream);
 int exl_silu_mul_launch(half* x, const half* y, int height, int width, cudaStream_t stream);
 int exl_update_cache_launch(const half* k, const half* v, half* kc, half* vc, int head_dim, int kvh, int q_len, int max_seq, int past_len, cudaStream_t stream);
 int exl_column_remap_launch(const half* x, half* x_new, int M, int K, const uint32_t* x_map, cudaStream_t stream);
@@ -160,6 +163,10 @@ int exl_decode_attn_launch(const half* q, const half* kc, const half* vc, half* 
 // prefill_attn.cu
 int exl_prefill_attn_launch(const half* q, const half* kc, const half* vc, half* out, int bsz, int q_len, int heads, int kv_heads,
                             int head_dim, int past_len, int max_seq, cudaStream_t stream);
+int exl_prefill_attn_ragged_launch(const half* q, const half* kc, const half* vc, half* out, const exl_ragged* r, int num_cache_seqs,
+                                   int heads, int kv_heads, int head_dim, int max_seq, cudaStream_t stream);
+// EXL_OK, or EXL_ERR_ARG naming the first bad field of r (who: the entry point named in the message)
+int exl_ragged_validate(const exl_ragged* r, int num_cache_seqs, int max_seq, const char* who);
 
 // half_matmul.cu
 int exl_half_matmul_cublas_launch(ExlDevice* ds, const half* x, const half* w, half* out, int M, int K, int N, bool no_zero, cudaStream_t stream);

@@ -9,19 +9,25 @@
 //   rows     a query tile is 64 ROWS of one KV group, row r = (token r / n_rep, query head r % n_rep of the group): under
 //            grouped-query attention the n_rep heads that share a KV head share every K/V tile, which is loaded once per group
 //            and not once per head, and no repeat_kv copy exists
-//   CTA      4 warps x 16 rows; grid (kv_heads * bsz, row tiles), row tiles in reverse so the longest rows start first
+//   CTA      4 warps x 16 rows; each CTA takes its (sequence, KV group, row tile) from the launch's work description
+//            (prefill_attn_sched.h): grid (kv_heads * bsz, row tiles) for a uniform batch (exl_prefill_attn), one CTA per tile of
+//            every sequence for a ragged batch (exl_prefill_attn_ragged, no CTA for padding, the sequences with the most keys
+//            first); row tiles in reverse so the longest rows start first; the math inside a tile is the same for both
 //   K / V    64-key tiles, double-buffered through cp.async (zero-filled past the CTA's last visible key: a cache row that was
 //            never written, NaN included, is never read); ldmatrix from XOR-swizzled shared memory (conflict-free phases)
 //   softmax  online, fp32 scores / max / sum / output accumulators; P rounded to fp16 for the P . V product; only the key
 //            tiles that cross the diagonal are masked, tiles entirely above it are never loaded
-//   output   one fp16 rounding of o / l, written straight into [bsz, q_len, heads * 128] (o_proj's input layout)
+//   output   one fp16 rounding of o / l, written straight into [tokens, heads * 128] (o_proj's input layout)
 // No atomics and a fixed reduction order: two launches are bitwise equal.  No programmatic dependent launch.
 #include "exl_common.cuh"
+#include "prefill_attn_sched.h"
+
+static_assert(pa_sched::MAX_SEQ == EXL_RAGGED_MAX_SEQ, "one ragged description holds every sequence exl_ragged may name");
 
 namespace {
 
 constexpr int PA_THREADS = 128;                          // 4 warps x 16 query rows
-constexpr int PA_BM = 64;                                // query rows per CTA
+constexpr int PA_BM = pa_sched::BM;                      // query rows per CTA
 constexpr int PA_BN = 64;                                // keys per K / V tile
 constexpr int HD = 128;
 constexpr uint32_t PA_TILE_BYTES = 64 * HD * 2;          // one [64][128] fp16 tile
@@ -66,8 +72,8 @@ __device__ __forceinline__ uint32_t pa_pack(float lo, float hi)
 
 __global__ void __launch_bounds__(PA_THREADS, 2) prefill_attn_kernel(const half* __restrict__ q, const half* __restrict__ kc,
                                                                   const half* __restrict__ vc, half* __restrict__ out,
-                                                                  int q_len, int heads, int kv_heads, int past_len, int max_seq,
-                                                                  float scale_log2, int row_tiles)
+                                                                  const __grid_constant__ pa_sched::Work work, int heads,
+                                                                  int max_seq, float scale_log2)
 {
     extern __shared__ __align__(128) unsigned char pa_sm[];
     const uint32_t sQ = pa_smem(pa_sm);
@@ -75,18 +81,18 @@ __global__ void __launch_bounds__(PA_THREADS, 2) prefill_attn_kernel(const half*
     const uint32_t sV = sQ + 3 * PA_TILE_BYTES;          // V[0], V[1]
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int n_rep = heads / kv_heads;
-    const int g = blockIdx.x % kv_heads, b = blockIdx.x / kv_heads;
-    const int R = q_len * n_rep;                          // rows of this (sequence, KV group)
-    const int m0 = (row_tiles - 1 - (int)blockIdx.y) * PA_BM;
+    const int kv_heads = work.kv_heads, n_rep = work.n_rep;
+    const pa_sched::Tile tile = pa_sched::tile_of(work, (int)blockIdx.x, (int)blockIdx.y);
+    const int g = tile.g, past_len = tile.past_len, m0 = tile.m0;
+    const int R = tile.q_len * n_rep;                     // rows of this (sequence, KV group)
     const int t_lo = m0 / n_rep, t_hi = (min(R, m0 + PA_BM) - 1) / n_rep;
     const int kv_end = past_len + t_hi + 1;               // keys any row of this CTA sees
     const int n_tiles = (kv_end + PA_BN - 1) / PA_BN;
     const int diag = past_len + t_lo;                     // a key tile ending at or before this key needs no mask
-    const size_t cache_off = (size_t)(b * kv_heads + g) * max_seq * HD;
+    const size_t cache_off = ((size_t)tile.cache_seq * kv_heads + g) * max_seq * HD;
     const half* kbase = kc + cache_off;
     const half* vbase = vc + cache_off;
-    const size_t qrow0 = (size_t)b * q_len * heads + (size_t)g * n_rep;   // (token 0, first head of the group) of this sequence
+    const size_t qrow0 = (size_t)tile.tok0 * heads + (size_t)g * n_rep;   // (token 0, first head of the group) of this sequence
 
     // ---- Q tile (rows past R zero-filled) and K / V tile 0 ----
     #pragma unroll
@@ -224,6 +230,24 @@ __global__ void __launch_bounds__(PA_THREADS, 2) prefill_attn_kernel(const half*
 
 } // namespace
 
+// one launch of prefill_attn_kernel over a validated work description
+static int pa_launch(const half* q, const half* kc, const half* vc, half* out, const pa_sched::Work& work, int heads, int max_seq,
+                     cudaStream_t stream)
+{
+    int dev = 0;
+    EXL_CUDA_TRY(cudaGetDevice(&dev));
+    static bool attr_done[EXL_MAX_DEVICES] = {};
+    if (dev >= 0 && dev < EXL_MAX_DEVICES && !attr_done[dev]) {
+        EXL_CUDA_TRY(cudaFuncSetAttribute(prefill_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PA_SMEM));
+        attr_done[dev] = true;
+    }
+    const float scale_log2 = 1.4426950408889634f / sqrtf((float)HD);
+    const dim3 grid((unsigned)pa_sched::grid_x(work), (unsigned)pa_sched::grid_y(work));
+    prefill_attn_kernel<<<grid, PA_THREADS, PA_SMEM, stream>>>(q, kc, vc, out, work, heads, max_seq, scale_log2);
+    EXL_CHECK_LAUNCH("prefill_attn_kernel");
+    return EXL_OK;
+}
+
 int exl_prefill_attn_launch(const half* q, const half* kc, const half* vc, half* out, int bsz, int q_len, int heads, int kv_heads,
                             int head_dim, int past_len, int max_seq, cudaStream_t stream)
 {
@@ -243,17 +267,48 @@ int exl_prefill_attn_launch(const half* q, const half* kc, const half* vc, half*
     if (row_tiles > 65535 || (long long)bsz * kv_heads > 0x7fffffffLL)
         return exl_set_err(EXL_ERR_ARG, "prefill_attn: q_len %d x %d heads per KV head needs %lld row tiles (at most 65535)",
                            q_len, heads / kv_heads, row_tiles);
-    int dev = 0;
-    EXL_CUDA_TRY(cudaGetDevice(&dev));
-    static bool attr_done[EXL_MAX_DEVICES] = {};
-    if (dev >= 0 && dev < EXL_MAX_DEVICES && !attr_done[dev]) {
-        EXL_CUDA_TRY(cudaFuncSetAttribute(prefill_attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PA_SMEM));
-        attr_done[dev] = true;
+    pa_sched::Work work;
+    pa_sched::make_uniform(work, bsz, q_len, past_len, kv_heads, heads / kv_heads);
+    return pa_launch(q, kc, vc, out, work, heads, max_seq, stream);
+}
+
+int exl_ragged_validate(const exl_ragged* r, int num_cache_seqs, int max_seq, const char* who)
+{
+    if (!r || !r->q_len || !r->past_len || !r->cache_seq)
+        return exl_set_err(EXL_ERR_ARG, "%s: NULL pointer (ragged %p, q_len %p, past_len %p, cache_seq %p)", who, (const void*)r,
+                           r ? (const void*)r->q_len : nullptr, r ? (const void*)r->past_len : nullptr,
+                           r ? (const void*)r->cache_seq : nullptr);
+    if (r->n_seq < 1 || r->n_seq > EXL_RAGGED_MAX_SEQ)
+        return exl_set_err(EXL_ERR_ARG, "%s: n_seq %d outside [1, %d]", who, r->n_seq, EXL_RAGGED_MAX_SEQ);
+    for (int i = 0; i < r->n_seq; i++) {
+        const int ql = r->q_len[i], pl = r->past_len[i], cs = r->cache_seq[i];
+        if (ql < 1) return exl_set_err(EXL_ERR_ARG, "%s: q_len[%d] %d < 1", who, i, ql);
+        if (pl < 0) return exl_set_err(EXL_ERR_ARG, "%s: past_len[%d] %d < 0", who, i, pl);
+        if ((long long)pl + ql > max_seq)
+            return exl_set_err(EXL_ERR_ARG, "%s: past_len[%d] %d + q_len[%d] %d > max_seq_len %d", who, i, pl, i, ql, max_seq);
+        if (cs < 0 || cs >= num_cache_seqs)
+            return exl_set_err(EXL_ERR_ARG, "%s: cache_seq[%d] %d outside [0, num_cache_seqs %d)", who, i, cs, num_cache_seqs);
+        for (int j = 0; j < i; j++)
+            if (r->cache_seq[j] == cs) return exl_set_err(EXL_ERR_ARG, "%s: cache_seq[%d] %d repeats cache_seq[%d]", who, i, cs, j);
     }
-    const float scale_log2 = 1.4426950408889634f / sqrtf((float)HD);
-    const dim3 grid((unsigned)(bsz * kv_heads), (unsigned)row_tiles);
-    prefill_attn_kernel<<<grid, PA_THREADS, PA_SMEM, stream>>>(q, kc, vc, out, q_len, heads, kv_heads, past_len, max_seq, scale_log2,
-                                                              (int)row_tiles);
-    EXL_CHECK_LAUNCH("prefill_attn_kernel");
     return EXL_OK;
+}
+
+int exl_prefill_attn_ragged_launch(const half* q, const half* kc, const half* vc, half* out, const exl_ragged* r, int num_cache_seqs,
+                                   int heads, int kv_heads, int head_dim, int max_seq, cudaStream_t stream)
+{
+    const char* who = "prefill_attn_ragged";
+    if (!q || !kc || !vc || !out)
+        return exl_set_err(EXL_ERR_ARG, "%s: NULL pointer (q %p, key_cache %p, value_cache %p, out %p)", who,
+                           (const void*)q, (const void*)kc, (const void*)vc, (void*)out);
+    if (head_dim != HD) return exl_set_err(EXL_ERR_ARG, "%s: head_dim %d != 128", who, head_dim);
+    if (heads < 1 || kv_heads < 1 || heads % kv_heads != 0)
+        return exl_set_err(EXL_ERR_ARG, "%s: num_kv_heads %d does not divide num_heads %d", who, kv_heads, heads);
+    if (const int rc = exl_ragged_validate(r, num_cache_seqs, max_seq, who)) return rc;
+    long long ctas = 0;
+    for (int i = 0; i < r->n_seq; i++) ctas += (long long)kv_heads * pa_sched::row_tiles_of(r->q_len[i], heads / kv_heads);
+    if (ctas > 0x7fffffffLL) return exl_set_err(EXL_ERR_ARG, "%s: %lld CTAs (at most 2^31 - 1)", who, ctas);
+    pa_sched::Work work;
+    pa_sched::make_ragged(work, r->n_seq, r->q_len, r->past_len, r->cache_seq, kv_heads, heads / kv_heads);
+    return pa_launch(q, kc, vc, out, work, heads, max_seq, stream);
 }

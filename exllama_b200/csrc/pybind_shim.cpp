@@ -286,6 +286,74 @@ void prefill_attn(torch::Tensor q, torch::Tensor key_cache, torch::Tensor value_
                               num_heads, num_kv_heads, head_dim, past_len, max_seq_len, cur_stream()));
 }
 
+// a ragged batch: the three per-sequence lists as exl_ragged (the vectors must outlive the call)
+static exl_ragged ragged_of(const std::vector<int>& q_lens, const std::vector<int>& past_lens, const std::vector<int>& cache_seqs,
+                            const char* who)
+{
+    TORCH_CHECK(q_lens.size() == past_lens.size() && q_lens.size() == cache_seqs.size(), who,
+                ": q_lens, past_lens and cache_seqs must have the same length");
+    return exl_ragged{(int)q_lens.size(), q_lens.data(), past_lens.data(), cache_seqs.data()};
+}
+
+static int64_t ragged_tokens(const std::vector<int>& q_lens)
+{
+    int64_t T = 0;
+    for (int l : q_lens) T += l;
+    return T;
+}
+
+static void check_caches(const torch::Tensor& kc, const torch::Tensor& vc, const torch::Tensor& like, int num_kv_heads, int head_dim,
+                         int max_seq_len, const char* who)
+{
+    CHECK_DTYPE(kc, kHalf); CHECK_DTYPE(vc, kHalf);
+    TORCH_CHECK(kc.dim() == 4 && kc.is_contiguous() && vc.is_contiguous() && kc.sizes() == vc.sizes() && kc.size(1) == num_kv_heads &&
+                kc.size(2) == max_seq_len && kc.size(3) == head_dim,
+                who, ": caches must be contiguous [num_cache_seqs, num_kv_heads, max_seq_len, head_dim]");
+    TORCH_CHECK(kc.device() == like.device() && vc.device() == like.device(), who, ": tensors on different devices");
+}
+
+// causal attention of a ragged batch over the caches: q [T, heads(*hd)] packed -> out [T, heads*hd]; sequence i attends cache
+// sequence cache_seqs[i] of caches [num_cache_seqs, kv_heads, max_seq_len, hd]
+void prefill_attn_ragged(torch::Tensor q, torch::Tensor key_cache, torch::Tensor value_cache, torch::Tensor out,
+                         std::vector<int> q_lens, std::vector<int> past_lens, std::vector<int> cache_seqs, int num_heads,
+                         int num_kv_heads, int head_dim, int max_seq_len)
+{
+    const char* who = "prefill_attn_ragged";
+    CHECK_DTYPE(q, kHalf); CHECK_DTYPE(out, kHalf);
+    const exl_ragged r = ragged_of(q_lens, past_lens, cache_seqs, who);
+    const int64_t n = ragged_tokens(q_lens) * num_heads * head_dim;
+    TORCH_CHECK(q.is_contiguous() && q.numel() == n, who, ": q must be contiguous [sum(q_lens), num_heads, head_dim]");
+    TORCH_CHECK(out.is_contiguous() && out.numel() == n, who, ": out must be contiguous [sum(q_lens), num_heads * head_dim]");
+    check_caches(key_cache, value_cache, q, num_kv_heads, head_dim, max_seq_len, who);
+    TORCH_CHECK(out.device() == q.device(), who, ": tensors on different devices");
+    const at::cuda::OptionalCUDAGuard device_guard(q.device());
+    EXL_CALL(exl_prefill_attn_ragged(q.data_ptr(), key_cache.data_ptr(), value_cache.data_ptr(), out.data_ptr(), &r,
+                                     (int)key_cache.size(0), num_heads, num_kv_heads, head_dim, max_seq_len, cur_stream()));
+}
+
+// rope q [T, heads(*hd)] and k [T, kv_heads(*hd)] of a ragged batch in place and write k, v [T, kv_heads(*hd)] into the caches
+void rope_cache_ragged(torch::Tensor q, torch::Tensor k, torch::Tensor v, torch::Tensor key_cache, torch::Tensor value_cache,
+                       torch::Tensor sin, torch::Tensor cos, std::vector<int> q_lens, std::vector<int> past_lens,
+                       std::vector<int> cache_seqs, int num_heads, int num_kv_heads, int head_dim, int max_seq_len)
+{
+    const char* who = "rope_cache_ragged";
+    CHECK_DTYPE(q, kHalf); CHECK_DTYPE(k, kHalf); CHECK_DTYPE(v, kHalf); CHECK_DTYPE(sin, kHalf); CHECK_DTYPE(cos, kHalf);
+    const exl_ragged r = ragged_of(q_lens, past_lens, cache_seqs, who);
+    const int64_t T = ragged_tokens(q_lens);
+    TORCH_CHECK(q.is_contiguous() && q.numel() == T * num_heads * head_dim, who, ": q must be contiguous [sum(q_lens), num_heads, head_dim]");
+    TORCH_CHECK(k.is_contiguous() && v.is_contiguous() && k.numel() == T * num_kv_heads * head_dim && v.numel() == k.numel(), who,
+                ": k and v must be contiguous [sum(q_lens), num_kv_heads, head_dim]");
+    TORCH_CHECK(sin.is_contiguous() && cos.is_contiguous() && sin.numel() >= (int64_t)max_seq_len * head_dim &&
+                cos.numel() >= (int64_t)max_seq_len * head_dim, who, ": sin and cos must be contiguous [>= max_seq_len, head_dim]");
+    check_caches(key_cache, value_cache, q, num_kv_heads, head_dim, max_seq_len, who);
+    TORCH_CHECK(k.device() == q.device() && v.device() == q.device() && sin.device() == q.device() && cos.device() == q.device(), who,
+                ": tensors on different devices");
+    const at::cuda::OptionalCUDAGuard device_guard(q.device());
+    EXL_CALL(exl_rope_cache_ragged(q.data_ptr(), k.data_ptr(), v.data_ptr(), key_cache.data_ptr(), value_cache.data_ptr(),
+                                   sin.data_ptr(), cos.data_ptr(), &r, (int)key_cache.size(0), num_heads, num_kv_heads, head_dim,
+                                   max_seq_len, cur_stream()));
+}
+
 // fused projection + peer-memory all-reduce
 pybind11::tuple tp_workspace_alloc(int device)
 {
@@ -348,6 +416,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m)
     m.def("q4_mlp_tp", &q4_mlp_tp, "q4_mlp_tp");
     m.def("decode_attn", &decode_attn, "decode_attn");
     m.def("prefill_attn", &prefill_attn, "prefill_attn");
+    m.def("prefill_attn_ragged", &prefill_attn_ragged, "prefill_attn_ragged");
+    m.def("rope_cache_ragged", &rope_cache_ragged, "rope_cache_ragged");
     m.def("tp_status", [](int device) { unsigned t = 0; EXL_CALL(exl_tp_status(device, &t)); return (int)t; }, "tp_status");
     m.def("tp_workspace_alloc", &tp_workspace_alloc, "tp_workspace_alloc");
     m.def("tp_workspace_open", &tp_workspace_open, "tp_workspace_open");

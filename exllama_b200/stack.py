@@ -400,5 +400,69 @@ class DecodeStack:
         hn = cuda_ext.ext_rms_norm(hidden, self.norm, s.eps)
         return torch.matmul(hn.view(-1, s.hidden), self.lm_head.t()).float()
 
+    RAGGED_MAX_SEQ = 64                        # EXL_RAGGED_MAX_SEQ: sequences of one prefill_ragged call
+
+    def prefill_ragged(self, hidden, q_lens, past_lens, seqs=None, last_only=True):
+        """n prompts or follow-up turns of different lengths at different past_lens in one call.  hidden: [T, hidden] fp16, the
+        sequences' tokens packed in order (sequence i owns rows [sum(q_lens[:i]), + q_lens[i])); sequence i fills rows
+        [past_lens[i], past_lens[i] + q_lens[i]) of cache sequence seqs[i] (default 0 .. n-1, distinct) and attends rows
+        [0, past_lens[i] + t] of it.  The same results as n prefill(x_i, past_lens[i], seq=seqs[i]) calls except for the GEMM route:
+        the q4 GEMMs run once per layer on all T rows.  Per layer one rope_cache_ragged and one prefill_attn_ragged launch
+        (csrc/elementwise.cu, csrc/prefill_attn.cu).  Returns the logits [n, vocab] of each sequence's last token (last_only) or
+        [T, vocab]."""
+        s = self.shape
+        if self.tp_size > 1:
+            raise NotImplementedError("prefill_ragged under tensor parallelism is not implemented")
+        q_lens, past_lens = [int(v) for v in q_lens], [int(v) for v in past_lens]
+        n = len(q_lens)
+        seqs = list(range(n)) if seqs is None else [int(v) for v in seqs]
+        if not 1 <= n <= self.RAGGED_MAX_SEQ:
+            raise ValueError(f"prefill_ragged of {n} sequences: one call takes 1 .. {self.RAGGED_MAX_SEQ}")
+        if len(past_lens) != n or len(seqs) != n:
+            raise ValueError(f"prefill_ragged: {n} q_lens, {len(past_lens)} past_lens and {len(seqs)} seqs")
+        for ql, pl, sq in zip(q_lens, past_lens, seqs):
+            if ql < 1:
+                raise ValueError(f"prefill of {ql} tokens: q_len must be at least 1")
+            if pl < 0 or pl + ql > self.max_seq:
+                raise ValueError(f"prefill of {ql} tokens at past_len {pl}: rows [{pl}, {pl + ql}) do not fit max_seq {self.max_seq}")
+            if not 0 <= sq < self.batch:
+                raise ValueError(f"prefill into cache sequence {sq}: the caches hold [0, {self.batch}) (DecodeStack(..., batch=))")
+        if len(set(seqs)) != n:
+            raise ValueError(f"prefill_ragged into cache sequences {seqs}: a cache sequence is named twice")
+        T = sum(q_lens)
+        if hidden.dim() != 2 or tuple(hidden.shape) != (T, s.hidden):
+            raise ValueError(f"prefill_ragged: hidden {tuple(hidden.shape)} is not [sum(q_lens) = {T}, {s.hidden}]")
+        hq = self.local_heads * s.head_dim
+        kvh = self.local_kv_heads
+        ad = lambda i, n: (self.lora[i] or {}).get(n) if self.lora is not None else None      # (A, B) or None
+        hidden = hidden.view(1, T, s.hidden)
+        for i, L in enumerate(self.layers):
+            residual = hidden
+            x = cuda_ext.ext_rms_norm(hidden, L.ln1, s.eps)
+            q = L.q.forward(x, ad(i, "q"))
+            k = L.k.forward(x, ad(i, "k"))
+            v = L.v.forward(x, ad(i, "v"))
+            ext.rope_cache_ragged(q, k, v, self.key_cache[i], self.value_cache[i], self.sin, self.cos, q_lens, past_lens, seqs,
+                                  self.local_heads, kvh, s.head_dim, self.max_seq)
+            attn = torch.empty((1, T, hq), dtype=torch.float16, device=self.device)
+            ext.prefill_attn_ragged(q, self.key_cache[i], self.value_cache[i], attn, q_lens, past_lens, seqs, self.local_heads, kvh,
+                                    s.head_dim, self.max_seq)
+            hidden = residual + L.o.forward(attn, ad(i, "o"))
+            residual = hidden
+            x = cuda_ext.ext_rms_norm(hidden, L.ln2, s.eps)
+            y = torch.nn.functional.silu(L.gate.forward(x, ad(i, "gate")))
+            y *= L.up.forward(x, ad(i, "up"))
+            hidden = residual + L.down.forward(y, ad(i, "down"))
+        if self.lm_head is None:
+            return hidden.view(T, s.hidden)
+        if last_only:
+            ends, t = [], 0
+            for ql in q_lens:
+                t += ql
+                ends.append(t - 1)
+            hidden = hidden[:, torch.tensor(ends, device=self.device), :].contiguous()
+        hn = cuda_ext.ext_rms_norm(hidden, self.norm, s.eps)
+        return torch.matmul(hn.view(-1, s.hidden), self.lm_head.t()).float()
+
     def close(self):
         ext.cleanup()

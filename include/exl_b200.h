@@ -185,6 +185,42 @@ int exl_prefill_attn(const void* q, const void* key_cache, const void* value_cac
                      int bsz, int q_len, int num_heads, int num_kv_heads, int head_dim,
                      int past_len, int max_seq_len, void* stream);
 
+/* A ragged batch: n_seq sequences, each with its own chunk length, history and cache sequence (host arrays of n_seq entries, read
+   during the call; the description travels in the kernel parameters, nothing is copied to the device, so a captured graph
+   replays the same call).  Tokens are packed in sequence order: sequence i owns token rows [off_i, off_i + q_len[i]),
+   off_i = sum_{j<i} q_len[j], T = sum_i q_len[i].  Token t of sequence i sits at position past_len[i] + t of cache sequence
+   cache_seq[i].  Requirements (else EXL_ERR_ARG naming the value): 1 <= n_seq <= EXL_RAGGED_MAX_SEQ, q_len[i] >= 1,
+   past_len[i] >= 0, past_len[i] + q_len[i] <= max_seq_len, 0 <= cache_seq[i] < num_cache_seqs and no cache_seq twice. */
+#define EXL_RAGGED_MAX_SEQ 64
+typedef struct {
+    int n_seq;
+    const int* q_len;
+    const int* past_len;
+    const int* cache_seq;
+} exl_ragged;
+
+/* exl_prefill_attn over a ragged batch, one launch (same kernel, same math inside a tile):
+     out[t, h, :] = softmax_j(q[t, h] . K[cache_seq[i], kvh(h), j] / sqrt(128)) . V[cache_seq[i], kvh(h), j],
+     j in [0, past_len[i] + t - off_i]  for token row t of sequence i
+   q [T, num_heads, 128] after rope; out [T, num_heads * 128] (o_proj's input); key_cache / value_cache
+   [num_cache_seqs, num_kv_heads, max_seq_len, 128].  One CTA per (sequence, KV group, 64-row query tile), none for padding, the
+   sequences with the most keys first.  Preconditions and guarantees as exl_prefill_attn, per sequence: rows
+   [past_len[i], past_len[i] + q_len[i]) of cache sequence cache_seq[i] already hold its k / v; reads only rows
+   [0, past_len[i] + q_len[i]) of the named cache sequences; writes only out.  A ragged batch of bsz equal sequences in cache
+   sequences 0..bsz-1 gives bitwise exl_prefill_attn's result.  EXL_ERR_ARG also for head_dim != 128, num_kv_heads not dividing
+   num_heads, or a NULL pointer. */
+int exl_prefill_attn_ragged(const void* q, const void* key_cache, const void* value_cache, void* out, const exl_ragged* r,
+                            int num_cache_seqs, int num_heads, int num_kv_heads, int head_dim, int max_seq_len, void* stream);
+
+/* Rope and cache write of a ragged batch in one launch: rope q [T, num_heads, 128] and k [T, num_kv_heads, 128] in place at each
+   token's position (bit-exact with exl_rope, the reference's fp16 instruction order, rope.cu:48-67), and write the roped k row and
+   the v [T, num_kv_heads, 128] row of token t of sequence i into row past_len[i] + t of cache sequence cache_seq[i] of
+   key_cache / value_cache [num_cache_seqs, num_kv_heads, max_seq_len, 128].  sin / cos [>= max_seq_len, 128].  Writes no other
+   cache row.  EXL_ERR_ARG as exl_prefill_attn_ragged. */
+int exl_rope_cache_ragged(void* q, void* k, const void* v, void* key_cache, void* value_cache, const void* sin, const void* cos,
+                          const exl_ragged* r, int num_cache_seqs, int num_heads, int num_kv_heads, int head_dim,
+                          int max_seq_len, void* stream);
+
 /* --- whole decode step as ONE persistent kernel (SURVEY.md 8f-4 "host loop"; 8f-2 lm_head + final norm) ------------- */
 
 /* Everything ExLlama.forward does for one new token of one sequence (model.py:1053-1077: per layer ExLlamaAttention.fused

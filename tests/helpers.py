@@ -72,20 +72,31 @@ def oracle_mm(oracle, xin, lin, ab=None, acc=None, recons=False):
     return out if acc is None else out + np.asarray(acc, np.float64)
 
 
-def oracle_decode_step(oracle, st, snap, x, past, seq=0):
-    """float64/fp16 restatement of one decode token of a DecodeStack (grouped-query attention, cache sequence `seq`, the stack's
-    adapter) on the cache snapshot `snap` (per layer (key_cache, value_cache) tensors): (final hidden fp16, logits float64, new k/v
-    rows per layer)."""
+def oracle_qkv(oracle, st, i, x, past):
+    """Layer i of a DecodeStack on the fp16 layer input x [1, hidden], as oracle_decode_step computes it: (normed x, roped fp16 q
+    [heads * hd], roped fp16 k [kv_heads, hd], fp16 v [kv_heads, hd]) of the new token at position `past`."""
     s = st.shape
     hd, heads, kvh = s.head_dim, s.heads, s.kv_heads
     sin = st.sin.view(-1, hd).cpu().numpy(); cos = st.cos.view(-1, hd).cpu().numpy()
+    L = st.layers[i]
+    xn, _ = oracle.rms_norm(x, _np(L.ln1), s.eps)
+    q, k, v = (oracle_mm(oracle, xn, getattr(L, n), adapter_of(st, i, n)).astype(np.float16) for n in ("q", "k", "v"))
+    q = oracle.rope(q.reshape(1, heads, hd), sin, cos, 1, heads, hd, heads, past).reshape(-1)
+    k = oracle.rope(k.reshape(1, kvh, hd), sin, cos, 1, kvh, hd, kvh, past).reshape(kvh, hd)
+    return xn, q, k, v.reshape(kvh, hd)
+
+
+def oracle_decode_step(oracle, st, snap, x, past, seq=0, n_layers=None):
+    """float64/fp16 restatement of one decode token of a DecodeStack (grouped-query attention, cache sequence `seq`, the stack's
+    adapter) on the cache snapshot `snap` (per layer (key_cache, value_cache) tensors): (final hidden fp16, logits float64 or None
+    for a stack without a head, new k/v rows per layer).  n_layers: stop after that many layers (hidden state after them, no
+    logits)."""
+    s = st.shape
+    hd, heads, kvh = s.head_dim, s.heads, s.kv_heads
     x = x.reshape(1, s.hidden).copy()
     rows = []
     for i, L in enumerate(st.layers):
-        xn, _ = oracle.rms_norm(x, _np(L.ln1), s.eps)
-        q, k, v = (oracle_mm(oracle, xn, getattr(L, n), adapter_of(st, i, n)).astype(np.float16) for n in ("q", "k", "v"))
-        q = oracle.rope(q.reshape(1, heads, hd), sin, cos, 1, heads, hd, heads, past).reshape(-1)
-        k = oracle.rope(k.reshape(1, kvh, hd), sin, cos, 1, kvh, hd, kvh, past).reshape(kvh, hd)
+        _, q, k, v = oracle_qkv(oracle, st, i, x, past)
         kc = _np(snap[i][0][seq]).copy(); vc = _np(snap[i][1][seq]).copy()
         kc[:, past] = k; vc[:, past] = v.reshape(kvh, hd)
         rows.append((k.copy(), v.reshape(kvh, hd).copy()))
@@ -95,6 +106,10 @@ def oracle_decode_step(oracle, st, snap, x, past, seq=0):
         act = oracle.silu_mul(oracle_mm(oracle, xn, L.gate, adapter_of(st, i, "gate")).astype(np.float16),
                               oracle_mm(oracle, xn, L.up, adapter_of(st, i, "up")).astype(np.float16))
         x = oracle_mm(oracle, act, L.down, adapter_of(st, i, "down"), acc=x).astype(np.float16)
+        if i + 1 == n_layers:
+            return x, None, rows
+    if st.lm_head is None:
+        return x, None, rows
     hn, _ = oracle.rms_norm(x, _np(st.norm), s.eps)
     return x, hn.astype(np.float64) @ _np(st.lm_head).astype(np.float64).T, rows
 
@@ -307,6 +322,278 @@ def to_cuda(*arrays):
     for a in arrays:
         out.append(None if a is None else torch.from_numpy(np.ascontiguousarray(a)).cuda())
     return out if len(out) > 1 else out[0]
+
+
+# ---------------------------------------------------------------------------------------------------------------------------------
+# Attention probe: a DecodeStack whose final hidden state is, up to fp16 rounding, the residual plus the attention outputs
+#
+# o_proj is the identity (stored zero nibble 7, nibble 9 on the diagonal and 8 elsewhere, scale 1), ln2 is zero so the MLP adds an
+# exact 0, the residual is small (1e-2 N(0, 1): the rms norm makes q / k / v independent of its scale) and there is no head.  Keys
+# planted in the caches then pin each head's answer: a set P of positions holding the same key bits, scoring >= PROBE_GAP above every
+# other position of the head, makes the answer the mean of V over P whatever small error the kernel's q has.
+# ---------------------------------------------------------------------------------------------------------------------------------
+
+PROBE_SCORE = 40.0                # planted keys score at least this, and 30 above the head's other keys
+PROBE_GAP = 25.0                  # the setup asserts every other score of a planted head is this far below its plateau
+POISON_LIFT = 20.0                # the poison row scores this far above everything else
+
+
+def identity_q4(n, act=False, seed=0, gs=128):
+    """GPTQ tensors (qweight, qzeros, scales, g_idx) of the n x n identity in original row order: stored zero nibble 7 (z + 1 = 8),
+    nibble 9 on the diagonal and 8 elsewhere, scale 1.  act: a random g_idx (make_q4 reorders the rows; the x gather undoes it)."""
+    qw = np.full((n // 8, n), 0x88888888, np.uint32)
+    k = np.arange(n)
+    qw[k // 8, k] += (np.uint32(1) << (4 * (k % 8)).astype(np.uint32))
+    qz = np.full((n // gs, n // 8), 0x77777777, np.uint32)
+    return (qw.view(np.int32), qz.view(np.int32), np.ones((n // gs, n), np.float16),
+            _g_idx(n, gs, act, np.random.default_rng(seed)))
+
+
+def scaled_q_as_k(qweight, qzeros, scales, heads, kv_heads, gamma, hd=128):
+    """k projection tensors whose output is gamma times the q projection's first query head of each KV group (q4_column_sample
+    of those columns, scales x gamma, gamma a power of two): k_new = gamma q up to the GEMV's accumulation order."""
+    n_rep = heads // kv_heads
+    cols = (np.arange(kv_heads)[:, None] * n_rep * hd + np.arange(hd)[None]).reshape(-1)
+    kw, kz, ks = q4_column_sample(qweight, qzeros, scales, cols)
+    return kw, kz, (ks.astype(np.float64) * gamma).astype(np.float16)
+
+
+def attn_probe_stack(shape, layers, max_seq, act=False, batch=1, seed=0, gamma=None, lora_rank=0):
+    """A DecodeStack (groupsize 128, no head) turned into an attention probe: identity o_proj (its own g_idx under act-order),
+    ln2 = 0.  gamma: k projection = gamma x the q projection of each KV group's first query head (scaled_q_as_k).  lora_rank:
+    adapters on q and v only, so o_proj stays the identity."""
+    import torch
+    from exllama_b200.stack import DecodeStack, Q4Linear
+    st = DecodeStack(shape, groupsize=128, act_order=act, max_seq=max_seq, layers=layers, seed=seed, with_head=False, batch=batch)
+    for i, L in enumerate(st.layers):
+        qw, qz, sc, g = identity_q4(shape.heads * shape.head_dim, act, seed * 31 + i)
+        L.o = Q4Linear(*to_cuda(qw, qz, sc), None if g is None else torch.from_numpy(g), st.dev_index)
+        L.ln2.zero_()
+        if gamma is not None:
+            assert not act, "gamma needs the q projection in original row order"
+            kw, kz, ks = scaled_q_as_k(_np(L.q.qweight), _np(L.q.qzeros), _np(L.q.scales), shape.heads, shape.kv_heads, gamma)
+            L.k = Q4Linear(*to_cuda(kw, kz, ks), None, st.dev_index)
+    if lora_rank:
+        st.add_lora(lora_rank, targets=("q", "v"), seed=seed)
+    torch.cuda.synchronize()
+    return st
+
+
+def probe_caches(st, seed):
+    """Background caches for a probe stack: per layer [key_cache, value_cache] numpy fp16 [batch, kv_heads, max_seq, hd] of
+    N(0, 0.25)."""
+    rng = np.random.default_rng(seed)
+    return [[(0.5 * rng.standard_normal(tuple(kc.shape))).astype(np.float16) for _ in range(2)] for kc in st.key_cache]
+
+
+def dense_positions(past, r=0, n_rep=1):
+    """The dense plateau of query head r of a KV group of n_rep heads: positions p < past with p mod 16 in {r, 15 - r} -- for r = 0
+    the first and the last position of every 16-position chunk (16k and 16k - 1) -- and past - 1 for the head whose residues hold
+    it (head 0 when none does)."""
+    p = np.arange(past)
+    sel = p[(p % 16 == r) | (p % 16 == 15 - r)]
+    if past > 0:
+        m = (past - 1) % 16
+        owner = min(m, 15 - m)
+        if (owner if owner < n_rep else 0) == r:
+            sel = np.union1d(sel, [past - 1])
+    return sel
+
+
+def single_positions(past):
+    """Where a lone planted key goes: 0, 15, 16, the first / a middle / the last 16-position chunk, past - 1 (those below past)."""
+    nch = (past + 15) // 16
+    c = [0, 15, 16, 7, 16 * (nch // 2) + 9, 16 * (nch - 1) + 3, past - 1]
+    return sorted({p for p in c if 0 <= p < past})
+
+
+def plant_group(q, kc, vc, plants, past, s_new, rng, poison=True):
+    """Plant keys for the query heads of one KV group (numpy, in place).
+
+    q [n_rep, hd] the heads' roped fp16 q; kc / vc [max_seq, hd] the group's cache rows of one sequence; plants[r] the positions
+    (< past) of head r's plateau, or None; s_new [n_rep] the new token's scores.  The key of head r is the least-norm k with
+    q_j . k / sqrt(hd) = T_r for j = r and 0 for the other heads of the group, T_r = max(PROBE_SCORE, 30 + every other score of
+    head r), written in fp16 at every position of plants[r], with a random +-1 V row per position.  poison: row `past` (which
+    the step overwrites with the new token) gets a key scoring POISON_LIFT above everything for every head and V = 100 x a
+    signature, and the rows past it NaN: a kernel that reads either shows it."""
+    hd = q.shape[1]
+    Q = q.astype(np.float64)
+    G = Q @ Q.T
+    bg = (kc[:past].astype(np.float64) @ Q.T).max(0) / np.sqrt(hd) if past > 0 else np.full(len(Q), -np.inf)
+    top = np.maximum(bg, s_new)
+    tmax = top.max()
+    for r, P in enumerate(plants):
+        if P is None or len(P) == 0:
+            continue
+        assert np.max(P) < past, (P, past)
+        T = max(PROBE_SCORE, top[r] + 30.0)
+        tmax = max(tmax, T)
+        t = np.zeros(len(Q)); t[r] = T * np.sqrt(hd)
+        kc[P] = (Q.T @ np.linalg.solve(G, t)).astype(np.float16)
+        assert np.isfinite(kc[P]).all(), f"plateau key of head {r} at score {T:.0f} overflows fp16"
+        vc[P] = rng.choice([-1.0, 1.0], (len(P), hd)).astype(np.float16)
+    if poison and past < kc.shape[0]:
+        t = np.full(len(Q), (tmax + POISON_LIFT) * np.sqrt(hd))
+        kc[past] = (Q.T @ np.linalg.solve(G, t)).astype(np.float16)
+        assert np.isfinite(kc[past]).all(), "poison key overflows fp16"
+        vc[past] = 100 * rng.choice([-1.0, 1.0], hd).astype(np.float16)
+        kc[past + 1:] = np.nan; vc[past + 1:] = np.nan
+
+
+def snap_of(caches):
+    import torch
+    return [(torch.from_numpy(kc), torch.from_numpy(vc)) for kc, vc in caches]
+
+
+def plant_probe(oracle, st, caches, x, past, spec, seed, seq=0, poison=True):
+    """Plant every layer of cache sequence `seq` of a probe stack (caches from probe_caches, modified in place), layer by layer:
+    layer l's q depends on the layers below, so they are planted first.  spec(l, h) -> positions of head h's plateau, "new" (the
+    new token dominates: nothing to plant) or None (background).  Returns plants[l] = {head: positions} for probe_expectation."""
+    s = st.shape
+    hd, heads, kvh = s.head_dim, s.heads, s.kv_heads
+    n_rep = heads // kvh
+    rng = np.random.default_rng(seed)
+    out = []
+    for l in range(len(st.layers)):
+        xl = np.asarray(x, np.float16).reshape(1, -1)
+        if l > 0:
+            xl = oracle_decode_step(oracle, st, snap_of(caches), x, past, seq, n_layers=l)[0]
+        _, q, k, _ = oracle_qkv(oracle, st, l, xl, past)
+        q = q.reshape(heads, hd)
+        pl = {}
+        for g in range(kvh):
+            qg = q[g * n_rep:(g + 1) * n_rep]
+            s_new = qg.astype(np.float64) @ k[g].astype(np.float64) / np.sqrt(hd)
+            ps = []
+            for r in range(n_rep):
+                P = spec(l, g * n_rep + r)
+                if isinstance(P, str):
+                    assert P == "new"
+                    pl[g * n_rep + r] = np.array([past])
+                    P = None
+                elif P is not None:
+                    taken = np.concatenate([np.zeros(0, np.int64)] + [p for p in ps if p is not None])
+                    P = np.setdiff1d(np.asarray(P, np.int64), taken)          # a position serves one head of the group
+                    if len(P):
+                        pl[g * n_rep + r] = P
+                    else:
+                        P = None
+                ps.append(P)
+            plant_group(qg, caches[l][0][seq, g], caches[l][1][seq, g], ps, past, s_new, rng, poison)
+        out.append(pl)
+    return out
+
+
+def _rope_err(v, e, sin_row, cos_row):
+    """Bound on |kernel - oracle| after rope (l' = hfma(l, cos, hmul(r, -sin)), both in fp16) of rows v [n, hd] whose pre-rope
+    values differ by at most e [n, hd]: the propagated difference plus one fp16 rounding difference (2^-10 relative) for each
+    of the two operations."""
+    hd = v.shape[1]
+    c = np.abs(cos_row.astype(np.float64)); sn = np.abs(sin_row.astype(np.float64))
+    partner = np.r_[np.arange(hd // 2, hd), np.arange(hd // 2)]
+    v64 = np.abs(v.astype(np.float64))
+    lin = c * e + sn * e[:, partner]
+    return 1.01 * (lin + 2.0 ** -10 * (sn * (v64[:, partner] + e[:, partner]) + v64 + lin)) + 2 * FP16_TINY
+
+
+def probe_expectation(oracle, st, snap, x, past, plants, kind, seq=0):
+    """(want, bound): the oracle's final hidden state of a probe stack (oracle_decode_step on the cache snapshot) and a float64
+    bound B >= |kernel - want| per element.
+
+    Per layer, with the layer input known to within bx (0 for layer 0):
+      q, k, v  The GEMV error is quant_error_bound(kind) of each projection, plus the oracle's own fp16 rounding 2^-11 |ref|,
+               plus the effect of a perturbed input: rms norm moves xn by at most |w| rm (bx + |x| rms(bx) / rms(x)) + 2 ulps,
+               contracted with |W| (adapters: the same for x . A, a rounding of x . A, and the 16-bit x grid, contracted with
+               |B|).  Rope adds the propagated error and 2 fp16 ulps (_rope_err): Dq, Dk, Dv.
+      scores   A score q . k_p / sqrt(hd) moves by at most delta_h = max(sum_d Dq_d max_p |k_pd|, sum_d Dq_d |kn_d| +
+               (|q_d| + Dq_d) Dk_d) / sqrt(hd) (cached rows hold the same bits in kernel and oracle; kn is the new token's
+               k), plus 2^-20 of sum_d |q_d| max_p |k_pd| / sqrt(hd) for the fp32 dot product and scale.
+      softmax  Scores within delta of the oracle's move every weight by a factor in [e^-2delta, e^2delta], so the output moves by
+               at most (e^{2 delta} - 1) max|V| (and never more than 2 max|V|: both are averages of the same rows).  A planted head (plants[l][h] = P) whose P scores at least gap above every
+               other position has its answer within 2 n e^{-(gap - 2 delta)} max|V| of the mean of V over P in both kernel and
+               oracle (n = past + 1 positions): that bound is used instead, and the setup asserts gap >= PROBE_GAP.  At past = 0 the
+               new row is the only one and has weight 1.  Add Dv of
+               the new row times the most weight it can have (1, or n e^{-(gap - 2 delta)} when it is off the plateau), and (past / 16 + 64) 2^-23 max|V| for fp32 accumulation along a chain of at most past / 16 + 64
+               additions and the exponential approximations.
+      o_proj   Two fp16 roundings of the attention output, then the identity o GEMV's x quantisation: quant_error_bound(kind)
+               of the identity at an upper bound of |attention| (segments: group and 128-k stage, so a head under plain order).
+      x_out    bx + the attention bound + the o bound + two fp16 roundings of the residual sum; the MLP adds an exact 0.
+    The fp16 roundings are taken relative (2^-11 |value|) with FP16_TINY for the subnormal range."""
+    s = st.shape
+    hd, heads, kvh = s.head_dim, s.heads, s.kv_heads
+    n_rep = heads // kvh
+    sin = st.sin.view(-1, hd).cpu().numpy()[past]; cos = st.cos.view(-1, hd).cpu().numpy()[past]
+    x = np.asarray(x, np.float16).reshape(1, -1)
+    want, _, rows = oracle_decode_step(oracle, st, snap, x, past, seq)
+    xs = [x] + [oracle_decode_step(oracle, st, snap, x, past, seq, n_layers=l)[0] for l in range(1, len(st.layers))] + [want]
+    bx = np.zeros(s.hidden)
+    sq = np.sqrt(hd)
+    for l, L in enumerate(st.layers):
+        xl = xs[l].astype(np.float64).reshape(-1)
+        xn, q, k, v = oracle_qkv(oracle, st, l, xs[l], past)
+        xn64 = xn.astype(np.float64).reshape(-1)
+        dxn = None
+        if bx.any():
+            w = np.abs(_np(L.ln1).astype(np.float64))
+            r = np.sqrt(np.mean(xl * xl) + s.eps)
+            dxn = 1.01 * (w / r * (bx + np.abs(xl) * (np.sqrt(np.mean(bx * bx)) / r + 2.0 ** -9)) + 2.0 ** -9 * np.abs(xn64))
+
+        def proj_err(name):
+            lin = getattr(L, name)
+            xm = None if lin.g_idx is None else oracle.make_x_map(lin.g_idx.numpy(), lin.qzeros.shape[0])
+            qw, qz, sc = _np(lin.qweight), _np(lin.qzeros), _np(lin.scales)
+            B, ref = quant_error_bound(oracle, xn, qw, qz, sc, xm, kind)
+            e = B[0] + 2.0 ** -11 * np.abs(ref[0]) + FP16_TINY
+            if dxn is not None:
+                W = np.abs(oracle.dequant_f64(qw, qz, sc))
+                e = e + 1.01 * ((dxn if xm is None else dxn[np.asarray(xm, np.int64)]) @ W)
+            ab = adapter_of(st, l, name)
+            if ab is not None:
+                A, Bm = (np.abs(_np(t).astype(np.float64)) for t in ab)
+                ex = 2.0 ** -9 * np.abs(xn64) + np.abs(xn64).max() / QUANT_Q["step"] + (0 if dxn is None else dxn)
+                t16 = np.abs(oracle.half_matmul_f64(xn, _np(ab[0])))
+                e = e + 1.01 * ((ex @ A + 2.0 ** -10 * t16[0]) @ Bm) + 2.0 ** -10 * (t16[0] @ Bm)
+            return e
+        eq, ek, ev = proj_err("q"), proj_err("k"), proj_err("v")
+        q = q.reshape(heads, hd)
+        dq = _rope_err(q, eq.reshape(heads, hd), sin, cos)
+        dk = _rope_err(k, ek.reshape(kvh, hd), sin, cos)
+        dv = ev.reshape(kvh, hd)
+        kc = _np(snap[l][0][seq]).copy(); vc = _np(snap[l][1][seq]).copy()
+        kc[:, past] = rows[l][0]; vc[:, past] = rows[l][1]
+        attn = oracle.decode_attn_f64(q.reshape(-1), kc, vc, heads, kvh, hd, past + 1, st.max_seq).reshape(heads, hd)
+        K = kc[:, :past + 1].astype(np.float64); V = vc[:, :past + 1].astype(np.float64)
+        q64 = q.astype(np.float64)
+        bh = np.zeros(heads)
+        for h in range(heads):
+            g = h // n_rep
+            kmax = np.abs(K[g]).max(0)
+            kold = np.abs(K[g, :past]).max(0) if past > 0 else np.zeros(hd)
+            kn = np.abs(K[g, past])
+            delta = max(dq[h] @ kold, dq[h] @ kn + (np.abs(q64[h]) + dq[h]) @ dk[g]) / sq
+            delta = delta * (1 + 2.0 ** -10) + 2.0 ** -20 * (np.abs(q64[h]) @ kmax) / sq
+            vmax = np.abs(V[g]).max() + dv[g].max()
+            P = plants[l].get(h) if plants is not None else None
+            if P is not None:
+                sc_h = K[g] @ q64[h] / sq
+                inP = np.zeros(past + 1, bool); inP[P] = True
+                assert len(set(sc_h[inP].tolist())) == 1 or P.tolist() == [past], f"layer {l} head {h}: planted keys differ"
+                gap = sc_h[inP].min() - sc_h[~inP].max() if (~inP).any() else np.inf
+                assert gap >= PROBE_GAP, f"layer {l} head {h}: plateau only {gap:.2f} above the other scores"
+                w_off = min(1.0, (past + 1) * np.exp(min(50.0, 2 * delta - gap))) if np.isfinite(gap) else 0.0
+                t = 2 * w_off * vmax + dv[g].max() * (1.0 if inP[past] else w_off)
+            elif past == 0:
+                t = dv[g].max()                                   # one row: weight 1 whatever the scores
+            else:
+                t = min(2.0, np.expm1(min(50.0, 2 * delta))) * vmax + dv[g].max()
+            bh[h] = t + (past / 16 + 64) * 2.0 ** -23 * vmax
+        battn = (bh[:, None] + 2.0 ** -10 * np.abs(attn) + 2 * FP16_TINY).reshape(-1)
+        lin = L.o
+        xm = None if lin.g_idx is None else oracle.make_x_map(lin.g_idx.numpy(), lin.qzeros.shape[0])
+        amax = ((np.abs(attn).reshape(-1) + battn) * (1 + 2.0 ** -9)).astype(np.float16)
+        Bo, _ = quant_error_bound(oracle, amax[None], _np(lin.qweight), _np(lin.qzeros), _np(lin.scales), xm, kind)
+        bx = bx + battn + Bo[0] + 2.0 ** -10 * np.abs(xs[l + 1].astype(np.float64).reshape(-1)) + 2 * FP16_TINY
+    return want.reshape(-1), bx
 
 
 class RefLib:

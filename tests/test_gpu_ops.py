@@ -226,7 +226,8 @@ def test_pybind_surface_end_to_end(oracle):
 # ---- decode attention over the KV cache (SURVEY.md 8f-1; model.py:372-409) --------------------------------------------------
 @pytest.mark.parametrize("heads,kv_heads,seq,max_seq", [
     (32, 32, 1, 2048), (32, 32, 255, 2048), (32, 32, 257, 2048), (32, 32, 1921, 2048), (4, 4, 2048, 2048),
-    (8, 2, 300, 512), (64, 8, 1000, 1024), (2, 1, 3001, 4096), (40, 40, 777, 2048)])
+    (8, 2, 300, 512), (64, 8, 1000, 1024), (2, 1, 3001, 4096), (40, 40, 777, 2048),
+    (8, 8, 1025, 2048), (8, 2, 1300, 2048), (32, 32, 1537, 2048), (64, 8, 1792, 2048), (8, 8, 4096, 4096)])
 def test_decode_attn(oracle, heads, kv_heads, seq, max_seq):
     import torch
     from exllama_b200 import capi
@@ -238,6 +239,8 @@ def test_decode_attn(oracle, heads, kv_heads, seq, max_seq):
     # a few dominant keys so the softmax is not flat (exercises the running-max rescale across splits / sub-blocks)
     for h in range(kv_heads):
         kc[h, rng.integers(0, seq)] *= 4
+    # rows past the context are never read (a weight-0 read of a NaN row would still poison the sum)
+    kc[:, seq:] = np.nan; vc[:, seq:] = np.nan
     want = oracle.decode_attn_f64(q, kc, vc, heads, kv_heads, hd, seq, max_seq)
     tq, tk, tv = to_cuda(q, kc, vc)
     got = capi.decode_attn(tq, tk, tv, heads, kv_heads, hd, seq, max_seq).cpu().numpy()

@@ -15,8 +15,8 @@
 //    shared-memory ring with full/empty mbarriers and never wait for a grid barrier: weight units (ONE 3-D TMA op for the
 //    8 KB of packed qweight + one 2-D op each for the unit's scale and zero rows), KV-cache rows older than the current token
 //    (bulk copies) and lm_head rows do not depend on activations, so up to 4 x depth x 8 KB per SM (~19 MB chip-wide) of the
-//    NEXT phase is already in flight while the consumers are in a barrier or in a phase prologue.  HBM stays busy across
-//    phase and layer boundaries -- the thing separate launches could not do.
+//    NEXT phase is loaded while the consumers are in a barrier or in a phase prologue, one stage per pipeline in flight at a
+//    time.  HBM stays busy across phase and layer boundaries -- the thing separate launches could not do.
 //  * Work of a GEMV phase = (128-column tile) x (128-row K stage) units, flattened tile-major and cut into G equal contiguous
 //    ranges (G = grid size): every SM streams the same number of bytes whatever the matrix shapes (65B gate/up: 172 tiles on
 //    132 SMs is no longer a problem).  A warp accumulates its 32 columns over the stages it sees and, at a tile boundary,
@@ -366,8 +366,14 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         const uint32_t ring_a = smem_u32(ring) + (uint32_t)pq * depth * STAGE_STRIDE;
         const uint32_t full0 = smem_u32(&full_bar[pq * depth]), empty0 = smem_u32(&empty_bar[pq * depth]);
         int jbase = 0;
+        // One stage in flight per pipeline: a stage is issued only once the pipeline's previous stage has landed.  The ring still
+        // fills ahead of the consumers, but stage by stage.  With the whole ring in flight (16 x 8 KB per SM), the release fence of
+        // every CTA's grid-barrier arrival took ~4.7 us on an H100, over 80 % of the barrier; with one stage per pipeline it takes
+        // ~1.7 us, and 4 x 8 KB per SM (4.2 MB chip-wide) still keep HBM busy.  Two or three per pipeline did not help
+        // (DESIGN 3c, profiles/step_trace_h100.json).
         auto acquire = [&](uint32_t tx) -> uint32_t {
             if (issued >= depth) mbar_wait(empty0 + ls * 8, par ^ 1u);
+            if (issued > 0) mbar_wait(full0 + (ls == 0 ? depth - 1 : ls - 1) * 8, ls == 0 ? par ^ 1u : par);
             if (lane == 0) mbar_expect_tx(full0 + ls * 8, tx);
             __syncwarp();
             return ring_a + (uint32_t)ls * STAGE_STRIDE;

@@ -15,6 +15,7 @@ import torch  # noqa: E402
 
 from helpers import RefLib, golden_cols, to_cuda  # noqa: E402
 from oracle import oracle as O  # noqa: E402
+from stack_harness import sincos  # noqa: E402
 import test_gpu_q4_matmul as TQ  # noqa: E402
 import test_gpu_ref_pin as TP  # noqa: E402
 
@@ -47,7 +48,7 @@ for rows, dim in [(1, 4096), (1, 5120), (3, 6656), (7, 8192), (17, 4096)]:
 for bsz, q_len, heads, hd, past in [(1, 1, 32, 128, 0), (1, 1, 40, 128, 1919), (1, 5, 8, 128, 3), (2, 3, 4, 128, 100)]:
     x = np.random.default_rng(17 + past).standard_normal((bsz, q_len, heads * hd)).astype(np.float16)
     t = to_cuda(x)
-    call(ref.lib.ref_rope, t, *to_cuda(*TP._sincos(2048, hd)), bsz, q_len * heads, hd, heads, past)
+    call(ref.lib.ref_rope, t, *to_cuda(*sincos(2048, hd)), bsz, q_len * heads, hd, heads, past)
     out[f"rope_{bsz}_{q_len}_{heads}_{hd}_{past}"] = t.cpu().numpy()
 rng = np.random.default_rng(3)
 for M, K in ((1, 4096), (7, 5120), (33, 6656)):
@@ -70,7 +71,7 @@ for act in (False, True):
         rng = np.random.default_rng(11)
         x = rng.standard_normal((1, q_len, hidden)).astype(np.float16)
         w = (1 + 0.1 * rng.standard_normal(hidden)).astype(np.float16)
-        ts, tc = to_cuda(*TP._sincos(max_seq, hd))
+        ts, tc = to_cuda(*sincos(max_seq, hd))
         hq, hk, hv = (handle(t[n]) for n in ("q", "k", "v"))
         tx, q, k, v = to_cuda(x), f16(1, q_len, hidden), f16(1, q_len, hidden), f16(1, q_len, hidden)
         kc, vc = f16(1, heads, max_seq, hd), f16(1, heads, max_seq, hd)

@@ -17,6 +17,7 @@ import torch  # noqa: E402
 
 from helpers import RefLib, to_cuda  # noqa: E402
 from oracle import oracle as O  # noqa: E402
+from stack_harness import sincos  # noqa: E402
 import test_gpu_gqa as TG  # noqa: E402
 
 out = {}
@@ -29,7 +30,7 @@ for heads, kv, q_len, past, act in TG.REF_CASES:
     hidden = heads * hd
     t, x, w = TG.q4_attn_inputs(O, heads, kv, q_len, act)
     hq, hk, hv = (ref.make_q4(*to_cuda(qw.copy(), qz, sc), g) for (qw, qz, sc, g) in (t["q"], t["k"], t["v"]))
-    ts, tc = to_cuda(*TG._sincos(max_seq, hd))
+    ts, tc = to_cuda(*sincos(max_seq, hd))
     tx, q, k, v = to_cuda(x), f16(1, q_len, hidden), f16(1, q_len, kv * hd), f16(1, q_len, kv * hd)
     kc, vc = f16(1, kv, max_seq, hd), f16(1, kv, max_seq, hd)
     torch.cuda.synchronize()

@@ -26,6 +26,25 @@ def assert_close_ref64(got_f16, ref64, rel=REL_TOL, rms=RMS_TOL, what=""):
     return float(np.sqrt(np.mean(err * err)) / max(r, 1e-30))
 
 
+def close_to_reference(mine, ref, what):
+    """Within 2e-2 relative plus 2e-2 of the rms of the reference kernel's output (its own fp16 rounding points differ from ours)."""
+    mine = np.asarray(mine, np.float64); ref = np.asarray(ref, np.float64)
+    rms = np.sqrt(np.mean(ref ** 2))
+    bad = np.abs(mine - ref) > 2e-2 * np.abs(ref) + 2e-2 * rms
+    assert not bad.any(), f"{what}: {bad.sum()} / {bad.size} outside 2e-2; max {np.abs(mine - ref).max():.4g}, rms {rms:.4g}"
+
+
+def att_needs_reset(heads, kv_heads, longest, grid, bsz=1):
+    """decode_step_sched.h att_needs_reset: whether exl_decode_step resets the attention-partial table before a launch whose longest
+    context is `longest`.  The attention phase has bsz x kv_heads x ceil(longest / 16) units (at least one per virtual KV head) for
+    min(grid, bsz x kv_heads x cap) CTAs, cap 16 per KV head under grouped-query attention and 7 per head without; with two or more
+    units per head and fewer units than CTAs, some CTA inside a head's range owns none (tests/test_batch_schedule.py proves this
+    restatement against the header)."""
+    nph = max(1, (longest + 15) // 16)
+    cap = 16 if kv_heads < heads else 7
+    return nph >= 2 and bsz * kv_heads * nph < min(grid, bsz * kv_heads * cap)
+
+
 def ulp_diff_f16(a, b):
     """Distance in fp16 ulps (monotone integer mapping of the bit patterns)."""
     def key(x):

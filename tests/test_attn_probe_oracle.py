@@ -7,12 +7,7 @@ import pytest
 
 from helpers import (PROBE_GAP, dense_positions, identity_q4, plant_group, plant_probe, probe_expectation, scaled_q_as_k,
                      single_positions, snap_of, synth_q4_ckpt)
-
-
-def _sincos(max_seq, hd):
-    inv = 1.0 / (10000 ** (np.arange(0, hd, 2, dtype=np.float64) / hd))
-    emb = np.concatenate([np.outer(np.arange(max_seq), inv)] * 2, -1)
-    return np.sin(emb).astype(np.float16), np.cos(emb).astype(np.float16)
+from stack_harness import sincos
 
 
 @pytest.mark.parametrize("act", [False, True])
@@ -34,7 +29,7 @@ def test_scaled_q_as_k_is_gamma_q_through_rope(oracle, heads, kv):
     qw, qz, sc, _ = synth_q4_ckpt(hidden, heads * hd, 128, seed=heads + kv)
     kw, kz, ks = scaled_q_as_k(qw, qz, sc, heads, kv, gamma)
     xn = np.random.default_rng(3).standard_normal((1, hidden)).astype(np.float16)
-    sin, cos = _sincos(1024, hd)
+    sin, cos = sincos(1024, hd)
     q = oracle.q4_matmul_f64(xn, qw, qz, sc).astype(np.float16)
     k = oracle.q4_matmul_f64(xn, kw, kz, ks).astype(np.float16)
     q = oracle.rope(q.reshape(1, heads, hd), sin, cos, 1, heads, hd, heads, past).reshape(heads, hd)
@@ -102,7 +97,7 @@ def _cpu_stack(oracle, heads, kv, layers, max_seq, gamma=None, seed=0):
         if gamma is not None:
             L.k = lin(*scaled_q_as_k(L.q.qweight.numpy(), L.q.qzeros.numpy(), L.q.scales.numpy(), heads, kv, gamma))
         Ls.append(L)
-    sin, cos = _sincos(max_seq, hd)
+    sin, cos = sincos(max_seq, hd)
     kc = [torch.zeros((1, kv, max_seq, hd), dtype=torch.float16) for _ in range(layers)]
     return SimpleNamespace(shape=shape, layers=Ls, sin=t(sin), cos=t(cos), max_seq=max_seq, lora=None, lm_head=None,
                            key_cache=kc)

@@ -15,6 +15,7 @@ import subprocess
 import pytest
 
 from exllama_b200.shapes import GQA_SHAPES, SHAPES
+from helpers import att_needs_reset
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SMEM_OPTIN = 232448          # cudaDevAttrMaxSharedMemoryPerBlockOptin on sm_90 (227 KB)
@@ -122,21 +123,14 @@ def test_batch1_small_shapes_match(lib, H, I, heads, kv):
     assert check(lib, H, I, heads, kv, 512, 1, 1, 0, 300) == check_gqa(lib, H, I, heads, kv, 512, 0, 300)
 
 
-def _needs_reset(heads, kv, bsz, longest, grid=SMS):
-    """decode_step_sched.h att_needs_reset over virtual heads: fewer attention units than the CTAs that take part."""
-    nph = max(1, (longest + 15) // 16)
-    cap = 16 if kv < heads else 7
-    return nph >= 2 and bsz * kv * nph < min(grid, bsz * kv * cap)
-
-
 @pytest.mark.parametrize("heads,kv,bsz", [(8, 8, 2), (8, 2, 3), (8, 2, 4), (64, 8, 2)])
 def test_reset_over_virtual_heads(lib, heads, kv, bsz):
     """The table is reset exactly where the predicate (longest context) holds, and nowhere past the short contexts."""
     H, I = (1024, 2816) if heads == 8 else (8192, 28672)
     rc, msg, gaps, resets = check(lib, H, I, heads, kv, 512, bsz, bsz, 0, 1023)
     assert rc == 0, msg
-    assert resets == sum(_needs_reset(heads, kv, bsz, p) for p in range(1024)) and resets > 0
-    last = max(p for p in range(1024) if _needs_reset(heads, kv, bsz, p))
+    assert resets == sum(att_needs_reset(heads, kv, p, SMS, bsz) for p in range(1024)) and resets > 0
+    last = max(p for p in range(1024) if att_needs_reset(heads, kv, p, SMS, bsz))
     rc, msg, gaps, resets = check(lib, H, I, heads, kv, 512, bsz, bsz, last + 1, 1023)
     assert rc == 0 and gaps == 0 and resets == 0
 

@@ -3,15 +3,9 @@ import numpy as np
 import pytest
 
 from helpers import RefLib, assert_close_ref64, to_cuda, ulp_diff_f16
+from stack_harness import sincos
 
 pytestmark = pytest.mark.gpu
-
-
-def _sincos(max_seq, hd):
-    inv = 1.0 / (10000 ** (np.arange(0, hd, 2, dtype=np.float64) / hd))
-    ang = np.outer(np.arange(max_seq), inv)
-    emb = np.concatenate([ang, ang], -1)
-    return np.sin(emb).astype(np.float16), np.cos(emb).astype(np.float16)
 
 
 @pytest.mark.parametrize("rows,dim", [(1, 4096), (3, 5120), (17, 6656), (2, 100)])
@@ -36,7 +30,7 @@ def test_rope_bit_exact(oracle, bsz, q_len, heads, hd, past):
     from exllama_b200 import capi
     rng = np.random.default_rng(7)
     x = rng.standard_normal((bsz, q_len, heads * hd)).astype(np.float16)
-    sin, cos = _sincos(2048, hd)
+    sin, cos = sincos(2048, hd)
     want = oracle.rope(x.reshape(bsz, q_len * heads, hd), sin, cos, bsz, q_len * heads, hd, heads, past).reshape(x.shape)
     tx = to_cuda(x.copy())
     capi.rope_(tx, to_cuda(sin), to_cuda(cos), past, heads, hd)
@@ -121,7 +115,7 @@ def test_q4_attn_block(oracle, act, q_len, past):
     rng = np.random.default_rng(1)
     x = rng.standard_normal((1, q_len, hidden)).astype(np.float16)
     w = (1 + 0.1 * rng.standard_normal(hidden)).astype(np.float16)
-    sin, cos = _sincos(max_seq, hd)
+    sin, cos = sincos(max_seq, hd)
     kc = np.zeros((1, heads, max_seq, hd), np.float16); vc = np.zeros_like(kc)
 
     # oracle sequence: norm -> q,k,v -> fp16 -> rope(q,k) -> cache (q4_attn.cu:130-165)

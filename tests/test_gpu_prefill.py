@@ -19,66 +19,17 @@ import numpy as np
 import pytest
 
 from helpers import REL_TOL, RMS_TOL, adapter_of, assert_close_ref64, oracle_decode_step, oracle_mm, to_cuda
+from stack_harness import lib_state, restore, snapshot, stacks  # noqa: F401
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("lib_state")]
 
+MAX_SEQ = 320                                   # the caches of the small stacks
 LOGIT_TOL = dict(rel=1.5e-2, rms=1.5e-2)       # the decode tests' logit tolerance
 CACHE_TOL = dict(rel=1e-2, rms=1e-2)
 
 
-@pytest.fixture(autouse=True)
-def lib_state():
-    import torch
-    from exllama_b200 import capi
-    capi.check(capi.lib().exl_cleanup())
-    yield capi
-    torch.cuda.synchronize()
-    capi.check(capi.lib().exl_cleanup())
-
-
-@pytest.fixture
-def stacks(lib_state):
-    """make(shape, **DecodeStack kwargs) -> a stack with random caches; every stack made is closed (with its plan) at teardown."""
-    made = []
-
-    def make(shape, **kw):
-        made.append(_mk_stack(shape, **kw))
-        return made[-1]
-    yield make
-    for st in made:
-        if getattr(st, "dplan", None) is not None:
-            st.dplan.close()
-        st.close()
-
-
 def _np(t):
     return t.cpu().numpy()
-
-
-def _shape(kv_heads=8, hidden=1024, inter=2816, heads=8, vocab=2048):
-    from exllama_b200.stack import LlamaShape
-    return LlamaShape("synthetic-prefill", hidden, inter, 2, heads, vocab=vocab, kv_heads=kv_heads)
-
-
-def _mk_stack(shape, gs=128, act=False, max_seq=320, batch=1, seed=3):
-    """Two layers; the caches are filled with random values so that a stray write shows."""
-    import torch
-    from exllama_b200.stack import DecodeStack
-    st = DecodeStack(shape, groupsize=gs, act_order=act, device="cuda:0", max_seq=max_seq, layers=2, seed=seed, batch=batch)
-    g = torch.Generator(device="cuda"); g.manual_seed(seed + 100)
-    for kc, vc in zip(st.key_cache, st.value_cache):
-        kc.copy_((torch.randn(kc.shape, device="cuda", generator=g) * 0.5).half())
-        vc.copy_((torch.randn(vc.shape, device="cuda", generator=g) * 0.5).half())
-    return st
-
-
-def _snap(st):
-    return [(kc.clone(), vc.clone()) for kc, vc in zip(st.key_cache, st.value_cache)]
-
-
-def _restore(st, snap):
-    for (kc, vc), (k0, v0) in zip(zip(st.key_cache, st.value_cache), snap):
-        kc.copy_(k0); vc.copy_(v0)
 
 
 def _x(bsz, T, hidden, seed, scale=0.5):
@@ -282,7 +233,7 @@ def _check_prefill(oracle, st, x, what):
     import torch
     from exllama_b200 import capi
     bsz, T, _ = x.shape
-    snap = _snap(st)
+    snap = snapshot(st)
     logits = st.prefill(x.clone(), last_only=False)
     torch.cuda.synchronize()
     assert capi.last_q4_path() == ("skinny_mma" if bsz * T <= 48 else "tc_gemm"), (what, capi.last_q4_path())
@@ -312,7 +263,7 @@ PREFILL_CASES = [  # (T, kv_heads, groupsize, act_order)
 
 @pytest.mark.parametrize("T,kv,gs,act", PREFILL_CASES)
 def test_prefill_vs_oracle(oracle, stacks, T, kv, gs, act):
-    st = stacks(_shape(kv), gs=gs, act=act, seed=T + kv + gs)
+    st = stacks(kv_heads=kv, max_seq=MAX_SEQ, gs=gs, act=act, seed=T + kv + gs)
     _check_prefill(oracle, st, _x(1, T, 1024, seed=T), f"T {T} kv {kv} g{gs} act {act}")
 
 
@@ -320,12 +271,12 @@ def test_prefill_vs_oracle(oracle, stacks, T, kv, gs, act):
 @pytest.mark.parametrize("T", [5, 130])
 def test_prefill_lora_vs_oracle(oracle, stacks, T):
     """A rank-16 adapter on all seven projections: each adds fp16(fp16(x . A) . B) before the q4 accumulate (q4_matmul_lora)."""
-    st = stacks(_shape(2), seed=40 + T)
+    st = stacks(kv_heads=2, max_seq=MAX_SEQ, seed=40 + T)
     st.add_lora(16, "all", seed=T)
     x = _x(1, T, 1024, seed=T + 1)
-    snap = _snap(st)
+    snap = snapshot(st)
     got = _check_prefill(oracle, st, x, f"LoRA T {T}")
-    _restore(st, snap)
+    restore(st, snap)
     saved, st.lora = st.lora, None
     plain = _np(st.prefill(x.clone(), last_only=False)).reshape(got.shape)
     st.lora = saved
@@ -341,13 +292,13 @@ def test_prefill_then_decode(oracle, stacks, T, kv):
     """Token T after a prefill of T tokens, through the per-op decode_step and the fused step, against the whole-token oracle on the
     post-prefill caches; and the per-op logits against a prefill of all T + 1 tokens, which reads no cache row decode reads."""
     import torch
-    st = stacks(_shape(kv), seed=60 + T + kv)
+    st = stacks(kv_heads=kv, max_seq=MAX_SEQ, seed=60 + T + kv)
     x = _x(1, T + 1, 1024, seed=T + kv)
-    snap0 = _snap(st)
+    snap0 = snapshot(st)
     whole = _np(st.prefill(x.clone())).reshape(-1)
-    _restore(st, snap0)
+    restore(st, snap0)
     st.prefill(x[:, :T].contiguous())
-    snap = _snap(st)
+    snap = snapshot(st)
     xt = x[:, T:T + 1].contiguous()
     _, want, rows = oracle_decode_step(oracle, st, snap, _np(xt), T)
     what = f"T {T} kv {kv}"
@@ -357,7 +308,7 @@ def test_prefill_then_decode(oracle, stacks, T, kv):
     for i, (kc, vc) in enumerate(zip(st.key_cache, st.value_cache)):
         assert_close_ref64(_np(kc[0, :, T]), rows[i][0].astype(np.float64), **CACHE_TOL, what=f"{what} layer {i} new k")
         assert_close_ref64(_np(vc[0, :, T]), rows[i][1].astype(np.float64), **CACHE_TOL, what=f"{what} layer {i} new v")
-    _restore(st, snap)
+    restore(st, snap)
     st.make_plan()
     fused = st.decode_step_fused(xt, T)
     torch.cuda.synchronize()
@@ -369,13 +320,13 @@ def test_batched_prefill_then_fused_batch_step(oracle, stacks):
     sequence fills cache sequence 0 and leaves sequence 1 alone; three sequences do not fit."""
     import torch
     T = 37
-    st = stacks(_shape(2), batch=2, seed=71)
+    st = stacks(kv_heads=2, max_seq=MAX_SEQ, batch=2, seed=71)
     x = _x(2, T + 1, 1024, seed=72)
-    snap0 = _snap(st)
+    snap0 = snapshot(st)
     _check_prefill(oracle, st, x[:1, :T].contiguous(), "batch-2 stack, one sequence")
-    _restore(st, snap0)
+    restore(st, snap0)
     _check_prefill(oracle, st, x[:, :T].contiguous(), "batch 2")
-    snap = _snap(st)
+    snap = snapshot(st)
     st.make_plan()
     xt = x[:, T:T + 1].contiguous()
     got = _np(st.decode_step_fused_batch(xt, [T, T]))
@@ -399,12 +350,12 @@ def test_full_size_prefill_vs_decode(stacks, name, act):
     T = 1920
     st = stacks(s, gs=128, act=act, max_seq=2048, seed=17)
     x = _x(1, T, s.hidden, seed=29)
-    snap0 = _snap(st)
+    snap0 = snapshot(st)
     pos = sorted(set(range(0, T, 97)) | {T - 3, T - 2, T - 1})
     logits = st.prefill(x.clone(), last_only=False)[pos].cpu()
     assert capi.last_q4_path() == "tc_gemm"
-    prefilled = _snap(st)
-    _restore(st, snap0)
+    prefilled = snapshot(st)
+    restore(st, snap0)
     want = []
     for p in range(T):
         lg = st.decode_step(x[:, p:p + 1].clone(), p)

@@ -15,24 +15,16 @@ import pytest
 
 from helpers import assert_close_ref64, oracle_decode_step
 from prefill_oracle import oracle_prefill, prefill_attn_f64
+from stack_harness import lib_state, restore, snapshot, stacks  # noqa: F401
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("lib_state")]
 
 HD = 128
+MAX_SEQ = 384                                   # the caches of the small stacks
 ATTN_TOL = dict(rel=1.5e-3, rms=1.5e-3)        # decode_attn's tolerance
 LOGIT_TOL = dict(rel=1.5e-2, rms=1.5e-2)       # the decode tests' logit tolerance
 CACHE_TOL = dict(rel=1e-2, rms=1e-2)
 NAN_BITS = 0x7D2B                               # a NaN payload no fp16 arithmetic produces
-
-
-@pytest.fixture(autouse=True)
-def lib_state():
-    import torch
-    from exllama_b200 import capi
-    capi.check(capi.lib().exl_cleanup())
-    yield capi
-    torch.cuda.synchronize()
-    capi.check(capi.lib().exl_cleanup())
 
 
 def _np(t):
@@ -172,42 +164,6 @@ def test_kernel_argument_errors():
 
 
 # ---- DecodeStack.prefill at past_len > 0 --------------------------------------------------------------------------------------------
-def _shape(kv_heads=8, hidden=1024, inter=2816, heads=8, vocab=2048):
-    from exllama_b200.stack import LlamaShape
-    return LlamaShape("synthetic-prefill-past", hidden, inter, 2, heads, vocab=vocab, kv_heads=kv_heads)
-
-
-@pytest.fixture
-def stacks(lib_state):
-    made = []
-
-    def make(shape, gs=128, act=False, max_seq=384, batch=1, seed=3):
-        """Two layers; the caches hold random values so that a stray write or read shows."""
-        import torch
-        from exllama_b200.stack import DecodeStack
-        st = DecodeStack(shape, groupsize=gs, act_order=act, device="cuda:0", max_seq=max_seq, layers=2, seed=seed, batch=batch)
-        g = torch.Generator(device="cuda"); g.manual_seed(seed + 100)
-        for kc, vc in zip(st.key_cache, st.value_cache):
-            kc.copy_((torch.randn(kc.shape, device="cuda", generator=g) * 0.5).half())
-            vc.copy_((torch.randn(vc.shape, device="cuda", generator=g) * 0.5).half())
-        made.append(st)
-        return st
-    yield make
-    for st in made:
-        if getattr(st, "dplan", None) is not None:
-            st.dplan.close()
-        st.close()
-
-
-def _snap(st):
-    return [(kc.clone(), vc.clone()) for kc, vc in zip(st.key_cache, st.value_cache)]
-
-
-def _restore(st, snap):
-    for (kc, vc), (k0, v0) in zip(zip(st.key_cache, st.value_cache), snap):
-        kc.copy_(k0); vc.copy_(v0)
-
-
 def _x(bsz, T, hidden, seed, scale=0.5):
     import torch
     g = torch.Generator(device="cuda"); g.manual_seed(seed)
@@ -219,7 +175,7 @@ def _check_prefill(oracle, st, x, past_len, what, seq=0):
     position, the new cache rows [past_len, past_len + T) of every layer, every other row of every sequence bitwise unchanged."""
     import torch
     bsz, T, _ = x.shape
-    snap = _snap(st)
+    snap = snapshot(st)
     logits = st.prefill(x.clone(), past_len, last_only=False, seq=seq)
     torch.cuda.synchronize()
     logits = _np(logits).reshape(bsz, T, -1)
@@ -229,7 +185,7 @@ def _check_prefill(oracle, st, x, past_len, what, seq=0):
             for name, c, c0 in (("k", kc, snap[i][0]), ("v", vc, snap[i][1])):
                 assert torch.equal(c[b, :, :lo], c0[b, :, :lo]) and torch.equal(c[b, :, hi:], c0[b, :, hi:]), \
                     f"{what}: layer {i} {name} cache of sequence {b}: a row outside [{lo}, {hi}) was written"
-    caches = _snap(st)
+    caches = snapshot(st)
     for b in range(bsz):
         want, rows = oracle_prefill(oracle, st, caches, _np(x[b]), past_len, seq + b, bsz * T)
         assert_close_ref64(logits[b], want, **LOGIT_TOL, what=f"{what} seq {b} logits")
@@ -249,7 +205,7 @@ STACK_CASES = [  # (past_len, T, kv_heads, groupsize, act_order)
 
 @pytest.mark.parametrize("past_len,T,kv,gs,act", STACK_CASES)
 def test_prefill_past_vs_oracle(oracle, stacks, past_len, T, kv, gs, act):
-    st = stacks(_shape(kv), gs=gs, act=act, seed=past_len + T + kv)
+    st = stacks(kv_heads=kv, gs=gs, act=act, seed=past_len + T + kv, max_seq=MAX_SEQ)
     _check_prefill(oracle, st, _x(1, T, 1024, seed=T + past_len), past_len, f"past {past_len} T {T} kv {kv} g{gs} act {act}")
 
 
@@ -258,7 +214,7 @@ def test_follow_up_turn(oracle, stacks, kv):
     """Prefill T0 tokens, three fused decode steps, prefill T1 more at the current past_len, one fused decode step; each step against
     the oracle on the caches it started from."""
     import torch
-    st = stacks(_shape(kv), seed=80 + kv)
+    st = stacks(kv_heads=kv, seed=80 + kv, max_seq=MAX_SEQ)
     T0, T1, steps = 50, 70, 3
     x = _x(1, T0 + steps + T1 + 1, 1024, seed=81 + kv)
     _check_prefill(oracle, st, x[:, :T0].contiguous(), 0, f"kv {kv} first turn")
@@ -266,7 +222,7 @@ def test_follow_up_turn(oracle, stacks, kv):
     p = T0
 
     def fused_step(p):
-        snap = _snap(st)
+        snap = snapshot(st)
         xt = x[:, p:p + 1].contiguous()
         _, want, _ = oracle_decode_step(oracle, st, snap, _np(xt), p)
         got = st.decode_step_fused(xt, p)
@@ -283,12 +239,12 @@ def test_follow_up_turn(oracle, stacks, kv):
 @pytest.mark.parametrize("kv,p", [(8, 1), (2, 77), (8, 200)])
 def test_single_token_prefill_matches_decode_step(stacks, kv, p):
     """T = 1 at past_len p through prefill agrees with decode_step at p (from the same caches)."""
-    st = stacks(_shape(kv), seed=90 + p)
+    st = stacks(kv_heads=kv, seed=90 + p, max_seq=MAX_SEQ)
     x = _x(1, 1, 1024, seed=p)
-    snap = _snap(st)
+    snap = snapshot(st)
     got = _np(st.prefill(x.clone(), p)).reshape(-1)
-    pre = _snap(st)
-    _restore(st, snap)
+    pre = snapshot(st)
+    restore(st, snap)
     want = _np(st.decode_step(x.clone(), p)).reshape(-1)
     assert_close_ref64(got, want.astype(np.float64), **LOGIT_TOL, what=f"kv {kv} prefill T=1 vs decode_step at {p}")
     for (kp, vp), kc, vc in zip(pre, st.key_cache, st.value_cache):
@@ -300,13 +256,13 @@ def test_prefill_into_one_sequence_of_a_batch(oracle, stacks):
     """batch=3: sequence 1 gets a prefill at past 60 while sequences 0 and 2 sit at 40 and 90; their caches stay bitwise unchanged.
     One fused batch step at the three past_lens then matches oracle_decode_step for each sequence."""
     import torch
-    st = stacks(_shape(2), batch=3, seed=95)
+    st = stacks(kv_heads=2, batch=3, seed=95, max_seq=MAX_SEQ)
     lens = [40, 60, 90]
     T = 33
     x = _x(1, T, 1024, seed=96)
     _check_prefill(oracle, st, x, lens[1], "seq 1 of 3", seq=1)
     lens[1] += T
-    snap = _snap(st)
+    snap = snapshot(st)
     st.make_plan()
     xt = _x(3, 1, 1024, seed=97)
     got = _np(st.decode_step_fused_batch(xt, lens))
@@ -330,11 +286,11 @@ def test_full_size_chunked_vs_single_prefill(stacks, name):
     T, C = 1920, 512
     st = stacks(s, gs=128, max_seq=2048, seed=17)
     x = _x(1, T, s.hidden, seed=29)
-    snap0 = _snap(st)
+    snap0 = snapshot(st)
     pos = sorted(set(range(0, T, 97)) | {T - 3, T - 2, T - 1})
     whole = st.prefill(x.clone(), last_only=False)[pos].cpu()
-    single = _snap(st)
-    _restore(st, snap0)
+    single = snapshot(st)
+    restore(st, snap0)
     parts = []
     for c0 in range(0, T, C):
         lg = st.prefill(x[:, c0:c0 + C].contiguous(), c0, last_only=False)

@@ -15,24 +15,16 @@ import pytest
 
 from helpers import assert_close_ref64, oracle_decode_step
 from prefill_oracle import oracle_prefill, prefill_attn_f64
+from stack_harness import lib_state, restore, snapshot, stacks  # noqa: F401
 
-pytestmark = pytest.mark.gpu
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("lib_state")]
 
 HD = 128
+MAX_SEQ = 384                                   # the caches of the small stacks
 CAP = 64                                        # EXL_RAGGED_MAX_SEQ
 ATTN_TOL = dict(rel=1.5e-3, rms=1.5e-3)
 LOGIT_TOL = dict(rel=1.5e-2, rms=1.5e-2)
 CACHE_TOL = dict(rel=1e-2, rms=1e-2)
-
-
-@pytest.fixture(autouse=True)
-def lib_state():
-    import torch
-    from exllama_b200 import capi
-    capi.check(capi.lib().exl_cleanup())
-    yield capi
-    torch.cuda.synchronize()
-    capi.check(capi.lib().exl_cleanup())
 
 
 def _np(t):
@@ -242,42 +234,6 @@ def test_argument_errors():
 
 
 # ---- DecodeStack.prefill_ragged ------------------------------------------------------------------------------------------------------
-def _shape(kv_heads=8, hidden=1024, inter=2816, heads=8, vocab=2048):
-    from exllama_b200.stack import LlamaShape
-    return LlamaShape("synthetic-prefill-ragged", hidden, inter, 2, heads, vocab=vocab, kv_heads=kv_heads)
-
-
-@pytest.fixture
-def stacks(lib_state):
-    made = []
-
-    def make(shape, gs=128, act=False, max_seq=384, batch=1, seed=3):
-        """Two layers; the caches hold random values so that a stray write or read shows."""
-        import torch
-        from exllama_b200.stack import DecodeStack
-        st = DecodeStack(shape, groupsize=gs, act_order=act, device="cuda:0", max_seq=max_seq, layers=2, seed=seed, batch=batch)
-        g = torch.Generator(device="cuda"); g.manual_seed(seed + 100)
-        for kc, vc in zip(st.key_cache, st.value_cache):
-            kc.copy_((torch.randn(kc.shape, device="cuda", generator=g) * 0.5).half())
-            vc.copy_((torch.randn(vc.shape, device="cuda", generator=g) * 0.5).half())
-        made.append(st)
-        return st
-    yield make
-    for st in made:
-        if getattr(st, "dplan", None) is not None:
-            st.dplan.close()
-        st.close()
-
-
-def _snap(st):
-    return [(kc.clone(), vc.clone()) for kc, vc in zip(st.key_cache, st.value_cache)]
-
-
-def _restore(st, snap):
-    for (kc, vc), (k0, v0) in zip(zip(st.key_cache, st.value_cache), snap):
-        kc.copy_(k0); vc.copy_(v0)
-
-
 def _x(T, hidden, seed, scale=0.5):
     import torch
     g = torch.Generator(device="cuda"); g.manual_seed(seed)
@@ -300,12 +256,12 @@ def test_prefill_ragged_vs_oracle(oracle, stacks, kv, gs, act, rank, q_lens, pas
     """Logits at every position and the new cache rows of every sequence against oracle_prefill with M = T; every other row of
     every cache sequence bitwise unchanged."""
     import torch
-    st = stacks(_shape(kv), gs=gs, act=act, batch=3, seed=sum(q_lens) + kv)
+    st = stacks(kv_heads=kv, gs=gs, act=act, max_seq=MAX_SEQ, batch=3, seed=sum(q_lens) + kv)
     if rank:
         st.add_lora(rank, targets="all", seed=rank)
     T = sum(q_lens)
     x = _x(T, 1024, seed=T)
-    snap = _snap(st)
+    snap = snapshot(st)
     logits = _np(st.prefill_ragged(x.clone(), q_lens, past_lens, seqs, last_only=False))
     torch.cuda.synchronize()
     what = f"kv {kv} g{gs} act {act} lora {rank} q_lens {q_lens} past {past_lens}"
@@ -316,7 +272,7 @@ def test_prefill_ragged_vs_oracle(oracle, stacks, kv, gs, act, rank, q_lens, pas
             for name, c, c0 in (("k", kc, snap[i][0]), ("v", vc, snap[i][1])):
                 assert torch.equal(c[b, :, :lo], c0[b, :, :lo]) and torch.equal(c[b, :, hi:], c0[b, :, hi:]), \
                     f"{what}: layer {i} {name} cache of sequence {b}: a row outside [{lo}, {hi}) was written"
-    caches = _snap(st)
+    caches = snapshot(st)
     off = _offsets(q_lens)
     for j, (ql, pl, cs) in enumerate(zip(q_lens, past_lens, seqs)):
         want, rows = oracle_prefill(oracle, st, caches, _np(x[off[j]:off[j + 1]]), pl, cs, T)
@@ -330,12 +286,12 @@ def test_prefill_ragged_last_only_and_errors(stacks):
     """last_only returns each sequence's last row of the full logits (same caches, up to the lm_head GEMM's rounding at another M);
     argument errors are ValueErrors."""
     import torch
-    st = stacks(_shape(2), batch=3, seed=41)
+    st = stacks(kv_heads=2, batch=3, seed=41, max_seq=MAX_SEQ)
     q_lens, past_lens = [9, 60, 1], [3, 0, 100]
     x = _x(sum(q_lens), 1024, seed=42)
-    snap = _snap(st)
+    snap = snapshot(st)
     full = st.prefill_ragged(x.clone(), q_lens, past_lens, last_only=False)
-    _restore(st, snap)
+    restore(st, snap)
     last = st.prefill_ragged(x.clone(), q_lens, past_lens)
     torch.cuda.synchronize()
     ends = torch.tensor(_offsets(q_lens)[1:] - 1, device="cuda")
@@ -354,11 +310,11 @@ def test_serving_flow_into_fused_batch_step(oracle, stacks):
     """batch=4: one prefill_ragged of prompts of 1, 77, 200 and 513 tokens at past 0, 0, 37 and 300, then one fused batch decode step
     at the resulting past_lens, against the whole-token oracle for each sequence."""
     import torch
-    st = stacks(_shape(2), batch=4, max_seq=1024, seed=61)
+    st = stacks(kv_heads=2, batch=4, max_seq=1024, seed=61)
     q_lens, past_lens = [1, 77, 200, 513], [0, 0, 37, 300]
     st.prefill_ragged(_x(sum(q_lens), 1024, seed=62), q_lens, past_lens)
     lens = [p + q for p, q in zip(past_lens, q_lens)]
-    snap = _snap(st)
+    snap = snapshot(st)
     st.make_plan()
     xt = _x(4, 1024, seed=63).view(4, 1, 1024)
     got = _np(st.decode_step_fused_batch(xt, lens))
@@ -380,12 +336,12 @@ def test_full_size_ragged_vs_prefill_per_prompt(stacks, name):
     st = stacks(s, gs=128, max_seq=2048, batch=5, seed=17)
     x = _x(T, s.hidden, seed=29)
     off = _offsets(q_lens)
-    snap0 = _snap(st)
+    snap0 = snapshot(st)
     pos = sorted(set(range(0, T, 97)) | {T - 1} | set(int(o) - 1 for o in off[1:]))
     loop = torch.cat([st.prefill(x[off[j]:off[j + 1]].view(1, -1, s.hidden).contiguous(), past_lens[j], last_only=False, seq=seqs[j])
                       for j in range(len(q_lens))])[pos].cpu()
-    looped = _snap(st)
-    _restore(st, snap0)
+    looped = snapshot(st)
+    restore(st, snap0)
     ragged = st.prefill_ragged(x.clone(), q_lens, past_lens, seqs, last_only=False)[pos].cpu()
     torch.cuda.synchronize()
     assert_close_ref64(ragged.numpy(), loop.numpy().astype(np.float64), rel=2e-2, rms=2e-2, what=f"{name} ragged vs per-prompt logits")

@@ -17,16 +17,10 @@ import pytest
 from helpers import (GOLDEN, adapter_of, assert_close_ref64, assert_within_bound, gen_x, oracle_decode_step,
                      outlier_channels, q4_column_sample, quant_error_bound, sample_cols, synth_q4_ckpt, synth_q4_saturated, to_cuda,
                      ulp_diff_f16)
+from stack_harness import fused_step, lib_state, per_op, restore, sincos, snapshot, stacks  # noqa: F401
 
-pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(autouse=True)
-def _cleanup():
-    """No q4 handle or borrowed buffer outlives a test (the 70B-width matrices here are large)."""
-    from exllama_b200 import capi
-    yield
-    capi.check(capi.lib().exl_cleanup())
+# No q4 handle or borrowed buffer outlives a test (the 70B-width matrices here are large).
+pytestmark = [pytest.mark.gpu, pytest.mark.usefixtures("lib_state")]
 
 
 def _q4(capi, qw, qz, sc, g_idx):
@@ -179,13 +173,6 @@ def _block_weights(hidden, inter, gs, seed, kv=None, act=False):
     return t
 
 
-def _sincos(max_seq, hd):
-    inv = 1.0 / (10000.0 ** (np.arange(0, hd, 2) / hd))
-    f = np.outer(np.arange(max_seq), inv)
-    emb = np.concatenate([f, f], axis=1)
-    return np.sin(emb).astype(np.float16), np.cos(emb).astype(np.float16)
-
-
 def _rope_allowance(B, ref, sin, cos, heads, hd, past):
     """The bound of q / k after rope: rope mixes element i with i +- 64 by |cos| and |sin| (the bound of each enters with those
     weights).  The fp16 roundings: the oracle rounds ref where the kernel rounds its own result (2^-11 |ref|, once), and rope's
@@ -218,7 +205,7 @@ def test_q4_attn_and_mlp_blocks_outliers(oracle, gs, kvh, act):
     t = _block_weights(hidden, inter, gs, seed=500 + (gs or 1), kv=kvw, act=act)
     x = gen_x("outlier1000", 1, hidden, seed=5, channels=outlier_channels(hidden, gs, 1)).reshape(1, 1, hidden)
     w = (1 + 0.1 * np.random.default_rng(6).standard_normal(hidden)).astype(np.float16)
-    sin, cos = _sincos(max_seq, hd)
+    sin, cos = sincos(max_seq, hd)
 
     def mk(n):
         return _q4(capi, *t[n])
@@ -284,33 +271,15 @@ def test_q4_attn_and_mlp_blocks_outliers(oracle, gs, kvh, act):
 
 
 # ------------------------------------------------------------------------------------- (d) the persistent step with one group
-def _mk_stack(hidden, inter, layers, heads, kv_heads, gs, max_seq, vocab=2048, seed=3, act=False, batch=1):
-    import torch
-    from exllama_b200.stack import DecodeStack, LlamaShape
-    shape = LlamaShape("synthetic-one-group", hidden, inter, layers, heads, vocab=vocab, kv_heads=kv_heads)
-    st = DecodeStack(shape, groupsize=gs, act_order=act, device="cuda:0", max_seq=max_seq, seed=seed, batch=batch)
-    g = torch.Generator(device="cuda"); g.manual_seed(seed + 100)
-    for kc, vc in zip(st.key_cache, st.value_cache):
-        kc.copy_((torch.randn(kc.shape, device="cuda", generator=g) * 0.5).half())
-        vc.copy_((torch.randn(vc.shape, device="cuda", generator=g) * 0.5).half())
-    return st
-
-
-def _check_step(oracle, st, xs, pasts, what, vs_oracle=True):
-    """Fused step vs the per-op path (and the float64 oracle composition) for every sequence of xs [bsz, 1, hidden]."""
+def _check_step(oracle, st, xs, pasts, what):
+    """Fused step vs the per-op path and the float64 oracle composition for every sequence of xs [bsz, 1, hidden].  The two kernels
+    quantise x with different steps (32767 and 32639 per segment), so the fused step meets the per-op path on the logits only."""
     import torch
     bsz = len(pasts)
-    snap = [(kc.clone(), vc.clone()) for kc, vc in zip(st.key_cache, st.value_cache)]
-
-    def restore():
-        for (kc, vc), (k0, v0) in zip(zip(st.key_cache, st.value_cache), snap):
-            kc.copy_(k0); vc.copy_(v0)
-    per_op = []
-    for b, past in enumerate(pasts):
-        per_op.append(st.decode_step(xs[b:b + 1].clone(), past, seq=b).cpu().numpy().reshape(-1))
-    restore()
+    snap = snapshot(st)
+    per_op_logits = [lg.cpu().numpy().reshape(-1) for lg in per_op(st, snap, xs, pasts)[0]]
     st.make_plan()
-    logits = (st.decode_step_fused_batch(xs, pasts) if bsz > 1 else st.decode_step_fused(xs[:1], pasts[0]).view(1, -1)).cpu().numpy()
+    logits = fused_step(st, xs, pasts).cpu().numpy()
     torch.cuda.synchronize()
     got_x = st._plan_xout.view(-1, st.shape.hidden)[:bsz].cpu().numpy()
     new_rows = [[(kc[b, :, pasts[b]].cpu().numpy(), vc[b, :, pasts[b]].cpu().numpy()) for kc, vc in zip(st.key_cache, st.value_cache)]
@@ -318,17 +287,15 @@ def _check_step(oracle, st, xs, pasts, what, vs_oracle=True):
     for b in range(bsz):
         w = f"{what} seq {b} (ctx {pasts[b]})"
         assert np.isfinite(logits[b]).all(), w
-        assert_close_ref64(logits[b], per_op[b].astype(np.float64), rel=1.5e-2, rms=1.5e-2, what=f"{w} logits vs per-op")
-        if vs_oracle:
-            want_x, want_logits, rows = oracle_decode_step(oracle, st, snap, xs[b].cpu().numpy(), pasts[b], b)
-            assert_close_ref64(got_x[b], want_x.reshape(-1).astype(np.float64), rel=1e-2, rms=1e-2, what=f"{w} final hidden vs oracle")
-            assert_close_ref64(logits[b], want_logits.reshape(-1), rel=1.5e-2, rms=1.5e-2, what=f"{w} logits vs oracle")
-            assert_close_ref64(per_op[b], want_logits.reshape(-1), rel=1.5e-2, rms=1.5e-2, what=f"{w} per-op logits vs oracle")
-            for i in range(len(st.layers)):
-                assert_close_ref64(new_rows[b][i][0], rows[i][0].astype(np.float64), rel=1e-2, rms=1e-2, what=f"{w} layer {i} new k")
-                assert_close_ref64(new_rows[b][i][1], rows[i][1].astype(np.float64), rel=1e-2, rms=1e-2, what=f"{w} layer {i} new v")
-    st.dplan.close()
-    restore()
+        assert_close_ref64(logits[b], per_op_logits[b].astype(np.float64), rel=1.5e-2, rms=1.5e-2, what=f"{w} logits vs per-op")
+        want_x, want_logits, rows = oracle_decode_step(oracle, st, snap, xs[b].cpu().numpy(), pasts[b], b)
+        assert_close_ref64(got_x[b], want_x.reshape(-1).astype(np.float64), rel=1e-2, rms=1e-2, what=f"{w} final hidden vs oracle")
+        assert_close_ref64(logits[b], want_logits.reshape(-1), rel=1.5e-2, rms=1.5e-2, what=f"{w} logits vs oracle")
+        assert_close_ref64(per_op_logits[b], want_logits.reshape(-1), rel=1.5e-2, rms=1.5e-2, what=f"{w} per-op logits vs oracle")
+        for i in range(len(st.layers)):
+            assert_close_ref64(new_rows[b][i][0], rows[i][0].astype(np.float64), rel=1e-2, rms=1e-2, what=f"{w} layer {i} new k")
+            assert_close_ref64(new_rows[b][i][1], rows[i][1].astype(np.float64), rel=1e-2, rms=1e-2, what=f"{w} layer {i} new v")
+    restore(st, snap)
 
 
 def _xs(bsz, hidden, seed, scale=0.5, outliers=()):
@@ -339,16 +306,15 @@ def _xs(bsz, hidden, seed, scale=0.5, outliers=()):
     return torch.from_numpy(x.astype(np.float16)).cuda()
 
 
-def test_one_group_stack_layout(oracle):
+def test_one_group_stack_layout(oracle, stacks):
     """DecodeStack(groupsize=None): every matrix holds one group (GPTQ groupsize -1), act-order g_idx is all zeros, and tensor
     parallelism is refused."""
     from exllama_b200.stack import DecodeStack, LlamaShape
-    st = _mk_stack(1024, 2816, 1, 8, 2, None, 64, act=True)
+    st = stacks(layers=1, kv_heads=2, gs=None, max_seq=64, act=True)
     for n in st.PROJ:
         lin = getattr(st.layers[0], n)
         assert lin.qzeros.shape[0] == 1 and lin.scales.shape[0] == 1, n
         assert lin.g_idx is not None and not lin.g_idx.any(), n
-    st.close()
     with pytest.raises(NotImplementedError, match="one quantisation group"):
         DecodeStack(LlamaShape("x", 1024, 2816, 1, 8, vocab=2048), groupsize=None, tp_rank=0, tp_size=2)
 
@@ -356,41 +322,36 @@ def test_one_group_stack_layout(oracle):
 @pytest.mark.parametrize("act", [False, True])
 @pytest.mark.parametrize("kv", [8, 2])
 @pytest.mark.parametrize("past", [0, 37, 200])
-def test_fused_step_one_group(oracle, kv, act, past):
-    st = _mk_stack(1024, 2816, 2, 8, kv, None, 256, seed=40 + kv, act=act)
+def test_fused_step_one_group(oracle, stacks, kv, act, past):
+    st = stacks(kv_heads=kv, gs=None, seed=40 + kv, act=act)
     _check_step(oracle, st, _xs(1, 1024, past + kv), [past], f"one group kv{kv} act{act}")
-    st.close()
 
 
-def test_fused_step_one_group_batch(oracle):
-    st = _mk_stack(1024, 2816, 2, 8, 2, None, 256, seed=61, batch=3)
+def test_fused_step_one_group_batch(oracle, stacks):
+    st = stacks(kv_heads=2, gs=None, seed=61, batch=3)
     _check_step(oracle, st, _xs(3, 1024, 62), [5, 200, 37], "one group, batch of 3")
-    st.close()
 
 
-def test_fused_step_one_group_lora(oracle):
-    st = _mk_stack(1024, 2816, 2, 8, 2, None, 256, seed=63)
+def test_fused_step_one_group_lora(oracle, stacks):
+    st = stacks(kv_heads=2, gs=None, seed=63)
     st.add_lora(16, targets="all", alpha=128, seed=2)
     _check_step(oracle, st, _xs(1, 1024, 64, scale=0.05), [37], "one group, LoRA")
     assert adapter_of(st, 0, "down") is not None
-    st.close()
 
 
-def test_fused_step_one_group_70b_shape(oracle):
+def test_fused_step_one_group_70b_shape(oracle, stacks):
     """Llama-2 70B widths (hidden 8192, inter 28672, 64 query heads over 8 KV heads), 2 layers at ctx 1920, one group."""
     from exllama_b200.shapes import GQA_SHAPES
     s = GQA_SHAPES["70b"]
-    st = _mk_stack(s.hidden, s.inter, 2, s.heads, s.kv_heads, None, 2048, vocab=s.vocab, seed=17)
+    st = stacks(hidden=s.hidden, inter=s.inter, heads=s.heads, kv_heads=s.kv_heads, gs=None, max_seq=2048, vocab=s.vocab, seed=17)
     _check_step(oracle, st, _xs(1, s.hidden, 70), [1920], "70B one group")
-    st.close()
 
 
 @pytest.mark.parametrize("gs", [128, None])
-def test_fused_step_outlier_embedding(oracle, gs):
+def test_fused_step_outlier_embedding(oracle, stacks, gs):
     """An embedding row with two channels at 300x the rest (a "massive activation"): both paths against the oracle."""
-    st = _mk_stack(1024, 2816, 2, 8, 2, gs, 256, seed=80)
+    st = stacks(kv_heads=2, gs=gs, seed=80)
     _check_step(oracle, st, _xs(1, 1024, 81, outliers=(77, 640)), [37], f"outlier embedding g{gs}")
-    st.close()
 
 
 # ------------------------------------------------------------------------------------------ (e) against the reference kernel

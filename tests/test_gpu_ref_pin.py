@@ -17,7 +17,8 @@ import os
 import numpy as np
 import pytest
 
-from helpers import GOLDEN, assert_close_ref64, golden_cols, to_cuda, ulp_diff_f16
+from helpers import GOLDEN, assert_close_ref64, close_to_reference, golden_cols, to_cuda, ulp_diff_f16
+from stack_harness import sincos
 
 pytestmark = pytest.mark.gpu
 
@@ -25,13 +26,6 @@ pytestmark = pytest.mark.gpu
 @pytest.fixture(scope="module")
 def golden():
     return np.load(os.path.join(GOLDEN, "ref_gpu.npz"))
-
-
-def _sincos(max_seq, hd):
-    inv = 1.0 / (10000 ** (np.arange(0, hd, 2, dtype=np.float64) / hd))
-    ang = np.outer(np.arange(max_seq), inv)
-    emb = np.concatenate([ang, ang], -1)
-    return np.sin(emb).astype(np.float16), np.cos(emb).astype(np.float16)
 
 
 @pytest.mark.parametrize("rows,dim", [(1, 4096), (1, 5120), (3, 6656), (7, 8192), (17, 4096)])
@@ -58,7 +52,7 @@ def test_rope_three_way_bit_exact(oracle, golden, bsz, q_len, heads, hd, past):
     from exllama_b200 import capi
     rng = np.random.default_rng(17 + past)
     x = rng.standard_normal((bsz, q_len, heads * hd)).astype(np.float16)
-    sin, cos = _sincos(2048, hd)
+    sin, cos = sincos(2048, hd)
     want = oracle.rope(x.reshape(bsz, q_len * heads, hd), sin, cos, bsz, q_len * heads, hd, heads, past).reshape(x.shape)
     ts, tc = to_cuda(sin, cos)
     ref = golden[f"rope_{bsz}_{q_len}_{heads}_{hd}_{past}"]
@@ -116,13 +110,6 @@ def _ours(capi, t):
     return capi.Q4(*to_cuda(qw.copy(), qz, sc), None if g is None else torch.from_numpy(g))
 
 
-def _close_to_reference(mine, ref, what):
-    mine = np.asarray(mine, np.float64); ref = np.asarray(ref, np.float64)
-    rms = np.sqrt(np.mean(ref ** 2))
-    bad = np.abs(mine - ref) > 2e-2 * np.abs(ref) + 2e-2 * rms
-    assert not bad.any(), f"{what}: {bad.sum()} / {bad.size} outside 2e-2 of the reference kernel; max {np.abs(mine - ref).max():.4g}, rms {rms:.4g}"
-
-
 @pytest.mark.parametrize("act", [False, True])
 @pytest.mark.parametrize("q_len,past", [(1, 0), (1, 37), (2, 5)])
 def test_q4_attn_vs_reference_block(oracle, golden, act, q_len, past):
@@ -134,7 +121,7 @@ def test_q4_attn_vs_reference_block(oracle, golden, act, q_len, past):
     rng = np.random.default_rng(11)
     x = rng.standard_normal((1, q_len, hidden)).astype(np.float16)
     w = (1 + 0.1 * rng.standard_normal(hidden)).astype(np.float16)
-    sin, cos = _sincos(max_seq, hd)
+    sin, cos = sincos(max_seq, hd)
     ts, tc, tw = to_cuda(sin, cos, w)
     Qa, Ka, Va = (_ours(capi, t[n]) for n in ("q", "k", "v"))
 
@@ -148,7 +135,7 @@ def test_q4_attn_vs_reference_block(oracle, golden, act, q_len, past):
     outs["ours"] = [a.cpu().numpy() for a in (q, k, v, kc, vc, tx)]
     outs["ref"] = [golden[f"q4_attn_{q_len}_{past}_{int(act)}_{n}"] for n in ("q", "k", "v", "kc", "vc", "x")]
     for i, name in enumerate(("q", "k", "v")):          # the caches are compared row by row below (mostly zeros: no meaningful rms)
-        _close_to_reference(outs["ours"][i], outs["ref"][i], f"q4_attn {name}")
+        close_to_reference(outs["ours"][i], outs["ref"][i], f"q4_attn {name}")
     np.testing.assert_array_equal(outs["ours"][5], x)            # x itself is not modified by q4_attn
     np.testing.assert_array_equal(outs["ref"][5], x)
     # cache layout: rows past..past+q_len hold k / v exactly, everything else untouched -- in both implementations
@@ -162,7 +149,7 @@ def test_q4_attn_vs_reference_block(oracle, golden, act, q_len, past):
     # the oracle composition pins the same block: v is a plain projection of the normalised x
     xn, _ = oracle.rms_norm(x.reshape(q_len, hidden), w, 1e-6)
     v64 = oracle.ref64_with_act_order(xn, *t["v"])
-    _close_to_reference(v64, outs["ref"][2].reshape(q_len, hidden), "oracle v vs reference")
+    close_to_reference(v64, outs["ref"][2].reshape(q_len, hidden), "oracle v vs reference")
     e_mine = np.sqrt(np.mean((outs["ours"][2].reshape(q_len, hidden) - v64) ** 2))
     e_ref = np.sqrt(np.mean((outs["ref"][2].reshape(q_len, hidden) - v64) ** 2))
     assert e_mine <= e_ref * 1.05 + 1e-6, (e_mine, e_ref)
@@ -186,8 +173,8 @@ def test_q4_attn_2_and_mlp_vs_reference_block(oracle, golden, act, rows):
     x_ours = to_cuda(x.copy()); capi.q4_attn_2(x_ours, ta, Oa)
     x_ref = golden[f"q4_attn_2_{rows}_{int(act)}"]
     want = oracle.ref64_with_act_order(attn, *t["o"], acc_in=x)
-    _close_to_reference(x_ours.cpu().numpy(), x_ref, "q4_attn_2")
-    _close_to_reference(want, x_ref, "oracle attn_2 vs reference")
+    close_to_reference(x_ours.cpu().numpy(), x_ref, "q4_attn_2")
+    close_to_reference(want, x_ref, "oracle attn_2 vs reference")
     assert_close_ref64(x_ours.cpu().numpy(), want, what="attn_2 vs oracle")
 
     x_ours = to_cuda(x.copy()); capi.q4_mlp(x_ours, tw, 1e-6, Ga, Ua, Da)

@@ -29,6 +29,12 @@ def ragged(q_lens, past_lens, cache_seqs):
     r._keep = arrs
     return r
 
+class ExlSampleParams(C.Structure):
+    """exl_sample_params (include/exl_b200.h): the settings of one exl_sample call."""
+    _fields_ = [("temperature", f32), ("top_k", i32), ("top_p", f32), ("min_p", f32), ("typical", f32),
+                ("rep_penalty_max", f32), ("rep_sustain", i32), ("rep_decay", i32), ("bos_token_id", i32),
+                ("banned", vp), ("n_banned", i32)]
+
 # name -> (restype, argtypes); mirrors include/exl_b200.h one to one
 SIGNATURES = {
     "exl_last_error": (C.c_char_p, []),
@@ -67,6 +73,7 @@ SIGNATURES = {
     "exl_q4_mlp_tp": (i32, [vp, vp, f32, vp, vp, vp, i32, i32, i32, i32, vp]),
     "exl_rep_penalty": (i32, [i32, vp, vp, f32, i32, i32, i32]),
     "exl_apply_rep_penalty": (i32, [i32, vp, f32, i32, i32, i32, vp]),
+    "exl_sample": (i32, [vp, i32, i32, i64, vp, i64, C.POINTER(i32), C.POINTER(ExlSampleParams), vp, vp, vp, vp, vp]),
     "exl_q4_matmul_host": (i32, [vp, i32, vp, vp, vp, vp, vp]),
     "exl_decode_plan_create": (i32, [vp, C.POINTER(vp)]),
     "exl_decode_plan_create_batch": (i32, [vp, i32, C.POINTER(vp)]),

@@ -76,8 +76,8 @@ int exl_own_scratch(ExlDevice* ds, int role, int64_t numel, half** out)
 extern "C" {
 
 const char* exl_last_error(void) { return t_err; }
-int exl_version(void) { return 105; }             // 101: exl_decode_desc.num_kv_heads; 102: batched decode plans and steps; 103: LoRA plans;
-                                                  // 104: exl_prefill_attn; 105: exl_prefill_attn_ragged, exl_rope_cache_ragged
+int exl_version(void) { return 106; }             // 101: exl_decode_desc.num_kv_heads; 102: batched decode plans and steps; 103: LoRA plans;
+                                                  // 104: exl_prefill_attn; 105: exl_prefill_attn_ragged, exl_rope_cache_ragged; 106: exl_sample
 int64_t exl_launch_count(void) { return g_launches.load(); }
 const char* exl_last_q4_path(void) { return g_last_q4_path; }
 
@@ -615,6 +615,14 @@ int exl_q4_matmul_host(const void* x_host, int M, const exl_q4_matrix* w, void* 
     EXL_CUDA_TRY(cudaMemcpyAsync(out_host, d_out, (size_t)M * w->N * sizeof(half), cudaMemcpyDeviceToHost, stream));
     EXL_CUDA_TRY(cudaStreamSynchronize(stream));
     return EXL_OK;
+}
+
+int exl_sample(const float* logits, int bsz, int vocab, int64_t logits_ld, const int64_t* history, int64_t hist_ld,
+               const int* hist_len_host, const exl_sample_params* p, const float* u, int64_t* tokens, float* probs, float* dist,
+               void* stream)
+{
+    return exl_sample_launch(logits, bsz, vocab, logits_ld, history, hist_ld, hist_len_host, p, u, tokens, probs, dist,
+                             (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------

@@ -168,6 +168,11 @@ int exl_prefill_attn_ragged_launch(const half* q, const half* kc, const half* vc
 // EXL_OK, or EXL_ERR_ARG naming the first bad field of r (who: the entry point named in the message)
 int exl_ragged_validate(const exl_ragged* r, int num_cache_seqs, int max_seq, const char* who);
 
+// sample.cu
+int exl_sample_launch(const float* logits, int bsz, int vocab, int64_t logits_ld, const int64_t* history, int64_t hist_ld,
+                      const int* hist_len, const exl_sample_params* p, const float* u, int64_t* tokens, float* probs, float* dist,
+                      cudaStream_t stream);
+
 // half_matmul.cu
 int exl_half_matmul_cublas_launch(ExlDevice* ds, const half* x, const half* w, half* out, int M, int K, int N, bool no_zero, cudaStream_t stream);
 int exl_half_matmul_custom_launch(const half* x, const half* w, half* out, int M, int K, int N, cudaStream_t stream);

@@ -1,0 +1,517 @@
+// sample.cu -- exl_sample: the generator's token sampling (generator.py:91-170 with apply_rep_penalty_cpu and the bos logit of
+// gen_single_token) on the device, one launch for up to EXL_RAGGED_MAX_SEQ rows.
+//
+// Layout     one thread-block cluster of SP_CL CTAs per row.  CTA r owns the contiguous slice [r * slice, (r + 1) * slice) of the
+//            vocabulary (slice = ceil(vocab / SP_CL) <= 32768) and keeps it in shared memory for the whole call, so every pass
+//            after the first reads shared memory, whatever the vocabulary size.  Cluster-wide quantities (the row maximum, sums,
+//            histograms) are merged over distributed shared memory; every CTA reads the same merged values in the same order and
+//            so takes the same decisions.
+// Penalty    the history window is scanned once: integer atomicMin of the position (newest first) per token of the slice, in the
+//            slice buffer itself, gives each token its newest occurrence; v at that position comes from the fp32 recurrence
+//            v += dv computed step by step (bit-exact with exl_apply_rep_penalty).
+// Filters    top-k, top-p and typical each keep a prefix of an order: probability descending (top-k, top-p) or entropy deviation
+//            ascending (typical), ties to the lower token id.  Both orders are 50-bit keys (the float's bits above the inverted
+//            token id, so keys are unique), and each cut is found by a radix descent over the key in five 10-bit digits with
+//            bucket histograms of counts and of probability mass -- no sort.  Mass is summed in 2^-60 fixed point with integer
+//            atomics, so its order does not matter; fp32 sums (softmax, normalisations) use one fixed reduction order.  Two
+//            launches are bitwise equal.
+// Draw       inverse CDF in ascending token-id order over the kept set, in the same fixed point.
+#include "exl_common.cuh"
+#include <cooperative_groups.h>
+#include <cmath>
+
+namespace cg = cooperative_groups;
+
+namespace {
+
+constexpr int SP_CL = 8;                        // CTAs per row
+constexpr int SP_THREADS = 512;
+constexpr int SP_MAX_VOCAB = 262144;            // token ids fit SP_ID_BITS
+constexpr int SP_ID_BITS = 18;
+constexpr int SP_DIGIT = 10;
+constexpr int SP_BINS = 1 << SP_DIGIT;
+constexpr int SP_KEY_BITS = 50;                 // 32-bit float field above the 18-bit id field
+constexpr int SP_PASSES = SP_KEY_BITS / SP_DIGIT;
+constexpr int SP_VTAB = 2048;                   // penalty recurrence values kept in shared memory (longer chains continue in registers)
+constexpr int SP_MAX_SLICE = (SP_MAX_VOCAB + SP_CL - 1) / SP_CL;
+constexpr double SP_FIX = 1152921504606846976.0;   // 2^60: probability mass in fixed point
+static_assert(SP_PASSES * SP_DIGIT == SP_KEY_BITS, "whole digits");
+static_assert(SP_MAX_VOCAB <= (1 << SP_ID_BITS), "ids fit the key's id field");
+static_assert(2 * SP_BINS == 4 * SP_THREADS, "each thread scans two bins");
+
+struct SampleArgs {
+    const float* logits; int64_t ld; int vocab; int slice;
+    const int64_t* hist; int64_t hist_ld; int hist_len[EXL_RAGGED_MAX_SEQ];
+    float temperature; int top_k; float top_p, min_p, typical;
+    float pmax; int sustain, decay, bos;
+    const int* banned; int n_banned;
+    const float* u; int64_t* tokens; float* probs; float* dist;
+};
+
+struct Part { float f; int bad; unsigned c; unsigned long long m; };
+
+struct Shared {
+    unsigned cnt[2][SP_BINS];
+    unsigned long long mass[2][SP_BINS];
+    float vtab[SP_VTAB];
+    Part xch[2];                 // this CTA's contribution to the last two cluster exchanges
+    Part bc;                     // merged result, broadcast to the block
+    float redf[SP_THREADS / 32];
+    unsigned long long redm[SP_THREADS / 32];
+    unsigned redc[SP_THREADS / 32];
+    int redi[SP_THREADS / 32];
+    int found_pos;
+    unsigned long long found_excl_m; unsigned found_excl_c;
+};
+
+__device__ __forceinline__ unsigned long long fix60(float w) { return __float2ull_rz(w * 0x1p60f); }
+
+// order keys: larger key = earlier in the order; the low SP_ID_BITS hold the inverted id, so a tie goes to the lower id
+__device__ __forceinline__ unsigned long long desc_key(float v, int id)
+{
+    return ((unsigned long long)__float_as_uint(v) << SP_ID_BITS) | (unsigned)((SP_MAX_VOCAB - 1) - id);
+}
+__device__ __forceinline__ unsigned long long asc_key(float v, int id)
+{
+    return ((unsigned long long)(0xFFFFFFFFu - __float_as_uint(v)) << SP_ID_BITS) | (unsigned)((SP_MAX_VOCAB - 1) - id);
+}
+
+// one fixed-order block reduction: warp butterflies, then warp 0 over the warp results
+__device__ float block_sum_f(float v, Shared& sh)
+{
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) sh.redf[threadIdx.x >> 5] = v;
+    __syncthreads();
+    float s = 0.f;
+    if (threadIdx.x == 0) for (int w = 0; w < SP_THREADS / 32; w++) s += sh.redf[w];
+    return s;                                                        // valid in thread 0
+}
+__device__ float block_max_f(float v, Shared& sh)
+{
+    for (int o = 16; o; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) sh.redf[threadIdx.x >> 5] = v;
+    __syncthreads();
+    float s = -INFINITY;
+    if (threadIdx.x == 0) for (int w = 0; w < SP_THREADS / 32; w++) s = fmaxf(s, sh.redf[w]);
+    return s;
+}
+__device__ unsigned block_sum_c(unsigned v, Shared& sh)
+{
+    v = __reduce_add_sync(0xffffffffu, v);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) sh.redc[threadIdx.x >> 5] = v;
+    __syncthreads();
+    unsigned s = 0;
+    if (threadIdx.x == 0) for (int w = 0; w < SP_THREADS / 32; w++) s += sh.redc[w];
+    return s;
+}
+__device__ int block_or(int v, Shared& sh)
+{
+    v = __any_sync(0xffffffffu, v);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) sh.redi[threadIdx.x >> 5] = v;
+    __syncthreads();
+    int s = 0;
+    if (threadIdx.x == 0) for (int w = 0; w < SP_THREADS / 32; w++) s |= sh.redi[w];
+    return s;
+}
+
+// Cluster exchange: thread 0's `mine` goes to every CTA; thread 0 combines the SP_CL parts in rank order (combine(parts, out))
+// and the result lands in sh.bc for the whole block.  One cluster barrier per exchange; the parity of `ph` alternates the
+// exchange slots and histogram buffers, so a slot is rewritten only after every CTA has passed the barrier that follows its read.
+template <class Combine>
+__device__ void cluster_exchange(Shared& sh, int& ph, const Part& mine, Combine combine)
+{
+    cg::cluster_group cluster = cg::this_cluster();
+    if (threadIdx.x == 0) sh.xch[ph & 1] = mine;
+    cluster.sync();
+    if (threadIdx.x == 0) {
+        Part parts[SP_CL];
+#pragma unroll
+        for (int r = 0; r < SP_CL; r++) parts[r] = *cluster.map_shared_rank(&sh.xch[ph & 1], r);
+        combine(parts, sh.bc);
+    }
+    __syncthreads();
+    ph++;
+}
+
+__device__ float cluster_sum_f(Shared& sh, int& ph, float v)
+{
+    Part p{}; p.f = block_sum_f(v, sh);
+    cluster_exchange(sh, ph, p, [](const Part* ps, Part& o) { float s = 0.f; for (int r = 0; r < SP_CL; r++) s += ps[r].f; o.f = s; });
+    return sh.bc.f;
+}
+__device__ unsigned cluster_sum_c(Shared& sh, int& ph, unsigned v)
+{
+    Part p{}; p.c = block_sum_c(v, sh);
+    cluster_exchange(sh, ph, p, [](const Part* ps, Part& o) { unsigned s = 0; for (int r = 0; r < SP_CL; r++) s += ps[r].c; o.c = s; });
+    return sh.bc.c;
+}
+
+// The row's filter state: each stage's cut (a key threshold; 0 keeps everything) and normaliser (1 until the stage has run, and for
+// a stage that is off: x / 1.0f is x, bit for bit).
+struct Row {
+    unsigned long long kk = 0, kp = 0, kt = 0;
+    float sk = 1.0f, sp = 1.0f, st = 1.0f, negent = 0.0f;
+};
+
+// One token after the stages up to `level` (1: top-k, 2: top-p, 3: typical): whether it is kept, its key in that level's order
+// and its probability there.
+struct Tok { bool in; unsigned long long key; float w; };
+
+__device__ __forceinline__ Tok eval(const Row& R, float p, int id, int level)
+{
+    Tok t;
+    t.key = desc_key(p, id);
+    t.in = t.key >= R.kk;
+    const float q = p / R.sk;
+    t.w = q;
+    if (level < 2) return t;
+    t.in = t.in && t.key >= R.kp;
+    const float r = q / R.sp;
+    t.w = r;
+    if (level < 3) return t;
+    const float d = fabsf(R.negent - logf(r + 1e-10f));
+    t.key = asc_key(d, id);
+    t.in = t.in && t.key >= R.kt;
+    t.w = r / R.st;
+    return t;
+}
+
+struct Descent { unsigned long long key; unsigned before; bool found; };
+
+// Radix descent over the keys of the tokens `in` at `level`, in decreasing key order.
+//   cross == false: the token of rank k (1-based).
+//   cross == true : the first token whose inclusive mass (fixed point, weights w) exceeds T.
+__device__ Descent radix_descent(Shared& sh, int& ph, const Row& R, const float* s_row, int n, int lo, int level, bool cross,
+                                 unsigned k, unsigned long long T)
+{
+    cg::cluster_group cluster = cg::this_cluster();
+    unsigned long long prefix = 0, acc = 0;
+    unsigned before = 0;
+    for (int pass = 0; pass < SP_PASSES; pass++) {
+        const int shift = SP_KEY_BITS - SP_DIGIT * (pass + 1);
+        const int buf = ph & 1;
+        for (int b = threadIdx.x; b < SP_BINS; b += SP_THREADS) { sh.cnt[buf][b] = 0; sh.mass[buf][b] = 0; }
+        if (threadIdx.x == 0) sh.found_pos = -1;
+        __syncthreads();
+        for (int i = threadIdx.x; i < n; i += SP_THREADS) {
+            const Tok t = eval(R, s_row[i], lo + i, level);
+            if (!t.in || (t.key >> (shift + SP_DIGIT)) != (prefix >> (shift + SP_DIGIT))) continue;
+            const int d = (int)(t.key >> shift) & (SP_BINS - 1);
+            atomicAdd(&sh.cnt[buf][d], 1u);
+            if (cross) atomicAdd(&sh.mass[buf][d], fix60(t.w));
+        }
+        cluster.sync();
+        // positions 2t, 2t + 1 of the descending bin order (bins SP_BINS-1-2t, SP_BINS-2-2t), merged over the cluster
+        unsigned c[2] = {0, 0}; unsigned long long m[2] = {0, 0};
+#pragma unroll
+        for (int e = 0; e < 2; e++) {
+            const int bin = SP_BINS - 1 - (2 * threadIdx.x + e);
+#pragma unroll
+            for (int r = 0; r < SP_CL; r++) {
+                c[e] += cluster.map_shared_rank(&sh.cnt[buf][0], r)[bin];
+                if (cross) m[e] += cluster.map_shared_rank(&sh.mass[buf][0], r)[bin];
+            }
+        }
+        // block inclusive scan of the pairs
+        unsigned cs = c[0] + c[1]; unsigned long long ms = m[0] + m[1];
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+        unsigned ci = cs; unsigned long long mi = ms;
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned cu = __shfl_up_sync(0xffffffffu, ci, o);
+            const unsigned long long mu = __shfl_up_sync(0xffffffffu, mi, o);
+            if (lane >= o) { ci += cu; mi += mu; }
+        }
+        if (lane == 31) { sh.redc[warp] = ci; sh.redm[warp] = mi; }
+        __syncthreads();
+        unsigned cb = ci - cs; unsigned long long mb = mi - ms;
+        for (int w = 0; w < warp; w++) { cb += sh.redc[w]; mb += sh.redm[w]; }
+#pragma unroll
+        for (int e = 0; e < 2; e++) {
+            const unsigned c_incl = cb + c[e]; const unsigned long long m_incl = mb + m[e];
+            const bool hit = cross ? (acc + mb <= T && acc + m_incl > T) : (cb < k && k <= c_incl);
+            if (hit) { sh.found_pos = 2 * threadIdx.x + e; sh.found_excl_c = cb; sh.found_excl_m = mb; }
+            cb = c_incl; mb = m_incl;
+        }
+        __syncthreads();
+        const int pos = sh.found_pos;
+        ph++;
+        if (pos < 0) return Descent{0, 0, false};                    // the same decision in every CTA
+        prefix |= (unsigned long long)(SP_BINS - 1 - pos) << shift;
+        before += sh.found_excl_c;
+        acc += sh.found_excl_m;
+        if (!cross) k -= sh.found_excl_c;
+        __syncthreads();                                             // sh.found_* are rewritten by the next pass
+    }
+    return Descent{prefix, before, true};
+}
+
+__device__ float penalty_value(const Shared& sh, long long j, long long s0, float dv)
+{
+    long long k = j - s0;
+    if (k <= 0) return sh.vtab[0];
+    if (k < SP_VTAB) return sh.vtab[k];
+    float v = sh.vtab[SP_VTAB - 1];
+    for (long long i = SP_VTAB - 1; i < k; i++) v += dv;
+    return v;
+}
+
+__global__ void __cluster_dims__(SP_CL, 1, 1) __launch_bounds__(SP_THREADS, 1) sample_kernel(const __grid_constant__ SampleArgs a)
+{
+    extern __shared__ __align__(16) float s_row[];
+    __shared__ Shared sh;
+    int* s_int = reinterpret_cast<int*>(s_row);
+    cg::cluster_group cluster = cg::this_cluster();
+    const int row = blockIdx.y;
+    const int rank = (int)cluster.block_rank();
+    const int lo = rank * a.slice;
+    const int n = max(0, min(a.slice, a.vocab - lo));
+    int ph = 0;
+    int bad = 0;
+
+    // 1. repetition penalty: newest window position of each token of the slice
+    const bool pen = a.hist != nullptr && a.pmax != 1.0f && a.hist_len[row] > 0;
+    long long s0 = 0, W = 0;
+    const float dv = a.decay ? (1.0f - a.pmax) / (float)a.decay : 0.0f;
+    if (pen) {
+        const long long len = a.hist_len[row];
+        s0 = a.sustain == -1 ? len : a.sustain;
+        const long long beg = max(0LL, len - s0 - a.decay);
+        W = len - beg;
+        for (int i = threadIdx.x; i < n; i += SP_THREADS) s_int[i] = INT_MAX;
+        if (threadIdx.x == 0) {
+            const long long kmax = min((long long)SP_VTAB - 1, max(0LL, W - 1 - s0));
+            float v = a.pmax;
+            sh.vtab[0] = v;
+            for (long long k = 1; k <= kmax; k++) { v += dv; sh.vtab[k] = v; }
+        }
+        __syncthreads();
+        const int64_t* h = a.hist + (int64_t)row * a.hist_ld;
+        for (long long j = threadIdx.x; j < W; j += SP_THREADS) {
+            const int64_t t = h[len - 1 - j];
+            if (t < 0 || t >= a.vocab) { bad = 1; continue; }
+            if (t >= lo && t < lo + n) atomicMin(&s_int[t - lo], (int)j);
+        }
+        __syncthreads();
+    }
+    // 2. penalised logits, bos, banned
+    const float* lg = a.logits + (int64_t)row * a.ld + lo;
+    for (int i = threadIdx.x; i < n; i += SP_THREADS) {
+        float x = lg[i];
+        if (pen) {
+            const int j = s_int[i];
+            if (j != INT_MAX) {
+                const float v = penalty_value(sh, j, s0, dv);
+                x = x > 0.0f ? __fdiv_rn(x, v) : x * v;
+            }
+        }
+        if (lo + i == a.bos) x = -10000.0f;
+        s_row[i] = x;
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < a.n_banned; k += SP_THREADS) {
+        const int t = a.banned[k];
+        if (t < 0 || t >= a.vocab) { bad = 1; continue; }
+        if (t >= lo && t < lo + n) s_row[t - lo] = -INFINITY;
+    }
+    __syncthreads();
+    // 3. temperature, + 1e-8, softmax
+    float mx = -INFINITY;
+    for (int i = threadIdx.x; i < n; i += SP_THREADS) {
+        const float y = __fadd_rn(__fdiv_rn(s_row[i], a.temperature), 1e-8f);
+        s_row[i] = y;
+        if (isnan(y)) bad = 1;
+        mx = fmaxf(mx, y);
+    }
+    {
+        Part p{}; p.f = block_max_f(mx, sh); p.bad = block_or(bad, sh);
+        cluster_exchange(sh, ph, p, [](const Part* ps, Part& o) {
+            float m = -INFINITY; int b = 0;
+            for (int r = 0; r < SP_CL; r++) { m = fmaxf(m, ps[r].f); b |= ps[r].bad; }
+            o.f = m; o.bad = b;
+        });
+        mx = sh.bc.f; bad = sh.bc.bad;
+    }
+    if (bad || mx == -INFINITY) {                                    // undefined row: -1 / NaN
+        if (rank == 0 && threadIdx.x == 0) { a.tokens[row] = -1; a.probs[row] = NAN; }
+        if (a.dist) for (int i = threadIdx.x; i < n; i += SP_THREADS) a.dist[(int64_t)row * a.vocab + lo + i] = NAN;
+        cluster.sync();                                              // no CTA leaves while another may read its exchange slot
+        return;
+    }
+    float z = 0.f;
+    for (int i = threadIdx.x; i < n; i += SP_THREADS) { const float e = expf(s_row[i] - mx); s_row[i] = e; z += e; }
+    z = cluster_sum_f(sh, ph, z);
+    for (int i = threadIdx.x; i < n; i += SP_THREADS) s_row[i] = s_row[i] / z;
+    __syncthreads();
+
+    Row R;
+    unsigned len = (unsigned)a.vocab;                                // length of the ordered list at the current stage
+    // 4. top-k, then L1 normalisation
+    if (a.top_k > 0) {
+        R.kk = radix_descent(sh, ph, R, s_row, n, lo, 1, false, (unsigned)a.top_k, 0).key;
+        len = (unsigned)a.top_k;
+        float s = 0.f;
+        for (int i = threadIdx.x; i < n; i += SP_THREADS) if (desc_key(s_row[i], lo + i) >= R.kk) s += s_row[i];
+        R.sk = fmaxf(cluster_sum_f(sh, ph, s), 1e-12f);
+    }
+    // 5. top-p with its min_p test, then renormalise
+    if (a.top_p > 0.0f) {
+        const unsigned long long T = (unsigned long long)((double)fminf(a.top_p, 2.0f) * SP_FIX);
+        const Descent c = radix_descent(sh, ph, R, s_row, n, lo, 1, true, 0, T);
+        const unsigned n_p = c.found ? c.before : len;
+        unsigned cm = 0;
+        for (int i = threadIdx.x; i < n; i += SP_THREADS) {
+            const Tok t = eval(R, s_row[i], lo + i, 1);
+            cm += (t.in && t.w >= a.min_p) ? 1u : 0u;
+        }
+        cm = cluster_sum_c(sh, ph, cm);
+        const unsigned keep = max(1u, min(min(n_p, cm), len));
+        if (c.found && keep == n_p) R.kp = c.key + 1;                // everything before the first token past top_p
+        else if (keep == len) R.kp = 0;
+        else R.kp = radix_descent(sh, ph, R, s_row, n, lo, 1, false, keep, 0).key;
+        len = keep;
+        float s = 0.f;
+        for (int i = threadIdx.x; i < n; i += SP_THREADS) {
+            const Tok t = eval(R, s_row[i], lo + i, 2);
+            if (t.in) s += t.w;
+        }
+        R.sp = fmaxf(cluster_sum_f(sh, ph, s), 1e-12f);
+    }
+    // 6. typical: order by |sum p log(p + eps) - log(p + eps)| ascending, the same prefix rule without min_p, renormalise
+    if (a.typical > 0.0f) {
+        float s = 0.f;
+        for (int i = threadIdx.x; i < n; i += SP_THREADS) {
+            const Tok t = eval(R, s_row[i], lo + i, 2);
+            if (t.in) s += t.w * logf(t.w + 1e-10f);
+        }
+        R.negent = cluster_sum_f(sh, ph, s);
+        const unsigned long long T = (unsigned long long)((double)fminf(a.typical, 2.0f) * SP_FIX);
+        const Descent c = radix_descent(sh, ph, R, s_row, n, lo, 3, true, 0, T);
+        const unsigned n_t = c.found ? c.before : len;
+        const unsigned keep = max(1u, min(n_t, len));
+        if (c.found && keep == n_t) R.kt = c.key + 1;
+        else if (keep == len) R.kt = 0;
+        else R.kt = radix_descent(sh, ph, R, s_row, n, lo, 3, false, keep, 0).key;
+        float s2 = 0.f;
+        for (int i = threadIdx.x; i < n; i += SP_THREADS) {
+            const Tok t = eval(R, s_row[i], lo + i, 3);
+            if (t.in) s2 += t.w;
+        }
+        R.st = fmaxf(cluster_sum_f(sh, ph, s2), 1e-12f);
+    }
+    const int level = a.typical > 0.0f ? 3 : (a.top_p > 0.0f ? 2 : 1);
+
+    // 7. final distribution and the draw: thread t owns the contiguous run [t * per, (t + 1) * per) of the slice
+    const int per = (n + SP_THREADS - 1) / SP_THREADS;
+    const int i0 = min(n, (int)threadIdx.x * per), i1 = min(n, i0 + per);
+    unsigned long long mine = 0;
+    int last_kept = -1;
+    for (int i = i0; i < i1; i++) {
+        const Tok t = eval(R, s_row[i], lo + i, level);
+        const float f = t.in ? t.w : 0.0f;
+        if (a.dist) a.dist[(int64_t)row * a.vocab + lo + i] = f;
+        if (t.in) { mine += fix60(f); last_kept = lo + i; }
+    }
+    // exclusive scan of the runs' masses inside the CTA
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned long long incl = mine;
+    for (int o = 1; o < 32; o <<= 1) { const unsigned long long v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
+    int lk = last_kept;
+    for (int o = 16; o; o >>= 1) lk = max(lk, __shfl_xor_sync(0xffffffffu, lk, o));
+    __syncthreads();
+    if (lane == 31) sh.redm[warp] = incl;
+    if (lane == 0) sh.redi[warp] = lk;
+    __syncthreads();
+    unsigned long long base = incl - mine, cta_total = 0;
+    int cta_last = -1;
+    for (int w = 0; w < SP_THREADS / 32; w++) {
+        if (w < warp) base += sh.redm[w];
+        cta_total += sh.redm[w];
+        cta_last = max(cta_last, sh.redi[w]);
+    }
+    Part p{}; p.m = cta_total; p.bad = cta_last;
+    if (threadIdx.x == 0) sh.xch[ph & 1] = p;
+    cluster.sync();
+    unsigned long long before_cta = 0, total = 0;
+    int row_last = -1;
+    for (int r = 0; r < SP_CL; r++) {
+        const Part q = *cluster.map_shared_rank(&sh.xch[ph & 1], r);
+        if (r < rank) before_cta += q.m;
+        total += q.m;
+        row_last = max(row_last, q.bad);
+    }
+    const unsigned long long U = (unsigned long long)((double)a.u[row] * SP_FIX);
+    if (U >= total) {                                                // rounding left u at or above the total: the largest kept id
+        if (lo <= row_last && row_last < lo + n && row_last == last_kept) {
+            a.tokens[row] = row_last;
+            a.probs[row] = eval(R, s_row[row_last - lo], row_last, level).w;
+        }
+    } else {
+        unsigned long long cum = before_cta + base;
+        if (cum <= U && U < cum + mine) {
+            for (int i = i0; i < i1; i++) {
+                const Tok t = eval(R, s_row[i], lo + i, level);
+                if (!t.in) continue;
+                cum += fix60(t.w);
+                if (cum > U) { a.tokens[row] = lo + i; a.probs[row] = t.w; break; }
+            }
+        }
+    }
+    cluster.sync();                                                  // keep this CTA's exchange slot alive until every CTA has read it
+}
+
+bool g_sample_attr[EXL_MAX_DEVICES];
+
+} // namespace
+
+int exl_sample_launch(const float* logits, int bsz, int vocab, int64_t logits_ld, const int64_t* history, int64_t hist_ld,
+                      const int* hist_len, const exl_sample_params* p, const float* u, int64_t* tokens, float* probs, float* dist,
+                      cudaStream_t stream)
+{
+    if (!p) return exl_set_err(EXL_ERR_ARG, "sample: params is NULL");
+    if (!logits || !u || !tokens || !probs)
+        return exl_set_err(EXL_ERR_ARG, "sample: NULL pointer (logits %p, u %p, tokens %p, probs %p)", (const void*)logits,
+                           (const void*)u, (void*)tokens, (void*)probs);
+    if (bsz < 1 || bsz > EXL_RAGGED_MAX_SEQ) return exl_set_err(EXL_ERR_ARG, "sample: bsz %d outside [1, %d]", bsz, EXL_RAGGED_MAX_SEQ);
+    if (vocab < 1 || vocab > SP_MAX_VOCAB) return exl_set_err(EXL_ERR_ARG, "sample: vocab %d outside [1, %d]", vocab, SP_MAX_VOCAB);
+    if (logits_ld < vocab) return exl_set_err(EXL_ERR_ARG, "sample: logits_ld %lld < vocab %d", (long long)logits_ld, vocab);
+    if (!std::isfinite(p->temperature) || !(p->temperature > 0.0f))
+        return exl_set_err(EXL_ERR_ARG, "sample: temperature %g is not finite and positive", (double)p->temperature);
+    if (p->top_k < 0 || p->top_k > vocab) return exl_set_err(EXL_ERR_ARG, "sample: top_k %d outside [0, vocab %d]", p->top_k, vocab);
+    if (!(p->top_p >= 0.0f)) return exl_set_err(EXL_ERR_ARG, "sample: top_p %g is negative", (double)p->top_p);
+    if (!(p->min_p >= 0.0f)) return exl_set_err(EXL_ERR_ARG, "sample: min_p %g is negative", (double)p->min_p);
+    if (!(p->typical >= 0.0f)) return exl_set_err(EXL_ERR_ARG, "sample: typical %g is negative", (double)p->typical);
+    if (p->rep_sustain < -1) return exl_set_err(EXL_ERR_ARG, "sample: rep_sustain %d < -1", p->rep_sustain);
+    if (p->rep_decay < 0) return exl_set_err(EXL_ERR_ARG, "sample: rep_decay %d < 0", p->rep_decay);
+    if (p->n_banned < 0 || (p->n_banned > 0 && !p->banned))
+        return exl_set_err(EXL_ERR_ARG, "sample: n_banned %d with banned %p", p->n_banned, (const void*)p->banned);
+    SampleArgs a{};
+    if (history) {
+        if (!hist_len) return exl_set_err(EXL_ERR_ARG, "sample: history without hist_len_host");
+        for (int b = 0; b < bsz; b++)
+            if (hist_len[b] < 0 || hist_len[b] > hist_ld)
+                return exl_set_err(EXL_ERR_ARG, "sample: hist_len[%d] %d outside [0, hist_ld %lld]", b, hist_len[b], (long long)hist_ld);
+        for (int b = 0; b < bsz; b++) a.hist_len[b] = hist_len[b];
+    }
+    a.logits = logits; a.ld = logits_ld; a.vocab = vocab; a.slice = (vocab + SP_CL - 1) / SP_CL;
+    a.hist = history; a.hist_ld = hist_ld;
+    a.temperature = p->temperature; a.top_k = p->top_k; a.top_p = p->top_p; a.min_p = p->min_p; a.typical = p->typical;
+    a.pmax = p->rep_penalty_max; a.sustain = p->rep_sustain; a.decay = p->rep_decay; a.bos = p->bos_token_id;
+    a.banned = p->banned; a.n_banned = p->n_banned;
+    a.u = u; a.tokens = tokens; a.probs = probs; a.dist = dist;
+
+    int dev = 0;
+    EXL_CUDA_TRY(cudaGetDevice(&dev));
+    if (dev < 0 || dev >= EXL_MAX_DEVICES) return exl_set_err(EXL_ERR_ARG, "sample: device %d", dev);
+    if (!g_sample_attr[dev]) {
+        EXL_CUDA_TRY(cudaFuncSetAttribute(sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SP_MAX_SLICE * (int)sizeof(float)));
+        g_sample_attr[dev] = true;
+    }
+    const size_t smem = (size_t)a.slice * sizeof(float);
+    sample_kernel<<<dim3(SP_CL, bsz), SP_THREADS, smem, stream>>>(a);
+    EXL_CHECK_LAUNCH("sample_kernel");
+    return EXL_OK;
+}

@@ -335,6 +335,49 @@ int exl_rep_penalty(int vocab_size, const uint64_t* sequence_host, float* rep_ma
 int exl_apply_rep_penalty(int vocab_size, const uint64_t* sequence_host, float penalty_max,
                           int sustain, int decay, int seq_len, float* logits_host);
 
+/* --- sampling on the device (exllama_b200/csrc/sample.cu; the reference samples on the host, generator.py:91-170) ---------- */
+
+/* Settings of one exl_sample call, shared by every row (ExLlamaGenerator.Settings, generator.py:9-19). */
+typedef struct {
+    float temperature;        /* finite and > 0 (generator.py:106); greedy is top_k = 1 */
+    int   top_k;              /* 0: off (the full order, generator.py:112-113); 1 .. vocab */
+    float top_p;              /* 0: off; the loop of generator.py:120-133, including its min_p test */
+    float min_p;              /* used only inside the top-p loop, as the reference does */
+    float typical;            /* 0: off; generator.py:137-158, epsilon 1e-10 */
+    float rep_penalty_max;    /* apply_rep_penalty_cpu semantics (cpu_func/rep_penalty.cpp:36-74); 1.0 or history == NULL: no penalty */
+    int   rep_sustain;        /* -1: the whole history */
+    int   rep_decay;
+    int   bos_token_id;       /* >= 0: its logit becomes -10000 after the penalty (generator.py:355); -1: untouched */
+    const int* banned;        /* device, n_banned ids set to -inf before the temperature (disallow_tokens, generator.py:101-102) */
+    int   n_banned;
+} exl_sample_params;
+
+/* One token per row from fp32 logits [bsz][logits_ld] (read only; the reference edits its logits in place, this does not).
+   Per row, in the generator's order:
+     1. the repetition penalty over history[b][0 .. hist_len_host[b]) (int64 token ids, newest last), bit-exact with
+        exl_apply_rep_penalty on that row: the newest occurrence of a token decides its factor, the factor steps by dv in fp32
+        one position at a time;
+     2. the bos logit -> -10000, then the banned logits -> -inf;
+     3. / temperature (IEEE division), + 1e-8, softmax;
+     4. top-k, then L1 normalisation (eps 1e-12);
+     5. the top-p loop: the first token of the order is always kept, a later one while the cumulative sum that includes it is
+        <= top_p and its probability >= min_p; renormalise;
+     6. typical: order by |sum p log(p + 1e-10) - log(p + 1e-10)| ascending, keep the same cumulative prefix (no min_p), renormalise;
+     7. the draw: the smallest kept id whose inclusive cumulative probability, in ascending token-id order, exceeds u[b]; if
+        rounding leaves u[b] at or above the total, the largest kept id.
+   The orders of 4-6 are probability descending and entropy deviation ascending; a tie goes to the lower token id.
+   Outputs: tokens[b] (int64), probs[b] = the final probability of that token (what sample() returns), and, when dist != NULL,
+   dist[b][vocab] = the final distribution (0 outside the kept set).  A row whose distribution is undefined (every logit -inf after
+   masking, a NaN logit, a history or banned id outside [0, vocab)) gets token -1, probability NaN and a NaN dist row; the other
+   rows are unaffected.  hist_len_host is read on the host (baked into a CUDA-graph capture).  No allocation, no floating-point
+   atomics: two launches are bitwise equal.
+   EXL_ERR_ARG (naming the value) for bsz outside 1 .. EXL_RAGGED_MAX_SEQ, vocab outside 1 .. 262144, logits_ld < vocab, a
+   temperature that is not finite and positive, top_k outside 0 .. vocab, a negative top_p / min_p / typical, rep_sustain < -1,
+   rep_decay < 0, hist_len_host[b] outside 0 .. hist_ld, or a NULL pointer (params, logits, u, tokens, probs). */
+int exl_sample(const float* logits, int bsz, int vocab, int64_t logits_ld,
+               const int64_t* history, int64_t hist_ld, const int* hist_len_host,
+               const exl_sample_params* p, const float* u, int64_t* tokens, float* probs, float* dist, void* stream);
+
 /* --- host-buffer entry point (end-to-end measurement and non-torch callers) ----- */
 
 /* q4_matmul with HOST x / out: copies x H2D, runs exl_q4_matmul, copies out D2H, synchronises `stream`.

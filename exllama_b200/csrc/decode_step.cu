@@ -16,7 +16,7 @@
 //    8 KB of packed qweight + one 2-D op each for the unit's scale and zero rows), KV-cache rows older than the current token
 //    (bulk copies) and lm_head rows do not depend on activations, so up to 4 x depth x 8 KB per SM (~19 MB chip-wide) of the
 //    NEXT phase is loaded while the consumers are in a barrier or in a phase prologue, one stage per pipeline in flight at a
-//    time.  HBM stays busy across phase and layer boundaries -- the thing separate launches could not do.
+//    time (up to MID_INFLIGHT later in a phase, away from the barriers).  HBM stays busy across phase and layer boundaries -- the thing separate launches could not do.
 //  * Work of a GEMV phase = (128-column tile) x (128-row K stage) units, flattened tile-major and cut into G equal contiguous
 //    ranges (G = grid size): every SM streams the same number of bytes whatever the matrix shapes (65B gate/up: 172 tiles on
 //    132 SMs is no longer a problem).  A warp accumulates its 32 columns over the stages it sees and, at a tile boundary,
@@ -66,6 +66,7 @@ constexpr int MAX_LAYERS = 128;
 constexpr int TRACE_LAYERS = 4;
 enum { ZR_QKV = 0, ZR_H = 1, ZR_GU = 2, ZR_LOGITS = 3, ZR_HALF = 4, ZR_COUNT = 5 };     // zero_share / push ranges
 constexpr unsigned long long WAIT_NS = 4000000000ull;   // any single wait longer than this aborts the launch
+constexpr int MID_INFLIGHT = 3;                  // ring stages in flight per pipeline past the first `depth` stages of a phase
 
 struct alignas(64) LayerDesc
 {
@@ -149,20 +150,21 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
     for (unsigned i = 1; !mbar_try(bar, parity); i++)
         if ((i & 1023u) == 0 && gtime() - t0 > WAIT_NS) __trap();
 }
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar)
+// HBM -> shared memory through the TMA unit, completing on mbarrier `bar`; pol: L2 cache policy (createpolicy)
+__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint64_t pol)
 {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 :: "r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                 :: "r"(dst), "l"(src), "r"(bytes), "r"(bar), "l"(pol) : "memory");
 }
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tmap, int c0, int c1, uint32_t bar)
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tmap, int c0, int c1, uint32_t bar, uint64_t pol)
 {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-                 :: "r"(dst), "l"(tmap), "r"(c0), "r"(c1), "r"(bar) : "memory");
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%2, %3}], [%4], %5;"
+                 :: "r"(dst), "l"(tmap), "r"(c0), "r"(c1), "r"(bar), "l"(pol) : "memory");
 }
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* tmap, int c0, int c1, int c2, uint32_t bar)
+__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* tmap, int c0, int c1, int c2, uint32_t bar, uint64_t pol)
 {
-    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
-                 :: "r"(dst), "l"(tmap), "r"(c0), "r"(c1), "r"(c2), "r"(bar) : "memory");
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%2, %3, %4}], [%5], %6;"
+                 :: "r"(dst), "l"(tmap), "r"(c0), "r"(c1), "r"(c2), "r"(bar), "l"(pol) : "memory");
 }
 // wait that hands back a zero "token": adding it to the addresses of the loads that follow makes them data-dependent on the wait, so
 // the (non-volatile, freely schedulable) shared-memory loads below can never be hoisted above it
@@ -366,19 +368,26 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         const uint32_t ring_a = smem_u32(ring) + (uint32_t)pq * depth * STAGE_STRIDE;
         const uint32_t full0 = smem_u32(&full_bar[pq * depth]), empty0 = smem_u32(&empty_bar[pq * depth]);
         int jbase = 0;
-        // One stage in flight per pipeline: a stage is issued only once the pipeline's previous stage has landed.  The ring still
-        // fills ahead of the consumers, but stage by stage.  With the whole ring in flight (16 x 8 KB per SM), the release fence of
-        // every CTA's grid-barrier arrival took ~4.7 us on an H100, over 80 % of the barrier; with one stage per pipeline it takes
-        // ~1.7 us, and 4 x 8 KB per SM (4.2 MB chip-wide) still keep HBM busy.  Two or three per pipeline did not help
-        // (DESIGN 3c, profiles/step_trace_h100.json).
+        // Stages in flight per pipeline: the cost of a grid-barrier arrival's release fence grows with the bytes the SM has in
+        // flight (whole ring in flight: ~4.7 us on an H100; one stage per pipeline: ~1.7 us).  The fences fall while the
+        // consumers finish a phase, and the producer is then issuing the first stages of the next phase; so the first `depth`
+        // stages of every phase go one at a time (a stage is issued once the pipeline's previous stage has landed), and the
+        // rest of the phase, streamed while no barrier is near, keeps up to MID_INFLIGHT stages in flight (DESIGN 3c).
+        int nph = 0;                                                          // stages of this pipeline issued in the current phase
+        const int kmid = MID_INFLIGHT < depth ? MID_INFLIGHT : depth;
         auto acquire = [&](uint32_t tx) -> uint32_t {
             if (issued >= depth) mbar_wait(empty0 + ls * 8, par ^ 1u);
-            if (issued > 0) mbar_wait(full0 + (ls == 0 ? depth - 1 : ls - 1) * 8, ls == 0 ? par ^ 1u : par);
+            const int k = nph < depth ? 1 : kmid;
+            if (issued >= k) { int pj = ls - k; uint32_t pp = par; if (pj < 0) { pj += depth; pp ^= 1u; } mbar_wait(full0 + pj * 8, pp); }
             if (lane == 0) mbar_expect_tx(full0 + ls * 8, tx);
             __syncwarp();
             return ring_a + (uint32_t)ls * STAGE_STRIDE;
         };
-        auto advance = [&]() { if (issued < depth) issued++; if (++ls == depth) { ls = 0; par ^= 1u; } };
+        auto advance = [&]() { nph++; if (issued < depth) issued++; if (++ls == depth) { ls = 0; par ^= 1u; } };
+        // Every byte the ring loads is read once per token: evict-first keeps it from pushing the phase accumulators, attention
+        // partials and barrier counter out of L2, which the prologues and barriers read back
+        uint64_t pol;
+        asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
         const int ngrow = a.gshift >= 2 ? 1 : (4 >> a.gshift);          // group rows per K stage (groupsize 32: 4, 64: 2, >= 128: 1)
         #pragma unroll 1
         for (int l = 0; l < a.n_layers; l++) {
@@ -389,6 +398,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
                 const int u0 = s_rng[ph][0], u1 = s_rng[ph][1];
                 const int i0 = ((pq - jbase) & 3);
                 jbase += u1 - u0;
+                nph = 0;
                 if (ph == PH_ATT) {
                     int h = (u0 + i0) / p.tpm, ch = (u0 + i0) - h * p.tpm;
                     #pragma unroll 1
@@ -400,8 +410,8 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
                         const uint32_t base = acquire((uint32_t)nv * 512u);
                         if (nv > 0) {
                             const size_t off = ((size_t)h * a.max_seq + pos0) * TILE;
-                            if (lane == 0) bulk_g2s(base, L->kc + off, (uint32_t)nv * 256u, full0 + ls * 8);
-                            if (lane == 1) bulk_g2s(base + 4096, L->vc + off, (uint32_t)nv * 256u, full0 + ls * 8);
+                            if (lane == 0) bulk_g2s(base, L->kc + off, (uint32_t)nv * 256u, full0 + ls * 8, pol);
+                            if (lane == 1) bulk_g2s(base + 4096, L->vc + off, (uint32_t)nv * 256u, full0 + ls * 8, pol);
                         }
                         advance();
                         ch += 4;
@@ -418,9 +428,9 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
                     const uint32_t base = acquire((uint32_t)W_BYTES + (uint32_t)ngrow * 320u);
                     const uint32_t fb = full0 + ls * 8;
                     const int grow = a.gshift >= 2 ? ((s * 4) >> a.gshift) : s * ngrow;
-                    if (lane == 0) tma_load_3d(base, &L->tw[m], 0, s * 16, ct * 4, fb);
-                    else if (lane == 1) tma_load_2d(base + META_SC, &L->ts[m], ct * TILE, grow, fb);
-                    else if (lane == 2) tma_load_2d(base + META_ZQ, &L->tz[m], ct * 16, grow, fb);
+                    if (lane == 0) tma_load_3d(base, &L->tw[m], 0, s * 16, ct * 4, fb, pol);
+                    else if (lane == 1) tma_load_2d(base + META_SC, &L->ts[m], ct * TILE, grow, fb, pol);
+                    else if (lane == 2) tma_load_2d(base + META_ZQ, &L->tz[m], ct * 16, grow, fb, pol);
                     advance();
                     s += 4;
                     while (s >= p.spt) { s -= p.spt; if (++ct == mat_tiles(p, mi)) { ct = 0; mi++; } }
@@ -430,6 +440,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         {
             const int u0 = s_rng[PH_HEAD][0], u1 = s_rng[PH_HEAD][1];
             const int i0 = ((pq - jbase) & 3);
+            nph = 0;
             const long long total = (long long)a.vocab * a.H * 2;
             const unsigned char* src = reinterpret_cast<const unsigned char*>(a.lm_head);
             #pragma unroll 1
@@ -437,7 +448,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
                 const long long off = (long long)u * W_BYTES;
                 const uint32_t bytes = (uint32_t)((total - off) < W_BYTES ? (total - off) : W_BYTES);
                 const uint32_t base = acquire(bytes);
-                if (lane == 0) bulk_g2s(base, src + off, bytes, full0 + ls * 8);
+                if (lane == 0) bulk_g2s(base, src + off, bytes, full0 + ls * 8, pol);
                 advance();
             }
         }

@@ -515,7 +515,7 @@ def _rope_err(v, e, sin_row, cos_row):
     return 1.01 * (lin + 2.0 ** -10 * (sn * (v64[:, partner] + e[:, partner]) + v64 + lin)) + 2 * FP16_TINY
 
 
-def probe_expectation(oracle, st, snap, x, past, plants, kind, seq=0):
+def probe_expectation(oracle, st, snap, x, past, plants, kind, seq=0, o_prop=False):
     """(want, bound): the oracle's final hidden state of a probe stack (oracle_decode_step on the cache snapshot) and a float64
     bound B >= |kernel - want| per element.
 
@@ -536,6 +536,8 @@ def probe_expectation(oracle, st, snap, x, past, plants, kind, seq=0):
                additions and the exponential approximations.
       o_proj   Two fp16 roundings of the attention output, then the identity o GEMV's x quantisation: quant_error_bound(kind)
                of the identity at an upper bound of |attention| (segments: group and 128-k stage, so a head under plain order).
+               o_prop: o_proj is any matrix (no adapter): the attention bound goes through |W_o| instead of unchanged, and the
+               quantisation term is the same bound for that matrix.
       x_out    bx + the attention bound + the o bound + two fp16 roundings of the residual sum; the MLP adds an exact 0.
     The fp16 roundings are taken relative (2^-11 |value|) with FP16_TINY for the subnormal range."""
     s = st.shape
@@ -611,6 +613,10 @@ def probe_expectation(oracle, st, snap, x, past, plants, kind, seq=0):
         xm = None if lin.g_idx is None else oracle.make_x_map(lin.g_idx.numpy(), lin.qzeros.shape[0])
         amax = ((np.abs(attn).reshape(-1) + battn) * (1 + 2.0 ** -9)).astype(np.float16)
         Bo, _ = quant_error_bound(oracle, amax[None], _np(lin.qweight), _np(lin.qzeros), _np(lin.scales), xm, kind)
+        if o_prop:
+            assert adapter_of(st, l, "o") is None, "o_prop carries no adapter on o"
+            battn = (battn if xm is None else battn[np.asarray(xm, np.int64)]) @ np.abs(
+                oracle.dequant_f64(_np(lin.qweight), _np(lin.qzeros), _np(lin.scales)))
         bx = bx + battn + Bo[0] + 2.0 ** -10 * np.abs(xs[l + 1].astype(np.float64).reshape(-1)) + 2 * FP16_TINY
     return want.reshape(-1), bx
 
@@ -677,3 +683,218 @@ class RefLib:
 
     def sync(self):
         self.lib.ref_sync()
+
+
+# ---------------------------------------------------------------------------------------------------------------------------------
+# Phase probes: stacks whose new k / v rows, x_out - x_in or logits are ONE phase's output, bounded element by element on the
+# kernel's own upstream output
+#
+# A stack from stack_harness.make_stack is edited in place before make_plan (the q4 handles borrow the tensors): o_proj's scales
+# zeroed makes its GEMV add exactly 0 (cs * sx * val = 0); ln2 zeroed stages an all-zero x, whose absmax 0 quantises it to 0, so
+# silu(0) * 0 = 0 and down adds exactly 0.  Norm weights log-uniform over [0.05, 4] with exact zeros, different for every tensor,
+# make a wrong tensor or a stale row a gross error.  With a residual of 1e-2 rms the block outputs dominate x_out.
+# ---------------------------------------------------------------------------------------------------------------------------------
+
+def distinct_norm(n, seed):
+    """Norm weights [n] fp16: log-uniform over [0.05, 4], n / 128 of them exactly 0 (at least two), a different draw per seed."""
+    rng = np.random.default_rng(seed)
+    w = np.exp(rng.uniform(np.log(0.05), np.log(4.0), n))
+    w[rng.choice(n, max(2, n // 128), replace=False)] = 0
+    return w.astype(np.float16)
+
+
+def phase_probe_edit(st, o_off=(), mlp_off=(), seed=0):
+    """Edit a DecodeStack in place (before make_plan): distinct_norm weights for ln1 / ln2 of every layer and the final norm,
+    o_proj's scales zeroed in the layers o_off, ln2 zeroed in the layers mlp_off."""
+    import torch
+    h = st.shape.hidden
+    for i, L in enumerate(st.layers):
+        L.ln1.copy_(torch.from_numpy(distinct_norm(h, seed * 101 + 3 * i)))
+        L.ln2.copy_(torch.from_numpy(distinct_norm(h, seed * 101 + 3 * i + 1)))
+        if i in o_off:
+            L.o.scales.zero_()
+        if i in mlp_off:
+            L.ln2.zero_()
+    st.norm.copy_(torch.from_numpy(distinct_norm(h, seed * 101 + 99)))
+    torch.cuda.synchronize()
+
+
+def hmul(a, b):
+    """fp16 x fp16 rounded to fp16 (the product is exact in float64, so this is __hmul's single rounding)."""
+    return (np.asarray(a, np.float16).astype(np.float64) * np.asarray(b, np.float16).astype(np.float64)).astype(np.float16)
+
+
+def norm_candidates(x, w, eps):
+    """rms_norm(x, w) of x [rows, dim] fp16, as (x * rm) * w in fp16 (rms_norm.cu:118-131), for rm = the fp16 row factor
+    rounded from float64 and its two fp16 neighbours: the kernel sums x^2 in fp32 in its own order and takes rsqrtf, so where the
+    exact factor lies near an fp16 rounding boundary its fp16 factor may be the neighbour.  Given the factor both compute the same
+    two roundings, so one of the three is the kernel's normalised x bit for bit.  Returns [rm, rm + 1 ulp, rm - 1 ulp] rows."""
+    x = np.asarray(x, np.float16).reshape(-1, np.shape(x)[-1])
+    x64 = x.astype(np.float64)
+    rm = (1.0 / np.sqrt(np.mean(x64 * x64, axis=1) + eps)).astype(np.float16)[:, None]
+    w = np.asarray(w, np.float16).reshape(1, -1)
+    return [hmul(hmul(x, r), w) for r in (rm, np.nextafter(rm, np.float16(np.inf)), np.nextafter(rm, np.float16(-np.inf)))]
+
+
+def step_gemv(oracle, x, lin, ab=None, dx=None):
+    """(ref, err) of one GEMV of the fused step (q4 `lin`, adapter ab = (A, B) or None) on its phase input x [M, K] in the
+    checkpoint's order, before the fp32 accumulator is rounded anywhere: ref = x . W + fp16(x . A) . B in float64 (t = x . A
+    rounded to nearest) and err >= |accumulator - ref|.  x may be float64 (an exact value the kernel only approximates); dx >= |x'
+    - x| bounds the kernel's own input x' (None: x' = x bit for bit).  With |x'| <= X = |x| + dx:
+
+        err = (1 + 2^-10) ( sum_k A(k) / (2Q) |w_kn| + n_fp32 2^-24 sum_k X_k |w_kn| + sum_k dx_k |w_kn| )
+            + sum_j |B_jn| e_j + (rank + 4) 2^-24 sum_j (|t16_j| + e_j) |B_jn|
+
+    The first line is quant_error_bound without its final fp16 rounding (A(k) the absmax of X over k's window, 4 more fp32
+    roundings for the adapter's atomics into the accumulator) plus the input's own error through |W|.  The adapter: the kernel's
+    fp32 t' = x' . A is within dt = (K + 8) 2^-24 (X . |A|) + dx . |A| of t, and its fp16(t') within e = dt + 2^-10 (|t| + dt) +
+    2^-24 of fp16(t) (each rounded to nearest, so less than one ulp apart whichever way t' falls); the B sum is a chain of rank
+    fp32 fmas and an atomic add."""
+    x64 = np.asarray(x, np.float64)
+    x64 = x64.reshape(-1, x64.shape[-1])
+    M, K = x64.shape
+    dx = np.zeros_like(x64) if dx is None else np.broadcast_to(np.asarray(dx, np.float64), x64.shape)
+    qw, qz, sc = _np(lin.qweight), _np(lin.qzeros), _np(lin.scales)
+    xm = None if lin.g_idx is None else np.asarray(oracle.make_x_map(lin.g_idx.numpy(), qz.shape[0]), np.int64)
+    g = slice(None) if xm is None else xm
+    W = oracle.dequant_f64(qw, qz, sc)
+    aw = np.abs(W)
+    ref = x64[:, g] @ W
+    X = np.abs(x64) + dx
+    Xg = X[:, g]
+    win = quant_windows(K, qz.shape[0])
+    starts = np.flatnonzero(np.r_[True, win[1:] != win[:-1]])
+    A = np.maximum.reduceat(Xg, starts, axis=1)[:, win]
+    n_fp32 = 5 * (win[-1] + 1 + -(-K // STAGE_K)) + QUANT_C + 4
+    err = (1 + 2.0 ** -10) * ((A / (2.0 * QUANT_Q["step"])) @ aw + n_fp32 * 2.0 ** -24 * (Xg @ aw) + dx[:, g] @ aw)
+    del W, aw
+    if ab is not None:
+        Am, Bm = (_np(t).astype(np.float64) for t in ab)
+        t = x64 @ Am
+        t16 = t.astype(np.float16).astype(np.float64)
+        ref = ref + t16 @ Bm
+        dt = (K + 8) * 2.0 ** -24 * (X @ np.abs(Am)) + dx @ np.abs(Am)
+        e = dt + 2.0 ** -10 * (np.abs(t) + dt) + FP16_TINY
+        err = err + e @ np.abs(Bm) + (Am.shape[1] + 4) * 2.0 ** -24 * ((np.abs(t16) + e) @ np.abs(Bm))
+    return ref, err
+
+
+def rounded_bound(ref, err, base=None):
+    """Bound on |fp16(base + acc) - (base + ref)| for an fp32 accumulator acc within err of ref (base: the fp16 residual the
+    accumulator is added to, or None): the error itself and one fp16 rounding of a value no larger than |base + ref| + err."""
+    v = np.abs(ref if base is None else np.asarray(base, np.float64) + ref)
+    return (1 + 2.0 ** -11) * err + 2.0 ** -11 * v + FP16_TINY
+
+
+def qkv_expectation(oracle, st, l, x, past):
+    """Layer l's new k and v rows on its fp16 layer input x [hidden] at position `past`: per norm candidate (norm_candidates of
+    ln1), ((k want [kv_heads, hd], k bound), (v want, v bound)).  v = fp16(accumulator): step_gemv's error and its rounding
+    (rounded_bound).  k: the kernel rounds its accumulator and ropes it in fp16 (hfma(l, cos, hmul(r, -sin))); want is the oracle's
+    rope of fp16(ref), and the pre-rope rows differ by at most the v-style bound plus the oracle's own rounding of ref, which
+    _rope_err carries through rope."""
+    s = st.shape
+    hd, kvh = s.head_dim, s.kv_heads
+    L = st.layers[l]
+    sin = st.sin.view(-1, hd).cpu().numpy(); cos = st.cos.view(-1, hd).cpu().numpy()
+    out = []
+    for xn in norm_candidates(x, _np(L.ln1), s.eps):
+        kr, ke = step_gemv(oracle, xn, L.k, adapter_of(st, l, "k"))
+        vr, ve = step_gemv(oracle, xn, L.v, adapter_of(st, l, "v"))
+        k16 = kr.astype(np.float16)
+        kw = oracle.rope(k16.reshape(1, kvh, hd), sin, cos, 1, kvh, hd, kvh, past).reshape(kvh, hd)
+        ek = (rounded_bound(kr, ke) + 2.0 ** -11 * np.abs(kr) + FP16_TINY).reshape(kvh, hd)
+        kb = _rope_err(kw, ek, sin[past], cos[past])
+        out.append(((kw.astype(np.float64), kb), (vr.reshape(kvh, hd), rounded_bound(vr, ve).reshape(kvh, hd))))
+    return out
+
+
+# silu_h (decode_step.cu) = hmul(x, hrcp(hadd(1, hexp(-x)))); hexp and hrcp are an fp32 approximation rounded to fp16 (cuda_fp16.hpp),
+# so each lands within one fp16 ulp (2^-10 relative) of the exact value, and hadd / hmul round to nearest (2^-11): silu_h(x) is
+# within 2^-10 + 2^-11 + 2^-10 + 2^-11 (+ second order) = SILU_REL of silu(x), for every fp16 x above -11.  Below -11, exp(-x)
+# overflows fp16 and silu_h gives 0 where |silu(x)| <= 11 e^-11 < SILU_FLOOR.
+SILU_REL = 3.1 * 2.0 ** -10
+SILU_FLOOR = 2e-4
+
+
+def silu64(g):
+    g = np.asarray(g, np.float64)
+    return g / (1.0 + np.exp(-g))
+
+
+def mlp_expectation(oracle, st, l, x):
+    """The MLP of layer l on its fp16 input x [hidden] (o_proj off, so x is also the residual): per norm candidate of ln2,
+    (want, bound) of x_out = fp16(x + down(act)), act = silu(gate) * up in float64 on the exact projections.
+
+    gate / up: the kernel's fp16 values are within Bg / Bu (rounded_bound of step_gemv) of the exact g / u.  silu moves by at most
+    1.1 Bg (|silu'| <= 1.1), and silu_h adds SILU_REL of its value (SILU_FLOOR where g may lie below -11): ds.  The product
+    rounds once more: |act' - act| <= (|s| + ds) Bu + |u| ds + 2^-11 (|act| + that).  down: step_gemv on act with that dx, then
+    the residual add's rounding."""
+    s = st.shape
+    L = st.layers[l]
+    out = []
+    for xn in norm_candidates(x, _np(L.ln2), s.eps):
+        gr, ge = step_gemv(oracle, xn, L.gate, adapter_of(st, l, "gate"))
+        ur, ue = step_gemv(oracle, xn, L.up, adapter_of(st, l, "up"))
+        bg, bu = rounded_bound(gr, ge), rounded_bound(ur, ue)
+        sr = silu64(gr)
+        ds = 1.1 * bg + SILU_REL * (np.abs(sr) + 1.1 * bg) + np.where(gr - bg < -11.0, SILU_FLOOR, 0.0) + 2 * FP16_TINY
+        act = sr * ur
+        da = (np.abs(sr) + ds) * bu + np.abs(ur) * ds
+        da = da + 2.0 ** -11 * (np.abs(act) + da) + FP16_TINY
+        dr, de = step_gemv(oracle, act, L.down, adapter_of(st, l, "down"), dx=da)
+        x64 = np.asarray(x, np.float16).astype(np.float64).reshape(1, -1)
+        out.append(((x64 + dr).reshape(-1), rounded_bound(dr, de, x64).reshape(-1)))
+    return out
+
+
+def o_expectation_ctx0(oracle, st, l, x, v_new):
+    """o_proj of layer l at context 0 on its fp16 residual x [hidden] (MLP off): the attention over one row gives that row weight
+    exactly 1, so every query head's output is its KV group's new v row v_new [kv_heads, hd] bit for bit (the kernel's own, read
+    from the cache).  (want, bound) of x_out = fp16(x + o(attn)): step_gemv on that exact input, and the residual's rounding."""
+    s = st.shape
+    n_rep = s.heads // s.kv_heads
+    attn = np.repeat(np.asarray(v_new, np.float16).reshape(s.kv_heads, 1, s.head_dim), n_rep, axis=1).reshape(1, -1)
+    r, e = step_gemv(oracle, attn, st.layers[l].o, adapter_of(st, l, "o"))
+    x64 = np.asarray(x, np.float16).astype(np.float64).reshape(1, -1)
+    return (x64 + r).reshape(-1), rounded_bound(r, e, x64).reshape(-1)
+
+
+def head_expectation(x_out, norm, lm_head, eps):
+    """Logits of the HEAD phase on the kernel's own final hidden state x_out [hidden]: per norm candidate (norm_candidates of the
+    final norm), (want, bound) with want = h . lm_head^T in float64 on the fp16 normalised h.  The products of two fp16 values
+    are exact in fp32, so the only error is fp32 summation (decode_step.cu, HEAD): a lane's fhfma2 chain over at most 2 chunks of
+    512 (32 fmas), 5 shuffle adds, and one atomic add per warp partial of the row (at most H / 1024 + 2 of them), each rounding
+    a partial sum no larger than sum_k |h_k w_k|: bound = n 2^-24 (1 + 2^-18) sum_k |h_k w_k|, n = 32 + 5 + H / 1024 + 2."""
+    x_out = np.asarray(x_out, np.float16).reshape(1, -1)
+    H = x_out.shape[1]
+    lm_head = np.asarray(lm_head, np.float16)
+    n = 32 + 5 + H // 1024 + 2
+    h = np.concatenate(norm_candidates(x_out, norm, eps)).astype(np.float64).T          # [H, 3]
+    want, s = np.empty((lm_head.shape[0], 3)), np.empty((lm_head.shape[0], 3))
+    for r in range(0, lm_head.shape[0], 2048):                                           # float64 in row blocks: 70B widths stay small
+        W = lm_head[r:r + 2048].astype(np.float64)
+        want[r:r + 2048] = W @ h
+        s[r:r + 2048] = np.abs(W) @ np.abs(h)
+    return [(want[:, c], n * 2.0 ** -24 * (1 + 2.0 ** -18) * s[:, c] + 1e-30) for c in range(3)]
+
+
+def assert_within_any(got, cands, what=""):
+    """got within the bound of at least one candidate: cands is a list of (want, bound), or -- several outputs checked together,
+    got a tuple of them -- a list of tuples of (want, bound).  Returns the largest err / bound of the best candidate."""
+    if not isinstance(got, tuple):
+        got, cands = (got,), [(c,) for c in cands]
+    best, msg = np.inf, ""
+    for c in cands:
+        ratios = []
+        for gv, (want, bound) in zip(got, c):
+            gv = np.asarray(gv, np.float64).reshape(np.shape(want))
+            assert np.isfinite(gv).all(), f"{what}: non-finite output"
+            ratios.append(np.abs(gv - want) / bound)
+        j = int(np.argmax([r.max() for r in ratios]))
+        if ratios[j].max() < best:
+            best, r, (want, bound) = float(ratios[j].max()), ratios[j], c[j]
+            i = np.unravel_index(np.argmax(r), r.shape)
+            msg = (f"output {j}: {(r > 1).sum()} / {r.size} outside; worst at {i}: err / bound {r[i]:.3g} (bound {bound[i]:.3g}, "
+                   f"want {want[i]:.4g}; rms bound / rms want {np.sqrt(np.mean(bound ** 2) / max(np.mean(want ** 2), 1e-300)):.2e})")
+    assert best <= 1.0, f"{what}: no norm candidate fits: {msg}"
+    return best

@@ -7,7 +7,7 @@ that wants the fixtures imports them by name (`from stack_harness import lib_sta
 import numpy as np
 import pytest
 
-from helpers import assert_close_ref64, att_needs_reset, oracle_decode_step
+from helpers import assert_close_ref64, assert_within_any, att_needs_reset, head_expectation, oracle_decode_step
 
 
 def _np(t):
@@ -108,11 +108,18 @@ def untouched_except(st, snap, pasts):
             assert torch.equal(kc[b][:, mask], snap[i][0][b][:, mask]) and torch.equal(vc[b][:, mask], snap[i][1][b][:, mask]), (i, b)
 
 
+def check_head(st, logits, x_out, what):
+    """The HEAD phase on the kernel's own final hidden state: logits [vocab] within head_expectation's fp32-summation bound of
+    rms_norm(x_out, norm) . lm_head^T (one of the three fp16 row factors), about 1e-4 of their rms."""
+    return assert_within_any(np.asarray(logits, np.float64).reshape(-1),
+                             head_expectation(x_out, _np(st.norm), _np(st.lm_head), st.shape.eps), f"{what} HEAD")
+
+
 def check_fused_step(oracle, st, xs, pasts, what):
     """The fused step (st's plan) on xs [bsz, 1, hidden] at contexts pasts against the per-op path, run sequence by sequence from the
     same caches, and -- unless oracle is None -- against oracle_decode_step: for every sequence the final hidden state, the logits
     and the new k and v rows, and no cache row written but pasts[b] of sequence b.  With oracle None: the logits against the per-op
-    path only.  Returns (logits [bsz, vocab], per-op logits, oracle logits or None) as numpy arrays per sequence."""
+    path only.  Either way the logits against the kernel's own final hidden state (check_head).  Returns (logits [bsz, vocab], per-op logits, oracle logits or None) as numpy arrays per sequence."""
     import torch
     bsz = len(pasts)
     snap = snapshot(st)
@@ -123,11 +130,13 @@ def check_fused_step(oracle, st, xs, pasts, what):
     logits = _np(got)
     ref_logits = [_np(r).reshape(-1) for r in ref_logits]
     want_logits = None
+    got_x = _np(st._plan_xout.view(-1, st.shape.hidden)[:bsz])
+    for b in range(bsz):
+        check_head(st, logits[b], got_x[b], f"{what} seq {b} (ctx {pasts[b]})")
     if oracle is None:
         for b in range(bsz):
             assert_close_ref64(logits[b], ref_logits[b].astype(np.float64), rel=1.5e-2, rms=1.5e-2, what=f"{what} seq {b} logits")
         return logits, ref_logits, want_logits
-    got_x = _np(st._plan_xout.view(-1, st.shape.hidden)[:bsz])
     want_logits = []
     for b in range(bsz):
         want_x, want, rows = oracle_decode_step(oracle, st, snap, _np(xs[b]), pasts[b], b)
@@ -150,7 +159,8 @@ def check_fused_step(oracle, st, xs, pasts, what):
 def check_sequence_and_graph(st, xs, starts, replay_tol=2e-3):
     """Consecutive tokens xs[t] [bsz, 1, hidden], sequence b at context starts[b] + t (barrier generation, accumulator clean-up and
     the cache rows carry over between launches), against the per-op path token by token and sequence by sequence; then the last
-    launch replayed from a CUDA graph.  fp32 atomics make bit-identical results across launches not required: the logits agree."""
+    launch replayed from a CUDA graph.  fp32 atomics make bit-identical results across launches not required: the logits agree, and
+    the replay's logits are held to check_head on the replay's own final hidden state."""
     import torch
     bsz = len(starts)
     snap = snapshot(st)
@@ -173,6 +183,9 @@ def check_sequence_and_graph(st, xs, starts, replay_tol=2e-3):
         gr.replay()
     torch.cuda.synchronize()
     assert_close_ref64(_np(st._plan_logits)[:bsz], _np(got[-1]).astype(np.float64), rel=replay_tol, rms=replay_tol, what="graph replay")
+    xo = _np(st._plan_xout.view(-1, st.shape.hidden)[:bsz]); lg = _np(st._plan_logits.view(-1, st.shape.vocab)[:bsz])
+    for b in range(bsz):
+        check_head(st, lg[b], xo[b], f"graph replay seq {b}")
 
 
 def check_reset_after_long_context(st, xs, contexts, check_untouched=False):

@@ -276,11 +276,13 @@ __device__ __forceinline__ float row_absmax(const uint4& hv)
 // Grid-wide barrier for the consumer threads of all CTAs: one monotonic 64-bit arrival counter (never reset, so graph replays
 // and back-to-back launches need no host-side state); every CTA adds 1 with release semantics and polls until the count reaches
 // the target of this barrier.  One L2 round trip to arrive, one to observe.
-__device__ __forceinline__ void grid_barrier(unsigned long long* ctr, unsigned long long& target, unsigned nctas, int tid)
+__device__ __forceinline__ void grid_barrier(unsigned long long* ctr, unsigned long long& target, unsigned nctas, int tid,
+                                             volatile int* arrived = nullptr)
 {
     consumer_sync();
     if (tid == 0) {
         asm volatile("red.release.gpu.global.add.u64 [%0], 1;" :: "l"(ctr) : "memory");
+        if (arrived) *arrived = *arrived + 1;
         unsigned long long v;
         asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(ctr) : "memory");
         if (v < target) {
@@ -331,6 +333,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
     // The schedule does not depend on the layer (nor, except ATT, on anything but the shapes): this CTA's unit range of every phase,
     // its shares of the buffers it zeroes and the CTA range of every head's attention units are computed ONCE per launch.  (They were
     // 64-bit divisions re-done by every thread in every phase of every layer: 5 % of all instructions executed, in the prologues.)
+    __shared__ volatile int s_arrived;                          // phase-end barrier arrivals of this CTA (release fence done)
     __shared__ int s_rng[6][4];                                  // [phase kind]{lo, hi, first K stage lo % spt, K stages to quantise min(hi - lo, spt)}
     __shared__ int s_zr[ZR_COUNT][2];                            // [buffer][lo, hi) in units of 4 floats (ZR_HALF: 2 floats)
     __shared__ unsigned short s_clo[DS_MAX_HEADS], s_chi[DS_MAX_HEADS];        // by virtual head b * heads + h
@@ -339,6 +342,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
     const int G = (int)gridDim.x, cta = (int)blockIdx.x;
 
     if (tid == 0) {
+        s_arrived = 0;
         for (int i = 0; i < nst; i++) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 4); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -375,7 +379,16 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         // rest of the phase, streamed while no barrier is near, keeps up to MID_INFLIGHT stages in flight (DESIGN 3c).
         int nph = 0;                                                          // stages of this pipeline issued in the current phase
         const int kmid = MID_INFLIGHT < depth ? MID_INFLIGHT : depth;
+        // The release fence of that arrival waits for every load the SM has in flight, so past the first stage of a phase the
+        // producer also waits until its CTA has arrived at the barrier that ends the previous phase (hold_q: phase-end arrivals
+        // before this phase).  The fence then finds at most the one stage per pipeline that was issued ahead, usually landed.
+        // Tensor parallel plans end O and DOWN with a push instead of a barrier, so they do not hold.
+        int hold_q = 0;
         auto acquire = [&](uint32_t tx) -> uint32_t {
+            if constexpr (!TP) if (nph == 1 && s_arrived < hold_q) {
+                const unsigned long long t0 = gtime();
+                while (s_arrived < hold_q) if (gtime() - t0 > WAIT_NS) __trap();
+            }
             if (issued >= depth) mbar_wait(empty0 + ls * 8, par ^ 1u);
             const int k = nph < depth ? 1 : kmid;
             if (issued >= k) { int pj = ls - k; uint32_t pp = par; if (pj < 0) { pj += depth; pp ^= 1u; } mbar_wait(full0 + pj * 8, pp); }
@@ -395,6 +408,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             #pragma unroll 1
             for (int ph = PH_QKV; ph <= PH_DOWN; ph++) {
                 const Phase p = phase_of(a, ph, G, nb);
+                hold_q = l * 5 + ph;
                 const int u0 = s_rng[ph][0], u1 = s_rng[ph][1];
                 const int i0 = ((pq - jbase) & 3);
                 jbase += u1 - u0;
@@ -441,6 +455,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             const int u0 = s_rng[PH_HEAD][0], u1 = s_rng[PH_HEAD][1];
             const int i0 = ((pq - jbase) & 3);
             nph = 0;
+            hold_q = a.n_layers * 5;
             const long long total = (long long)a.vocab * a.H * 2;
             const unsigned char* src = reinterpret_cast<const unsigned char*>(a.lm_head);
             #pragma unroll 1
@@ -1118,7 +1133,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             jbase += u1 - u0;
             stamp(l, 2);
         }
-        grid_barrier(a.bar, target, (unsigned)G, tid);
+        grid_barrier(a.bar, target, (unsigned)G, tid, &s_arrived);
         stamp(l, 3);
 
         // ======================================================== ATT ========================================================
@@ -1281,7 +1296,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             jbase += u1 - u0;
             stamp(l, 4);
         }
-        grid_barrier(a.bar, target, (unsigned)G, tid);
+        grid_barrier(a.bar, target, (unsigned)G, tid, &s_arrived);
         stamp(l, 5);
 
         // ========================================================= O =========================================================
@@ -1368,7 +1383,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             stamp(l, 7);
         }
         if constexpr (TP) push_partial(a.acc_o, a.push_o, epoch0 + 2u * l, l, 16);
-        else grid_barrier(a.bar, target, (unsigned)G, tid);
+        else grid_barrier(a.bar, target, (unsigned)G, tid, &s_arrived);
         stamp(l, 8);
 
         // ========================================================= GU ========================================================
@@ -1393,7 +1408,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             jbase += u1 - u0;
             stamp(l, 10);
         }
-        grid_barrier(a.bar, target, (unsigned)G, tid);
+        grid_barrier(a.bar, target, (unsigned)G, tid, &s_arrived);
         stamp(l, 11);
 
         // ======================================================== DOWN =======================================================
@@ -1451,7 +1466,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             stamp(l, 13);
         }
         if constexpr (TP) push_partial(a.acc_d, a.push_d, epoch0 + 2u * l + 1u, l, 18);
-        else grid_barrier(a.bar, target, (unsigned)G, tid);
+        else grid_barrier(a.bar, target, (unsigned)G, tid, &s_arrived);
         stamp(l, 14);
     }
 

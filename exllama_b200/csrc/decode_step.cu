@@ -35,7 +35,8 @@
 //  * Batched decode (template flag BATCH, up to MAX_BATCH = 4 sequences, each at its own context): the same weight stages, ring and
 //    IMMAs serve every sequence.  Sequence b's two x planes ride in B columns 2b, 2b + 1, so lane t of an MMA quad ends up holding
 //    sequence t's result; ATT runs over virtual heads (sequence, head) with each sequence's own context and cache rows; the head
-//    dots every lm_head stage with every sequence.  Only the K/V bytes grow with the batch.
+//    dots every lm_head stage with every sequence.  Only the K/V bytes grow with the batch.  The prologues and the head are written
+//    once, as loops over the nb sequences of the launch; without BATCH nb is the compile-time 1 and the loops fold away.
 //  * LoRA adapters (template flag LORA, one GPU): an adapted phase gets an LA step after its prologue (t = x . A over (matrix, K stage)
 //    units, fp32 red.add into L2, one grid barrier), and the CTA owning K stage 0 of an adapted tile adds fp16(t) . B to it after the
 //    GEMV (decode_step_sched.h: lora_*).
@@ -522,67 +523,10 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
     grid_barrier(a.bar, target, (unsigned)G, tid);
     if (TP && cta == 0 && tid == 0) *a.launch_ctr = (unsigned)s_base_x + 1u;      // every CTA has read it (it is past the barrier)
 
-    // ---- residual add (fp16(x + fp32 delta), the rounding point of q4_matmul's no_zero epilogue) + row factor of the RMS norm ----
-    auto residual_and_norm = [&](const float* delta, const uint2* slots = nullptr, unsigned epoch = 0u) -> float {
-        asm volatile("cp.async.wait_all;" ::: "memory");
-        float ss = 0.f;
-        for (int i = tid; i < a.H / 8; i += DS_CONSUMERS) {
-            uint4 xv = reinterpret_cast<uint4*>(xres)[i];
-            half2* h = reinterpret_cast<half2*>(&xv);
-            if (delta) {
-                const float4 own0 = ldcg4(delta + i * 8), own1 = ldcg4(delta + i * 8 + 4);
-                float4 d0 = own0, d1 = own1;
-                if (TP && slots) {
-                    // tensor parallel: the sum over ALL ranks' partials in rank order (bitwise identical on every rank); the peers'
-                    // partials sit in this rank's slots as {value, epoch} pairs, polled until the epoch of this (layer, phase) shows up
-                    d0 = make_float4(0.f, 0.f, 0.f, 0.f); d1 = d0;
-                    for (int r = 0; r < a.tp_world; r++) {
-                        float e[8];
-                        if (r == a.tp_rank) {
-                            e[0] = own0.x; e[1] = own0.y; e[2] = own0.z; e[3] = own0.w; e[4] = own1.x; e[5] = own1.y; e[6] = own1.z; e[7] = own1.w;
-                        } else {
-                            const uint4* sp = reinterpret_cast<const uint4*>(slots + (size_t)r * a.H + i * 8);
-                            #pragma unroll
-                            for (int q = 0; q < 4; q++) {
-                                uint4 v;
-                                asm volatile("ld.relaxed.sys.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(sp + q) : "memory");
-                                if (v.y != epoch || v.w != epoch) {
-                                    const unsigned long long t0 = gtime();
-                                    unsigned spin = 0;
-                                    do {
-                                        asm volatile("ld.relaxed.sys.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(sp + q) : "memory");
-                                        if ((++spin & 1023u) == 0 && gtime() - t0 > WAIT_NS) __trap();
-                                    } while (v.y != epoch || v.w != epoch);
-                                }
-                                e[2 * q] = __uint_as_float(v.x); e[2 * q + 1] = __uint_as_float(v.z);
-                            }
-                        }
-                        d0.x += e[0]; d0.y += e[1]; d0.z += e[2]; d0.w += e[3]; d1.x += e[4]; d1.y += e[5]; d1.z += e[6]; d1.w += e[7];
-                    }
-                }
-                float2 f;
-                f = __half22float2(h[0]); h[0] = __floats2half2_rn(f.x + d0.x, f.y + d0.y);
-                f = __half22float2(h[1]); h[1] = __floats2half2_rn(f.x + d0.z, f.y + d0.w);
-                f = __half22float2(h[2]); h[2] = __floats2half2_rn(f.x + d1.x, f.y + d1.y);
-                f = __half22float2(h[3]); h[3] = __floats2half2_rn(f.x + d1.z, f.y + d1.w);
-                reinterpret_cast<uint4*>(xres)[i] = xv;
-            }
-            #pragma unroll
-            for (int j = 0; j < 4; j++) { const float2 f = __half22float2(h[j]); ss = fmaf(f.x, f.x, ss); ss = fmaf(f.y, f.y, ss); }
-        }
-        #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-        if (lane == 0) s_red[warp] = ss;
-        consumer_sync();                                      // also publishes the updated xres
-        float tot = 0.f;
-        #pragma unroll
-        for (int w = 0; w < DS_NCW; w++) tot += s_red[w];     // same order in every thread
-        return __half2float(__float2half_rn(rsqrtf(tot / (float)a.H + a.eps)));       // rms_norm.cu:113-116
-    };
-
-    // ---- batched decode: the same per sequence b (residual stream b, accumulator row b, s_red row b); the row factors go to rmb ----
+    // ---- per sequence b (residual stream b, accumulator row b, s_red row b): residual add (fp16(x + fp32 delta), the rounding point of
+    // q4_matmul's no_zero epilogue) + row factor of the RMS norm into rmb[b].  Without BATCH nb is the constant 1 and the loops fold away.
     float rmb[MAX_BATCH] = {0.f, 0.f, 0.f, 0.f};
-    auto residual_and_norm_b = [&](const float* delta) {
+    auto residual_and_norm = [&](const float* delta, const uint2* slots = nullptr, unsigned epoch = 0u) {
         asm volatile("cp.async.wait_all;" ::: "memory");
         for (int b = 0; b < nb; b++) {
             float ss = 0.f;
@@ -592,7 +536,36 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
                 half2* h = reinterpret_cast<half2*>(&xv);
                 if (delta) {
                     const float* dp = delta + (size_t)b * a.H + i * 8;
-                    const float4 d0 = ldcg4(dp), d1 = ldcg4(dp + 4);
+                    const float4 own0 = ldcg4(dp), own1 = ldcg4(dp + 4);
+                    float4 d0 = own0, d1 = own1;
+                    if constexpr (TP) if (slots) {
+                        // tensor parallel (nb is 1): the sum over ALL ranks' partials in rank order (bitwise identical on every rank); the
+                        // peers' partials sit in this rank's slots as {value, epoch} pairs, polled until the epoch of this (layer, phase) shows up
+                        d0 = make_float4(0.f, 0.f, 0.f, 0.f); d1 = d0;
+                        for (int r = 0; r < a.tp_world; r++) {
+                            float e[8];
+                            if (r == a.tp_rank) {
+                                e[0] = own0.x; e[1] = own0.y; e[2] = own0.z; e[3] = own0.w; e[4] = own1.x; e[5] = own1.y; e[6] = own1.z; e[7] = own1.w;
+                            } else {
+                                const uint4* sp = reinterpret_cast<const uint4*>(slots + (size_t)r * a.H + i * 8);
+                                #pragma unroll
+                                for (int q = 0; q < 4; q++) {
+                                    uint4 v;
+                                    asm volatile("ld.relaxed.sys.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(sp + q) : "memory");
+                                    if (v.y != epoch || v.w != epoch) {
+                                        const unsigned long long t0 = gtime();
+                                        unsigned spin = 0;
+                                        do {
+                                            asm volatile("ld.relaxed.sys.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(sp + q) : "memory");
+                                            if ((++spin & 1023u) == 0 && gtime() - t0 > WAIT_NS) __trap();
+                                        } while (v.y != epoch || v.w != epoch);
+                                    }
+                                    e[2 * q] = __uint_as_float(v.x); e[2 * q + 1] = __uint_as_float(v.z);
+                                }
+                            }
+                            d0.x += e[0]; d0.y += e[1]; d0.z += e[2]; d0.w += e[3]; d1.x += e[4]; d1.y += e[5]; d1.z += e[6]; d1.w += e[7];
+                        }
+                    }
                     float2 f;
                     f = __half22float2(h[0]); h[0] = __floats2half2_rn(f.x + d0.x, f.y + d0.y);
                     f = __half22float2(h[1]); h[1] = __floats2half2_rn(f.x + d0.z, f.y + d0.w);
@@ -607,17 +580,19 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
             if (lane == 0) s_red[b * DS_NCW + warp] = ss;
         }
-        consumer_sync();
+        consumer_sync();                                      // also publishes the updated xres
         #pragma unroll
         for (int b = 0; b < MAX_BATCH; b++) {
             if (b >= nb) break;
             float tot = 0.f;
             #pragma unroll
-            for (int w = 0; w < DS_NCW; w++) tot += s_red[b * DS_NCW + w];
-            rmb[b] = __half2float(__float2half_rn(rsqrtf(tot / (float)a.H + a.eps)));
+            for (int w = 0; w < DS_NCW; w++) tot += s_red[b * DS_NCW + w];      // same order in every thread
+            rmb[b] = __half2float(__float2half_rn(rsqrtf(tot / (float)a.H + a.eps)));      // rms_norm.cu:113-116
         }
     };
-    auto rm_of = [&](int b) { return b == 0 ? rmb[0] : b == 1 ? rmb[1] : b == 2 ? rmb[2] : rmb[3]; };
+    // a select chain, not rmb[b]: a run-time index would put rmb in local memory.  Without BATCH b is always 0, which the compiler
+    // cannot see where b is computed (lora_a's i >> 4)
+    auto rm_of = [&](int b) { return (!BATCH || b == 0) ? rmb[0] : b == 1 ? rmb[1] : b == 2 ? rmb[2] : rmb[3]; };
 
     // ---- quantise the K stages [s0, s0 + n) (cyclic mod spt) of the phase input into xs / segt; `get(k8, it)` yields 8 fp16 values ----
     // BATCH: slot is the sequence, and stage s0 + j goes to compacted stage j of that sequence's area
@@ -664,20 +639,8 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         if (rpg == 16) stage_x(std::integral_constant<int, 16>{}, s0, n, spt, get, slot);
         else stage_x(std::integral_constant<int, 0>{}, s0, n, spt, get, slot);
     };
-    auto norm_get = [&](float rm) {
-        return [=](int k8, int it) -> uint4 {
-            uint4 xv = reinterpret_cast<const uint4*>(xres)[k8];
-            const uint4 wv = reinterpret_cast<const uint4*>(wnorm)[it * DS_CONSUMERS + tid];
-            const half2 rm2 = __float2half2_rn(rm);
-            half2* h = reinterpret_cast<half2*>(&xv); const half2* w2 = reinterpret_cast<const half2*>(&wv);
-            #pragma unroll
-            for (int i = 0; i < 4; i++) h[i] = __hmul2(__hmul2(h[i], rm2), w2[i]);      // rms_norm.cu:118-131
-            return xv;
-        };
-    };
-
-    // sequence b's residual stream, normalised with its row factor rm
-    auto norm_get_b = [&](int b, float rm) {
+    // sequence b's residual stream, normalised with its row factor rm and the norm weights preload_norm put in wnorm
+    auto norm_get = [&](int b, float rm) {
         const uint4* xr = reinterpret_cast<const uint4*>(xres + (size_t)b * a.H);
         return [=](int k8, int it) -> uint4 {
             uint4 xv = xr[k8];
@@ -685,7 +648,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             const half2 rm2 = __float2half2_rn(rm);
             half2* h = reinterpret_cast<half2*>(&xv); const half2* w2 = reinterpret_cast<const half2*>(&wv);
             #pragma unroll
-            for (int i = 0; i < 4; i++) h[i] = __hmul2(__hmul2(h[i], rm2), w2[i]);
+            for (int i = 0; i < 4; i++) h[i] = __hmul2(__hmul2(h[i], rm2), w2[i]);      // rms_norm.cu:118-131
             return xv;
         };
     };
@@ -1103,7 +1066,6 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         }
     };
 
-    float rm = 0.f;
     #pragma unroll 1
     for (int l = 0; l < a.n_layers; l++) {
         const LayerDesc* L = a.layers + l;
@@ -1113,19 +1075,13 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             const int u0 = s_rng[PH_QKV][0], u1 = s_rng[PH_QKV][1];
             stamp(l, 0);
             if (l > 0) zero_share(a.acc_gu, ZR_GU);
-            if constexpr (BATCH) {
-                residual_and_norm_b(l > 0 ? a.acc_d : nullptr);
-                stamp(l, 15);
-                if (u1 > u0) for (int b = 0; b < nb; b++) stage_xd(s_rng[p.kind][2], s_rng[p.kind][3], p.spt, norm_get_b(b, rm_of(b)), b);
-            } else {
-            rm = residual_and_norm(l > 0 ? a.acc_d : nullptr, (TP && !a.tp_reduce && l > 0) ? a.slots_d : nullptr, epoch0 + 2u * (l - 1) + 1u);
+            residual_and_norm(l > 0 ? a.acc_d : nullptr, (TP && !a.tp_reduce && l > 0) ? a.slots_d : nullptr, epoch0 + 2u * (l - 1) + 1u);
             stamp(l, 15);
-            if constexpr (!ACT) { if (u1 > u0) stage_xd(s_rng[p.kind][2], s_rng[p.kind][3], p.spt, norm_get(rm)); }
-            else stage_phase(p, u0, u1, [&](int m) { return norm_get_map(L->ln1, rm, L->xmap[m]); });
-            }
+            if constexpr (!ACT) { if (u1 > u0) for (int b = 0; b < nb; b++) stage_xd(s_rng[p.kind][2], s_rng[p.kind][3], p.spt, norm_get(b, rm_of(b)), b); }
+            else stage_phase(p, u0, u1, [&](int m) { return norm_get_map(L->ln1, rm_of(0), L->xmap[m]); });
             consumer_sync();
             if constexpr (LORA) {
-                if (lora_a(l, p, [&](int b) { return lora_norm_get(L->ln1, b, BATCH ? rm_of(b) : rm); })) grid_barrier(a.bar, target, (unsigned)G, tid);
+                if (lora_a(l, p, [&](int b) { return lora_norm_get(L->ln1, b, rm_of(b)); })) grid_barrier(a.bar, target, (unsigned)G, tid);
             }
             stamp(l, 1);
             gemv(p, u0, u1);
@@ -1341,14 +1297,11 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
                 for (int i = 0; i < 4; i++) hh[i] = __floats2half2_rn(ov[2 * i] * inv, ov[2 * i + 1] * inv);
                 return r;
             };
-            if constexpr (BATCH) {
-                // sequence b: stage k of o_proj is virtual head b * heads + k
+            if constexpr (!ACT) {
+                // stage k of sequence b's o_proj input is virtual head b * heads + k: the CTA combines exactly the heads its K range needs
                 if (u1 > u0)
                     for (int b = 0; b < nb; b++)
                         stage_xd(s_rng[PH_O][2], s_rng[PH_O][3], p.spt, [&](int k8, int) -> uint4 { return combine8(b * a.heads + (k8 >> 4), (k8 & 15) * 8); }, b);
-            } else if constexpr (!ACT) {
-                // stage k of o_proj is head k: the CTA combines exactly the heads its K range needs
-                if (u1 > u0) stage_xd(s_rng[PH_O][2], s_rng[PH_O][3], p.spt, [&](int k8, int) -> uint4 { return combine8(k8 >> 4, (k8 & 15) * 8); });
             } else {
                 // act-order o_proj: its input is a gather over ALL heads (x_map), so the combined attention output is first written
                 // to L2 once (head h by CTA h mod grid), one extra grid barrier, then every CTA gathers what its K range needs
@@ -1390,17 +1343,12 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         {
             const Phase p = phase_of(a, PH_GU, G, nb);
             const int u0 = s_rng[PH_GU][0], u1 = s_rng[PH_GU][1];
-            if constexpr (BATCH) {
-                residual_and_norm_b(a.acc_o);
-                if (u1 > u0) for (int b = 0; b < nb; b++) stage_xd(s_rng[p.kind][2], s_rng[p.kind][3], p.spt, norm_get_b(b, rm_of(b)), b);
-            } else {
-            rm = residual_and_norm(a.acc_o, (TP && !a.tp_reduce) ? a.slots_o : nullptr, epoch0 + 2u * l);
-            if constexpr (!ACT) { if (u1 > u0) stage_xd(s_rng[p.kind][2], s_rng[p.kind][3], p.spt, norm_get(rm)); }
-            else stage_phase(p, u0, u1, [&](int m) { return norm_get_map(L->ln2, rm, L->xmap[m]); });
-            }
+            residual_and_norm(a.acc_o, (TP && !a.tp_reduce) ? a.slots_o : nullptr, epoch0 + 2u * l);
+            if constexpr (!ACT) { if (u1 > u0) for (int b = 0; b < nb; b++) stage_xd(s_rng[p.kind][2], s_rng[p.kind][3], p.spt, norm_get(b, rm_of(b)), b); }
+            else stage_phase(p, u0, u1, [&](int m) { return norm_get_map(L->ln2, rm_of(0), L->xmap[m]); });
             consumer_sync();
             if constexpr (LORA) {
-                if (lora_a(l, p, [&](int b) { return lora_norm_get(L->ln2, b, BATCH ? rm_of(b) : rm); })) grid_barrier(a.bar, target, (unsigned)G, tid);
+                if (lora_a(l, p, [&](int b) { return lora_norm_get(L->ln2, b, rm_of(b)); })) grid_barrier(a.bar, target, (unsigned)G, tid);
             }
             stamp(l, 9);
             gemv(p, u0, u1);
@@ -1471,83 +1419,26 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
     }
 
     // ========================================================= HEAD ==========================================================
-    if constexpr (BATCH) residual_and_norm_b(a.n_layers > 0 ? a.acc_d : nullptr);
-    else rm = residual_and_norm(a.n_layers > 0 ? a.acc_d : nullptr, (TP && !a.tp_reduce && a.n_layers > 0) ? a.slots_d : nullptr, epoch0 + 2u * (a.n_layers - 1) + 1u);
+    residual_and_norm(a.n_layers > 0 ? a.acc_d : nullptr, (TP && !a.tp_reduce && a.n_layers > 0) ? a.slots_d : nullptr, epoch0 + 2u * (a.n_layers - 1) + 1u);
     if (a.x_out && cta == 0)
         for (int i = tid; i < nb * a.H / 8; i += DS_CONSUMERS) reinterpret_cast<uint4*>(a.x_out)[i] = reinterpret_cast<const uint4*>(xres)[i];
-    if constexpr (BATCH) {
-        if (a.lm_head) {
-            const int u0 = s_rng[PH_HEAD][0], u1 = s_rng[PH_HEAD][1];
-            const int h8 = a.H / 8;
-            for (int i = tid; i < nb * h8; i += DS_CONSUMERS) {
-                const int b = i / h8, j = i - b * h8;
-                uint4 xv = reinterpret_cast<const uint4*>(xres)[i];
-                const uint4 wv = __ldg(reinterpret_cast<const uint4*>(a.final_norm) + j);
-                const half2 rm2 = __float2half2_rn(rm_of(b));
-                half2* h = reinterpret_cast<half2*>(&xv); const half2* w2 = reinterpret_cast<const half2*>(&wv);
-                #pragma unroll
-                for (int q = 0; q < 4; q++) h[q] = __hmul2(__hmul2(h[q], rm2), w2[q]);
-                reinterpret_cast<uint4*>(xh)[i] = xv;
-            }
-            consumer_sync();
-            // as below, but every 8 KB lm_head stage is dotted with every sequence's normalised x
-            const int cpr = a.H >> 9;
-            const long long nchunks = (long long)a.vocab * cpr;
-            for (int u = u0 + ((wk - jbase) & 3); u < u1; u += 4) {
-                mbar_wait(full0 + ls * 8, par);
-                const unsigned char* sb = ring + (size_t)(wk * depth + ls) * STAGE_STRIDE;
-                const long long c0 = (long long)u * 8 + wn * 2;
-                long long row = c0 / cpr; int kc = (int)(c0 - row * cpr);
-                float part[MAX_BATCH] = {0.f, 0.f, 0.f, 0.f};
-                #pragma unroll 1
-                for (int cc = 0; cc < ((a.debug & 4) ? 0 : 2) && c0 + cc < nchunks; cc++) {
-                    #pragma unroll
-                    for (int hf = 0; hf < 2; hf++) {
-                        const uint4 wv = *reinterpret_cast<const uint4*>(sb + (wn * 2 + cc) * 1024 + hf * 512 + lane * 16);
-                        #pragma unroll
-                        for (int b = 0; b < MAX_BATCH; b++) {
-                            if (b < nb) {
-                                const uint4 xv = *reinterpret_cast<const uint4*>(reinterpret_cast<const unsigned char*>(xh + (size_t)b * a.H) + (size_t)kc * 1024 + hf * 512 + lane * 16);
-                                part[b] = fhfma2(wv.x, xv.x, part[b]); part[b] = fhfma2(wv.y, xv.y, part[b]);
-                                part[b] = fhfma2(wv.z, xv.z, part[b]); part[b] = fhfma2(wv.w, xv.w, part[b]);
-                            }
-                        }
-                    }
-                    if (++kc == cpr || cc == 1 || c0 + cc + 1 == nchunks) {
-                        #pragma unroll
-                        for (int b = 0; b < MAX_BATCH; b++) {
-                            if (b < nb) {
-                                float tot = part[b];
-                                #pragma unroll
-                                for (int off = 16; off > 0; off >>= 1) tot += __shfl_xor_sync(0xffffffffu, tot, off);
-                                if (lane == 0) atomicAdd(a.logits + (size_t)b * a.vocab + row, tot);
-                            }
-                            part[b] = 0.f;
-                        }
-                        if (kc == cpr) { kc = 0; row++; }
-                    }
-                }
-                __syncwarp();
-                if (lane == 0) mbar_arrive(empty0 + ls * 8);
-                if (++ls == depth) { ls = 0; par ^= 1u; }
-            }
-        }
-    } else if (a.lm_head) {
-        const Phase p = phase_of(a, PH_HEAD, G);
+    if (a.lm_head) {
         const int u0 = s_rng[PH_HEAD][0], u1 = s_rng[PH_HEAD][1];
-        {
-            const half2 rm2 = __float2half2_rn(rm);
-            for (int i = tid; i < a.H / 8; i += DS_CONSUMERS) {
-                uint4 xv = reinterpret_cast<const uint4*>(xres)[i];
-                const uint4 wv = __ldg(reinterpret_cast<const uint4*>(a.final_norm) + i);
+        const int h8 = a.H / 8;
+        for (int b = 0; b < nb; b++) {
+            const half2 rm2 = __float2half2_rn(rm_of(b));
+            for (int j = tid; j < h8; j += DS_CONSUMERS) {
+                uint4 xv = reinterpret_cast<const uint4*>(xres)[b * h8 + j];
+                const uint4 wv = __ldg(reinterpret_cast<const uint4*>(a.final_norm) + j);
                 half2* h = reinterpret_cast<half2*>(&xv); const half2* w2 = reinterpret_cast<const half2*>(&wv);
                 #pragma unroll
                 for (int q = 0; q < 4; q++) h[q] = __hmul2(__hmul2(h[q], rm2), w2[q]);
-                reinterpret_cast<uint4*>(xh)[i] = xv;
+                reinterpret_cast<uint4*>(xh)[b * h8 + j] = xv;
             }
         }
         consumer_sync();
-        // stage = 8 chunks of 512 fp16 of the row-major [vocab, H] matrix; the 4 warps of the pipeline take 2 chunks each
+        // stage = 8 chunks of 512 fp16 of the row-major [vocab, H] matrix; the 4 warps of the pipeline take 2 chunks each and dot
+        // every chunk with every sequence's normalised x
         const int cpr = a.H >> 9;                               // chunks per vocabulary row
         const long long nchunks = (long long)a.vocab * cpr;
         for (int u = u0 + ((wk - jbase) & 3); u < u1; u += 4) {
@@ -1555,22 +1446,32 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             const unsigned char* sb = ring + (size_t)(wk * depth + ls) * STAGE_STRIDE;
             const long long c0 = (long long)u * 8 + wn * 2;
             long long row = c0 / cpr; int kc = (int)(c0 - row * cpr);
-            float part = 0.f;
+            float part[MAX_BATCH] = {0.f, 0.f, 0.f, 0.f};
             #pragma unroll 1
             for (int cc = 0; cc < ((a.debug & 4) ? 0 : 2) && c0 + cc < nchunks; cc++) {
                 #pragma unroll
                 for (int hf = 0; hf < 2; hf++) {
                     const uint4 wv = *reinterpret_cast<const uint4*>(sb + (wn * 2 + cc) * 1024 + hf * 512 + lane * 16);
-                    const uint4 xv = *reinterpret_cast<const uint4*>(reinterpret_cast<const unsigned char*>(xh) + (size_t)kc * 1024 + hf * 512 + lane * 16);
-                    part = fhfma2(wv.x, xv.x, part); part = fhfma2(wv.y, xv.y, part);
-                    part = fhfma2(wv.z, xv.z, part); part = fhfma2(wv.w, xv.w, part);
+                    #pragma unroll
+                    for (int b = 0; b < MAX_BATCH; b++) {
+                        if (b < nb) {
+                            const uint4 xv = *reinterpret_cast<const uint4*>(reinterpret_cast<const unsigned char*>(xh + (size_t)b * a.H) + (size_t)kc * 1024 + hf * 512 + lane * 16);
+                            part[b] = fhfma2(wv.x, xv.x, part[b]); part[b] = fhfma2(wv.y, xv.y, part[b]);
+                            part[b] = fhfma2(wv.z, xv.z, part[b]); part[b] = fhfma2(wv.w, xv.w, part[b]);
+                        }
+                    }
                 }
                 if (++kc == cpr || cc == 1 || c0 + cc + 1 == nchunks) {
-                    float tot = part;
                     #pragma unroll
-                    for (int off = 16; off > 0; off >>= 1) tot += __shfl_xor_sync(0xffffffffu, tot, off);
-                    if (lane == 0) atomicAdd(a.logits + row, tot);
-                    part = 0.f;
+                    for (int b = 0; b < MAX_BATCH; b++) {
+                        if (b < nb) {
+                            float tot = part[b];
+                            #pragma unroll
+                            for (int off = 16; off > 0; off >>= 1) tot += __shfl_xor_sync(0xffffffffu, tot, off);
+                            if (lane == 0) atomicAdd(a.logits + (size_t)b * a.vocab + row, tot);
+                        }
+                        part[b] = 0.f;
+                    }
                     if (kc == cpr) { kc = 0; row++; }
                 }
             }

@@ -82,6 +82,8 @@ SIGNATURES = {
     "exl_decode_plan_info": (i32, [vp, C.POINTER(i32), C.POINTER(i32), C.POINTER(i64), C.POINTER(i64)]),
     "exl_decode_step": (i32, [vp, vp, i32, vp, vp, vp]),
     "exl_decode_step_batch": (i32, [vp, vp, i32, C.POINTER(i32), vp, vp, vp]),
+    "exl_decode_plan_create_multi": (i32, [vp, i32, i32, C.POINTER(vp)]),
+    "exl_decode_step_multi": (i32, [vp, vp, i32, i32, i32, vp, vp, vp]),
     "exl_decode_plan_trace": (i32, [vp, vp, i64]),
     "exl_decode_plan_ipc_export": (i32, [vp, vp]),
     "exl_decode_plan_ipc_import": (i32, [vp, vp, i32]),
@@ -298,10 +300,13 @@ class DecodePlan:
     borrowed and must outlive the plan.  num_kv_heads (grouped-query attention, default num_heads): k_proj / v_proj are
     num_kv_heads * head_dim wide; single GPU only.  max_batch (1..4): sequences a step_batch() may carry; the caches are then
     [max_batch, num_kv_heads, max_seq_len, head_dim]; single GPU, no act-order.  lora: per layer None or a 7-tuple (q, k, v, o,
-    gate, up, down) of None or (A half [in, r], B half [r, out] already scaled by alpha / r), lora.py's layout; single GPU."""
+    gate, up, down) of None or (A half [in, r], B half [r, out] already scaled by alpha / r), lora.py's layout; single GPU.
+    max_tokens (1..4, instead of max_batch and lora): a multi-token plan, stepped by step_multi() with up to max_tokens consecutive
+    tokens of one cache sequence; the caches [cache_seqs, num_kv_heads, max_seq_len, head_dim] hold cache_seqs = their first
+    dimension; single GPU, no act-order."""
 
     def __init__(self, handles, ln1, ln2, key_cache, value_cache, sin, cos, num_heads, head_dim, max_seq_len, eps,
-                 final_norm=None, lm_head=None, tp_rank=0, tp_world=1, num_kv_heads=None, max_batch=1, lora=None):
+                 final_norm=None, lm_head=None, tp_rank=0, tp_world=1, num_kv_heads=None, max_batch=1, lora=None, max_tokens=None):
         n = len(handles)
         self._keep = (ln1, ln2, key_cache, value_cache, sin, cos, final_norm, lm_head)
         flat = []
@@ -326,7 +331,13 @@ class DecodePlan:
         self.hidden = ln1[0].shape[-1] if n else 0
         self.tp_world = tp_world
         self.max_batch = max_batch
+        self.max_tokens = max_tokens
         self.handle = vp()
+        if max_tokens is not None:
+            assert lora is None and max_batch == 1, "a multi-token plan takes neither a batch nor an adapter"
+            cache_seqs = key_cache[0].shape[0] if key_cache[0].dim() == 4 else 1
+            check(lib().exl_decode_plan_create_multi(C.byref(d), int(max_tokens), int(cache_seqs), C.byref(self.handle)))
+            return
         if lora is None:
             check(lib().exl_decode_plan_create_batch(C.byref(d), max_batch, C.byref(self.handle)))
             return
@@ -380,6 +391,17 @@ class DecodePlan:
         if logits is None and self.vocab:
             logits = torch.empty((bsz, self.vocab), dtype=torch.float32, device=x_in.device)
         check(lib().exl_decode_step_batch(self.handle, _ptr(x_in), bsz, lens, _ptr(x_out), _ptr(logits), _stream()))
+        return logits if logits is not None else x_out
+
+    def step_multi(self, x_in, past_len, seq=0, x_out=None, logits=None):
+        """n consecutive tokens of cache sequence seq in one launch (a multi-token plan): x_in half [n, hidden] (any shape with
+        n * hidden contiguous elements); token t at position past_len + t attends rows [0, past_len) and tokens 0..t, and writes row
+        past_len + t.  Returns logits float [n, vocab] (allocated when not given and the plan has a head), else x_out."""
+        import torch
+        n = x_in.numel() // self.hidden
+        if logits is None and self.vocab:
+            logits = torch.empty((n, self.vocab), dtype=torch.float32, device=x_in.device)
+        check(lib().exl_decode_step_multi(self.handle, _ptr(x_in), n, int(seq), int(past_len), _ptr(x_out), _ptr(logits), _stream()))
         return logits if logits is not None else x_out
 
     def trace(self):

@@ -37,6 +37,10 @@
 //    sequence t's result; ATT runs over virtual heads (sequence, head) with each sequence's own context and cache rows; the head
 //    dots every lm_head stage with every sequence.  Only the K/V bytes grow with the batch.  The prologues and the head are written
 //    once, as loops over the nb sequences of the launch; without BATCH nb is the compile-time 1 and the loops fold away.
+//  * Multi-token steps (template flag MULTI, with BATCH and the grouped-query ATT path for any n_rep): up to 4 consecutive tokens of ONE
+//    sequence (speculative verification, short chunks).  Token t sits at past_len + t; ATT runs over the real KV heads at past_len, so
+//    the history's K/V bytes are read once for all tokens, each stage serving n_rep x n query vectors, and a causal tail partial over
+//    the launch's own new rows 0 .. t (kept in shared memory) replaces the single new-token partial.  No row >= past_len is read.
 //  * LoRA adapters (template flag LORA, one GPU): an adapted phase gets an LA step after its prologue (t = x . A over (matrix, K stage)
 //    units, fp32 red.add into L2, one grid barrier), and the CTA owning K stage 0 of an adapted tile adds fp16(t) . B to it after the
 //    GEMV (decode_step_sched.h: lora_*).
@@ -124,6 +128,8 @@ struct StepArgs
     // LoRA adapters (LORA kernels only; the others read none of these): [n_layers * 7] matrices' adapters, and the fp32 t = x . A
     // accumulators in L2 (matrix of rank r at t_off: [max_batch][r]), zeroed at launch start
     const LoraMat* lora; float* lora_t; int lora_t4;              // lora_t4: floats of lora_t / 4
+    // multi-token steps (MULTI kernels only): the bsz tokens of the launch sit at positions past_len + t of cache sequence seq
+    int seq;
 };
 
 // ------------------------------------------------------------------------------------------------------------ helpers
@@ -303,8 +309,15 @@ __device__ __forceinline__ void grid_barrier(unsigned long long* ctr, unsigned l
 // for more than one sequence (neither ACT nor TP).  Compile-time so that the common kernel (none of them) carries none of their
 // address arithmetic, branches or code (the runtime-flag version of the same source was 10 % slower on the plain 7B step; a runtime
 // n_rep branch around the attention phase made ptxas spill in it).  Without BATCH, nb below is the constant 1.  LORA: a plan with
-// LoRA adapters (single GPU; any of the others but TP): the LA steps and B terms below.
-template <bool ACT, bool TP, bool GQA, bool BATCH, bool LORA = false>
+// LoRA adapters (single GPU; any of the others but TP): the LA steps and B terms below.  MULTI: bsz consecutive tokens of ONE sequence
+// (with BATCH and GQA, for any n_rep; neither ACT, TP nor LORA): the batch's GEMV, norm and head phases, and ATT over the real KV
+// heads at the shared context past_len, each stage serving n_rep * bsz query vectors, plus a causal tail over the launch's own rows.
+template <bool MULTI> __device__ __forceinline__ Phase step_phase(const StepArgs& a, int kind, int G, int nb)
+{
+    if constexpr (MULTI) return phase_of_multi(a, kind, G);
+    else return phase_of(a, kind, G, nb);
+}
+template <bool ACT, bool TP, bool GQA, bool BATCH, bool LORA = false, bool MULTI = false>
 __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid_constant__ StepArgs a)
 {
     extern __shared__ __align__(128) unsigned char smem[];
@@ -319,7 +332,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
     [[maybe_unused]] const uint32_t xs_seq = (uint32_t)a.xst * 256u, seg_seq = (uint32_t)a.xst * 32u;
     unsigned char* xs = ring + (size_t)nst * STAGE_STRIDE;                            // xstages x 16 k8-rows x 16 B: quantised x planes by K stage
     unsigned char* segt = xs + (size_t)xstages * 256;                                  // xstages x 4 x {sum x_q, x scale}
-    half* xres = reinterpret_cast<half*>(xs + stage_area_bytes(xstages, a.n_rep));    // [nb][H] residual streams (fp16, as the reference keeps them)
+    half* xres = reinterpret_cast<half*>(xs + (MULTI ? stage_area_bytes_multi(xstages, a.n_rep, nb) : stage_area_bytes(xstages, a.n_rep)));    // [nb][H] residual streams (fp16, as the reference keeps them)
     float* parts = reinterpret_cast<float*>(xres + (size_t)nb * a.H);                  // [2 segments][17][PART_LD] attention partials of the warps (+ the new token)
     float* q_s = parts + 2 * 17 * PART_LD;                                             // [2][128] scaled q of the segment's head
     float* kn_s = q_s + 2 * TILE;                                                      // [2][128] newest k row (after rope)
@@ -348,7 +361,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     if (tid >= 32 && tid < 38) {
-        const Phase p = phase_of(a, tid - 32, G, nb);
+        const Phase p = step_phase<MULTI>(a, tid - 32, G, nb);
         const int lo = range_lo(p.U, cta, p.G), hi = range_lo(p.U, cta + 1, p.G);
         s_rng[tid - 32][0] = lo; s_rng[tid - 32][1] = hi;
         s_rng[tid - 32][2] = (p.spt > 0 && hi > lo) ? lo % p.spt : 0;
@@ -359,8 +372,9 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
         if constexpr (BATCH) n *= nb;                              // [nb][width] (ZR_HALF is tensor parallel only)
         s_zr[k][0] = share_lo(n, cta, G); s_zr[k][1] = share_lo(n, cta + 1, G);
     } else if (tid >= 128 && tid < 128 + nb * a.heads) {
-        const Phase pa = phase_of(a, PH_ATT, G, nb);
-        const int h = tid - 128, kvh = h / a.n_rep;                // a query head's partials come from the CTAs of its KV head (virtual: b * kv_heads + kvh)
+        const Phase pa = step_phase<MULTI>(a, PH_ATT, G, nb);
+        const int h = tid - 128, kvh = (MULTI ? h % a.heads : h) / a.n_rep;      // a query head's partials come from the CTAs of its KV head (virtual: b * kv_heads + kvh;
+                                                                                  // MULTI: virtual query head t * heads + h' of token t reads real KV head h' / n_rep)
         s_clo[h] = (unsigned short)cta_of((long long)kvh * pa.tpm, pa.U, pa.G);
         s_chi[h] = (unsigned short)cta_of((long long)(kvh + 1) * pa.tpm - 1, pa.U, pa.G);
     }
@@ -408,7 +422,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             const LayerDesc* L = a.layers + l;
             #pragma unroll 1
             for (int ph = PH_QKV; ph <= PH_DOWN; ph++) {
-                const Phase p = phase_of(a, ph, G, nb);
+                const Phase p = step_phase<MULTI>(a, ph, G, nb);
                 hold_q = l * 5 + ph;
                 const int u0 = s_rng[ph][0], u1 = s_rng[ph][1];
                 const int i0 = ((pq - jbase) & 3);
@@ -420,11 +434,12 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
                     for (int u = u0 + i0; u < u1; u += 4) {
                         const int pos0 = ch * 16;
                         int plen = a.past_len;
-                        if constexpr (BATCH) plen = a.past_lens[h / a.kv_heads];        // h: virtual KV head, its rows sit at h * max_seq
+                        if constexpr (BATCH && !MULTI) plen = a.past_lens[h / a.kv_heads];        // h: virtual KV head, its rows sit at h * max_seq
                         int nv = plen - pos0; nv = nv < 0 ? 0 : (nv > 16 ? 16 : nv);
                         const uint32_t base = acquire((uint32_t)nv * 512u);
                         if (nv > 0) {
-                            const size_t off = ((size_t)h * a.max_seq + pos0) * TILE;
+                            // MULTI: h is a real KV head of cache sequence seq; rows [0, past_len) only, never the launch's own
+                            const size_t off = ((size_t)(MULTI ? a.seq * a.kv_heads + h : h) * a.max_seq + pos0) * TILE;
                             if (lane == 0) bulk_g2s(base, L->kc + off, (uint32_t)nv * 256u, full0 + ls * 8, pol);
                             if (lane == 1) bulk_g2s(base + 4096, L->vc + off, (uint32_t)nv * 256u, full0 + ls * 8, pol);
                         }
@@ -929,20 +944,50 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
     // the QKV GEMV and the O prologue), so a query head of a segment ends with 4 pipeline partials + the new token's, combined into the
     // CTA's slot of att_part as in the multi-head path.
     auto att_gqa = [&](const LayerDesc* L, int u0, int u1, int nph, int h0, int nseg) {
-        const int nr = a.n_rep;
+        const int nr = MULTI ? a.n_rep * nb : a.n_rep;                  // query vectors per KV head (MULTI: token t, query head r at t * n_rep + r)
+        const int nt = MULTI ? nb : 1;                                  // new k / v rows per KV head
         const float scale = rsqrtf((float)TILE);
         const int l16 = lane & 15, sub = lane >> 4;
-        half* gq = reinterpret_cast<half*>(xs + gqa_qh_off(nr));        // [2][n_rep][128] q after rope, fp16 (unscaled)
-        float* gkn = reinterpret_cast<float*>(xs + gqa_kn_off(nr));    // [2][128] newest k row (after rope)
-        float* gvn = gkn + 2 * TILE;                                    // [2][128] newest v row
+        half* gq = reinterpret_cast<half*>(xs + gqa_qh_off(nr));        // [2][nr][128] q after rope, fp16 (unscaled)
+        float* gkn = reinterpret_cast<float*>(xs + gqa_kn_off(nr));    // [2][nt][128] newest k rows (after rope)
+        float* gvn = gkn + 2 * nt * TILE;                               // [2][nt][128] newest v rows
         auto owner = [&](int kvh) { return min(u1, (kvh + 1) * nph) == (kvh + 1) * nph; };      // holds the KV head's last chunk
-        // BATCH: kvh is a virtual KV head b * kv_heads + kvh' -- its sequence's context, rope row and accumulator row
-        auto plen_of = [&](int kvh) { if constexpr (BATCH) return a.past_lens[kvh / a.kv_heads]; else return a.past_len; };
+        // BATCH: kvh is a virtual KV head b * kv_heads + kvh' -- its sequence's context, rope row and accumulator row.  MULTI: kvh is
+        // a real KV head and every token attends the same history
+        auto plen_of = [&](int kvh) { if constexpr (BATCH && !MULTI) return a.past_lens[kvh / a.kv_heads]; else return a.past_len; };
         const size_t qkv_ld = (size_t)a.HQ + 2 * a.HKV;
         const half* sr1 = a.sin + (size_t)a.past_len * TILE;
         const half* cr1 = a.cos + (size_t)a.past_len * TILE;
         // rope q of every query head of the segments (rope.cu:48-67, as the multi-head path); rope k and write the k / v cache rows
         // once per KV head, by its owner; every pipeline partial to neutral
+        if constexpr (MULTI) {
+            // token t at position past_len + t: its q from accumulator row t, its k / v rows into row past_len + t of sequence seq
+            for (int i = tid; i < nseg * nr * TILE; i += DS_CONSUMERS) {
+                const int d = i & 127, w = i >> 7, sg = w / nr, j = w - sg * nr, t = j / a.n_rep;
+                const int qh = (h0 + sg) * a.n_rep + (j - t * a.n_rep);
+                const half* sr = a.sin + (size_t)(a.past_len + t) * TILE;
+                const half* cr = a.cos + (size_t)(a.past_len + t) * TILE;
+                const float* aq = a.acc_qkv + t * qkv_ld + (size_t)qh * TILE;
+                const half qv = __float2half_rn(__ldcg(aq + d)), qo = __float2half_rn(__ldcg(aq + (d ^ 64)));
+                const half sn = d < 64 ? __hneg(sr[d]) : sr[d];
+                gq[w * TILE + d] = __hfma(qv, cr[d], __hmul(qo, sn));
+            }
+            for (int i = tid; i < nseg * nt * TILE; i += DS_CONSUMERS) {
+                const int d = i & 127, w = i >> 7, sg = w / nt, t = w - sg * nt, kvh = h0 + sg;
+                if (!owner(kvh)) continue;
+                const int pos = a.past_len + t;
+                const half* sr = a.sin + (size_t)pos * TILE;
+                const half* cr = a.cos + (size_t)pos * TILE;
+                const half sn = d < 64 ? __hneg(sr[d]) : sr[d];
+                const float* ak = a.acc_qkv + t * qkv_ld + a.HQ + (size_t)kvh * TILE;
+                const half kv = __float2half_rn(__ldcg(ak + d)), ko = __float2half_rn(__ldcg(ak + (d ^ 64)));
+                const half kr = __hfma(kv, cr[d], __hmul(ko, sn));
+                const half vv = __float2half_rn(__ldcg(ak + a.HKV + d));
+                gkn[w * TILE + d] = __half2float(kr); gvn[w * TILE + d] = __half2float(vv);
+                const size_t off = (((size_t)a.seq * a.kv_heads + kvh) * a.max_seq + pos) * TILE + d;
+                L->kc[off] = kr; L->vc[off] = vv;
+            }
+        } else {
         for (int i = tid; i < nseg * nr * TILE; i += DS_CONSUMERS) {
             const int d = i & 127, w = i >> 7, sg = w / nr;
             int qh = (h0 + sg) * nr + (w - sg * nr);
@@ -970,6 +1015,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             gkn[sg * TILE + d] = __half2float(kr); gvn[sg * TILE + d] = __half2float(vv);
             const size_t off = ((size_t)kvh * a.max_seq + plen) * TILE + d;      // cache layout q4_attn.cu:32-51, kv_heads rows (per sequence)
             L->kc[off] = kr; L->vc[off] = vv;
+        }
         }
         for (int i = tid; i < nseg * nr * 4 * PART_LD; i += DS_CONSUMERS) {
             const int w = i / (4 * PART_LD), e = i - w * 4 * PART_LD;
@@ -1033,6 +1079,32 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             while (ch >= nph) { ch -= nph; kvh++; }
         }
         // the new token (KV heads whose last chunk this CTA holds): score q . k_new, weight 1 in its own partial, per query head
+        if constexpr (MULTI) {
+            // token t's causal tail: an online-softmax partial over the new rows 0 .. t of the launch (t == 0: exactly the single token's)
+            for (int w = warp; w < nseg * nr; w += DS_NCW) {
+                const int sg = w / nr, t = (w - sg * nr) / a.n_rep;
+                if (!owner(h0 + sg)) continue;
+                float m = -INFINITY, lsum = 0.f;
+                float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
+                for (int j = 0; j <= t; j++) {
+                    const float* kr = gkn + (sg * nt + j) * TILE + lane * 4;
+                    float d = 0.f;
+                    #pragma unroll
+                    for (int c = 0; c < 4; c++) d = fmaf(__half2float(gq[w * TILE + lane * 4 + c]) * scale, kr[c], d);
+                    #pragma unroll
+                    for (int off = 16; off > 0; off >>= 1) d += __shfl_xor_sync(0xffffffffu, d, off);
+                    const float mnew = fmaxf(m, d);
+                    const float alpha = __expf(m - mnew), pj = __expf(d - mnew);
+                    const float4 v = *reinterpret_cast<const float4*>(gvn + (sg * nt + j) * TILE + lane * 4);
+                    o.x = fmaf(pj, v.x, o.x * alpha); o.y = fmaf(pj, v.y, o.y * alpha); o.z = fmaf(pj, v.z, o.z * alpha); o.w = fmaf(pj, v.w, o.w * alpha);
+                    lsum = fmaf(lsum, alpha, pj);
+                    m = mnew;
+                }
+                float* pw = gparts + (w * 5 + 4) * PART_LD;
+                *reinterpret_cast<float4*>(pw + lane * 4) = o;
+                if (lane == 0) { pw[128] = m; pw[129] = lsum; }
+            }
+        } else {
         for (int w = warp; w < nseg * nr; w += DS_NCW) {
             const int sg = w / nr;
             if (!owner(h0 + sg)) continue;
@@ -1044,6 +1116,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             float* pw = gparts + (w * 5 + 4) * PART_LD;
             *reinterpret_cast<float4*>(pw + lane * 4) = *reinterpret_cast<const float4*>(gvn + sg * TILE + lane * 4);
             if (lane == 0) { pw[128] = d; pw[129] = 1.0f; }
+        }
         }
         consumer_sync();
         // this CTA's partial of every query head of its segments -> its slot of the head's CTA range
@@ -1060,7 +1133,9 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
                 Lt = fmaf(pp[k * PART_LD + 129], wgt, Lt);
                 ov = fmaf(pp[k * PART_LD + d], wgt, ov);
             }
-            float* dst = a.att_part + ((size_t)h * a.att_slots + (cta - (int)s_clo[h])) * PART_LD;
+            // MULTI: query vector j = t * n_rep + r of the segment is virtual query head t * heads + (KV head) * n_rep + r
+            const int hv = MULTI ? ((w - sg * nr) / a.n_rep) * a.heads + (h0 + sg) * a.n_rep + (w - sg * nr) % a.n_rep : h;
+            float* dst = a.att_part + ((size_t)hv * a.att_slots + (cta - (int)s_clo[hv])) * PART_LD;
             dst[d] = ov;
             if (d == 0) { dst[128] = M; dst[129] = Lt; }
         }
@@ -1094,7 +1169,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
 
         // ======================================================== ATT ========================================================
         {
-            const Phase p = phase_of(a, PH_ATT, G, nb);
+            const Phase p = step_phase<MULTI>(a, PH_ATT, G, nb);
             const int u0 = s_rng[PH_ATT][0], u1 = s_rng[PH_ATT][1];
             if (l > 0) zero_share(a.acc_d, ZR_H);
             const int nph = p.tpm;
@@ -1102,7 +1177,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             const int l16 = lane & 15, sub = lane >> 4;
             const int h0 = u1 > u0 ? u0 / nph : 0;
             const int nseg = u1 > u0 ? (u1 - 1) / nph - h0 + 1 : 0;            // <= 2 (heads <= grid, checked on the host)
-            if constexpr (GQA) att_gqa(L, u0, u1, nph, h0, nseg);
+            if constexpr (GQA || MULTI) att_gqa(L, u0, u1, nph, h0, nseg);
             else {
                 // every segment's q (and the new k / v rows where this CTA owns the head's last chunk): one L2 round trip
                 if (tid < nseg * TILE) {
@@ -1511,7 +1586,12 @@ struct exl_decode_plan
     int max_batch = 1;                          // sequences a step may carry (> 1: the BATCH kernels)
     LoraMat* d_lora = nullptr;                  // LoRA plans (the LORA kernels): [n_layers * 7] adapters
     long long lora_barriers = 0;                // their extra grid barriers per step
+    int max_tokens = 0;                         // multi-token plans (the MULTI kernel): tokens of one sequence a step may carry; else 0
+    int cache_seqs = 0;                         // multi-token plans: sequences the caches hold
 };
+
+// the one multi-token instantiation: batch GEMVs and head, the grouped-query attention path for any n_rep
+static const void* multi_kernel() { return (const void*)decode_step_kernel<false, false, true, true, false, true>; }
 
 static const void* step_kernel_for(bool act, bool tp, bool gqa, bool batch, bool lora = false)
 {
@@ -1544,11 +1624,25 @@ extern "C" int exl_decode_plan_create(const exl_decode_desc* d, exl_decode_plan*
     return exl_decode_plan_create_batch(d, 1, out);
 }
 
-static int plan_create(const exl_decode_desc* d, int max_batch, const exl_decode_lora* lora, exl_decode_plan** out);
+static int plan_create(const exl_decode_desc* d, int max_batch, const exl_decode_lora* lora, exl_decode_plan** out, int max_tokens = 0,
+                       int cache_seqs = 0);
 
 extern "C" int exl_decode_plan_create_batch(const exl_decode_desc* d, int max_batch, exl_decode_plan** out)
 {
     return plan_create(d, max_batch, nullptr, out);
+}
+
+extern "C" int exl_decode_plan_create_multi(const exl_decode_desc* d, int max_tokens, int cache_seqs, exl_decode_plan** out)
+{
+    if (!d || !out) return exl_set_err(EXL_ERR_ARG, "decode_plan_multi: NULL argument");
+    *out = nullptr;
+    if (max_tokens < 1 || max_tokens > MAX_BATCH)
+        return exl_set_err(EXL_ERR_ARG, "decode_plan_multi: max_tokens %d outside 1..%d: run longer chunks through prefill", max_tokens, MAX_BATCH);
+    if (d->tp_world > 1)
+        return exl_set_err(EXL_ERR_ARG, "decode_plan_multi: tensor parallelism (world %d) is not supported by the multi-token step: use exl_decode_step per token or prefill", d->tp_world);
+    if (cache_seqs < 1)
+        return exl_set_err(EXL_ERR_ARG, "decode_plan_multi: cache_seqs %d: the caches must hold at least 1 sequence", cache_seqs);
+    return plan_create(d, max_tokens, nullptr, out, max_tokens, cache_seqs);
 }
 
 extern "C" int exl_decode_plan_create_lora(const exl_decode_desc* d, int max_batch, const exl_decode_lora* lora, exl_decode_plan** out)
@@ -1578,8 +1672,10 @@ extern "C" int exl_decode_plan_create_lora(const exl_decode_desc* d, int max_bat
     return plan_create(d, max_batch, lora, out);
 }
 
-static int plan_create(const exl_decode_desc* d, int max_batch, const exl_decode_lora* lora, exl_decode_plan** out)
+static int plan_create(const exl_decode_desc* d, int max_batch, const exl_decode_lora* lora, exl_decode_plan** out, int max_tokens,
+                       int cache_seqs)
 {
+    const bool multi = max_tokens > 0;                 // max_batch == max_tokens then: accumulator rows and virtual heads per token
     if (!d || !out) return exl_set_err(EXL_ERR_ARG, "decode_plan: NULL argument");
     *out = nullptr;
     if (max_batch < 1 || max_batch > MAX_BATCH)
@@ -1636,7 +1732,9 @@ static int plan_create(const exl_decode_desc* d, int max_batch, const exl_decode
     a.act = any_act ? 1 : 0;
     if (any_act && d->tp_world > 1)
         return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: act-order matrices under tensor parallelism are not supported by the fused step (o_proj needs the all-gathered attention output): use the per-op path"));
-    if (max_batch > 1 && (any_act || d->tp_world > 1))
+    if (multi && any_act)
+        return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan_multi: act-order matrices are not supported by the multi-token step: use exl_decode_plan_create (one token per step) or prefill"));
+    if (max_batch > 1 && !multi && (any_act || d->tp_world > 1))
         return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: a batch (max_batch %d) with %s is not supported by the fused step: use max_batch 1 or the per-op path",
                                         max_batch, any_act ? "act-order matrices" : "tensor parallelism"));
     int dev_smem = 0;
@@ -1644,15 +1742,22 @@ static int plan_create(const exl_decode_desc* d, int max_batch, const exl_decode
     p->grid = ds->num_sms;
     if (const char* eg = getenv("EXL_DS_GRID")) { int v = atoi(eg); if (v >= 1 && v <= ds->num_sms) p->grid = v; }
     p->max_batch = max_batch;
+    p->max_tokens = max_tokens; p->cache_seqs = cache_seqs;
     a.bsz = 1;
-    if (max_batch > 1) {
+    if (multi) {
+        const int fits = max_tokens_for(H, HQ, I, d->num_heads, kv_heads, (size_t)dev_smem, p->grid);
+        if (max_tokens > fits)
+            return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan_multi: max_tokens %d does not fit this model on this GPU (shared memory for %d query vectors per KV head, or more KV heads than %d CTAs): the largest is %d",
+                                            max_tokens, max_tokens * a.n_rep, p->grid, fits));
+        a.xst = batch_xstages(H, HQ, HKV, I, p->grid);
+    } else if (max_batch > 1) {
         const int fits = max_batch_for(H, HQ, I, d->num_heads, kv_heads, false, (size_t)dev_smem, p->grid);
         if (max_batch > fits)
             return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: max_batch %d does not fit this model on this GPU (shared memory, or more virtual heads than %d CTAs): the largest batch is %d",
                                             max_batch, p->grid, fits));
         a.xst = batch_xstages(H, HQ, HKV, I, p->grid);
     }
-    const size_t fixed = smem_fixed_bytes(H, HQ, I, any_act, a.n_rep, max_batch, a.xst);
+    const size_t fixed = multi ? smem_fixed_bytes_multi(H, a.n_rep, max_tokens, a.xst) : smem_fixed_bytes(H, HQ, I, any_act, a.n_rep, max_batch, a.xst);
     int depth = ring_depth_for((size_t)dev_smem, fixed);
     if (const char* e = getenv("EXL_DS_DEPTH")) { int v = atoi(e); if (v >= 1 && v < depth) depth = v; }
     if (depth < 2) return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: model too wide for the shared-memory plan (%d ring stages per pipeline)", depth));
@@ -1660,13 +1765,13 @@ static int plan_create(const exl_decode_desc* d, int max_batch, const exl_decode
     a.depth = depth;
     p->smem = smem_dynamic_bytes(fixed, depth);
     if ((size_t)H * 2 > (size_t)a.spt_max * 256) return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: internal: head staging does not fit"));
-    const void* kfn = step_kernel_for(any_act, d->tp_world > 1, a.n_rep > 1, max_batch > 1, lora != nullptr);
+    const void* kfn = multi ? multi_kernel() : step_kernel_for(any_act, d->tp_world > 1, a.n_rep > 1, max_batch > 1, lora != nullptr);
     cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem);
     if (e != cudaSuccess) return plan_fail(p, exl_set_err(EXL_ERR_CUDA, "decode_plan: smem attribute (%zu B): %s", p->smem, cudaGetErrorString(e)));
     int per_sm = 0;
     e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kfn, DS_THREADS, p->smem);
     if (e != cudaSuccess || per_sm < 1) return plan_fail(p, exl_set_err(EXL_ERR_CUDA, "decode_plan: kernel does not fit an SM (smem %zu)", p->smem));
-    a.att_slots = att_slots_for(p->grid, d->num_heads, kv_heads);           // the most CTAs per head: one sequence
+    a.att_slots = multi ? att_slots_multi(p->grid, kv_heads) : att_slots_for(p->grid, d->num_heads, kv_heads);      // the most CTAs per head: one sequence
     // scratch: accumulators | attention partials | barrier (accumulators and partials: max_batch rows / virtual heads)
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
@@ -1784,9 +1889,41 @@ extern "C" int exl_decode_plan_trace(exl_decode_plan* p, unsigned long long* out
     return EXL_OK;
 }
 
+// the table reset (when `reset`) and the cooperative launch of kernel `kfn` with arguments `a`
+static int launch_step(exl_decode_plan* p, StepArgs& a, const void* kfn, bool reset, void* stream_)
+{
+    if (reset) {
+        // short context: some CTAs inside a head's CTA range own no attention unit in this launch (stateless test, so a captured
+        // CUDA graph -- past_len is baked into it -- replays the same decision)
+        const int n = a.bsz * a.heads * a.att_slots * PART_LD;
+        att_part_reset_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream_>>>(a.att_part, n);
+        g_launches.fetch_add(1, std::memory_order_relaxed);
+        cudaError_t er = cudaGetLastError();
+        if (er != cudaSuccess) return exl_set_err(EXL_ERR_CUDA, "launch of att_part_reset_kernel failed: %s", cudaGetErrorString(er));
+    }
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;      // all CTAs co-resident: the grid barrier relies on it
+    cfg.gridDim = dim3((unsigned)p->grid); cfg.blockDim = dim3(DS_THREADS); cfg.dynamicSmemBytes = p->smem; cfg.stream = (cudaStream_t)stream_;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    void* kargs[1] = {(void*)&a};
+    cudaError_t e = cudaLaunchKernelExC(&cfg, kfn, kargs);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    if (e != cudaSuccess) return exl_set_err(EXL_ERR_CUDA, "launch of decode_step_kernel failed: %s (grid %d, smem %zu)", cudaGetErrorString(e), p->grid, p->smem);
+    return EXL_OK;
+}
+
+static int reject_multi_plan(const exl_decode_plan* p)
+{
+    return exl_set_err(EXL_ERR_ARG, "decode_step: this plan carries up to %d tokens of one sequence per step: call exl_decode_step_multi "
+                                    "(or create the plan with exl_decode_plan_create / exl_decode_plan_create_batch)", p->max_tokens);
+}
+
 extern "C" int exl_decode_step(exl_decode_plan* p, const void* x_in, int past_len, void* x_out, void* logits, void* stream_)
 {
     if (!p) return exl_set_err(EXL_ERR_STATE, "decode_step: NULL plan");
+    if (p->max_tokens) return reject_multi_plan(p);
     if (past_len < 0 || past_len >= p->args.max_seq) return exl_set_err(EXL_ERR_ARG, "decode_step: past_len %d outside the cache (max_seq %d)", past_len, p->args.max_seq);
     return exl_decode_step_batch(p, x_in, 1, &past_len, x_out, logits, stream_);
 }
@@ -1794,6 +1931,7 @@ extern "C" int exl_decode_step(exl_decode_plan* p, const void* x_in, int past_le
 extern "C" int exl_decode_step_batch(exl_decode_plan* p, const void* x_in, int bsz, const int* past_len_host, void* x_out, void* logits, void* stream_)
 {
     if (!p) return exl_set_err(EXL_ERR_STATE, "decode_step: NULL plan");
+    if (p->max_tokens) return reject_multi_plan(p);
     if (!x_in) return exl_set_err(EXL_ERR_ARG, "decode_step: x_in is NULL");
     if (bsz < 1 || bsz > p->max_batch)
         return exl_set_err(EXL_ERR_ARG, "decode_step: bsz %d outside 1..%d (the plan's max_batch): create the plan with exl_decode_plan_create_batch for a larger batch", bsz, p->max_batch);
@@ -1811,24 +1949,28 @@ extern "C" int exl_decode_step_batch(exl_decode_plan* p, const void* x_in, int b
     a.x_in = (const half*)x_in; a.x_out = (half*)x_out; a.logits = (float*)logits; a.past_len = longest;
     a.bsz = bsz;
     for (int b = 0; b < bsz; b++) a.past_lens[b] = past_len_host[b];
-    if (att_needs_reset(a.heads, a.kv_heads, longest, p->grid, bsz)) {
-        // short context: some CTAs inside a head's CTA range own no attention unit in this launch (stateless test, so a captured
-        // CUDA graph -- past_len is baked into it -- replays the same decision)
-        const int n = bsz * a.heads * a.att_slots * PART_LD;
-        att_part_reset_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream_>>>(a.att_part, n);
-        g_launches.fetch_add(1, std::memory_order_relaxed);
-        cudaError_t er = cudaGetLastError();
-        if (er != cudaSuccess) return exl_set_err(EXL_ERR_CUDA, "launch of att_part_reset_kernel failed: %s", cudaGetErrorString(er));
-    }
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeCooperative; at[0].val.cooperative = 1;      // all CTAs co-resident: the grid barrier relies on it
-    cfg.gridDim = dim3((unsigned)p->grid); cfg.blockDim = dim3(DS_THREADS); cfg.dynamicSmemBytes = p->smem; cfg.stream = (cudaStream_t)stream_;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    void* kargs[1] = {(void*)&a};
-    cudaError_t e = cudaLaunchKernelExC(&cfg, step_kernel_for(a.act != 0, a.tp_world > 1, a.n_rep > 1, p->max_batch > 1, a.lora != nullptr), kargs);
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    if (e != cudaSuccess) return exl_set_err(EXL_ERR_CUDA, "launch of decode_step_kernel failed: %s (grid %d, smem %zu)", cudaGetErrorString(e), p->grid, p->smem);
-    return EXL_OK;
+    return launch_step(p, a, step_kernel_for(a.act != 0, a.tp_world > 1, a.n_rep > 1, p->max_batch > 1, a.lora != nullptr),
+                       att_needs_reset(a.heads, a.kv_heads, longest, p->grid, bsz), stream_);
+}
+
+extern "C" int exl_decode_step_multi(exl_decode_plan* p, const void* x_in, int n, int seq, int past_len, void* x_out, void* logits, void* stream_)
+{
+    if (!p) return exl_set_err(EXL_ERR_STATE, "decode_step_multi: NULL plan");
+    if (!p->max_tokens)
+        return exl_set_err(EXL_ERR_ARG, "decode_step_multi: the plan is not a multi-token plan: create it with exl_decode_plan_create_multi, "
+                                        "or step it with exl_decode_step / exl_decode_step_batch");
+    if (!x_in) return exl_set_err(EXL_ERR_ARG, "decode_step_multi: x_in is NULL");
+    if (n < 1 || n > p->max_tokens)
+        return exl_set_err(EXL_ERR_ARG, "decode_step_multi: n %d outside 1..%d (the plan's max_tokens): split the chunk, or create the plan with a larger max_tokens", n, p->max_tokens);
+    if (seq < 0 || seq >= p->cache_seqs)
+        return exl_set_err(EXL_ERR_ARG, "decode_step_multi: seq %d outside the caches' sequences [0, %d)", seq, p->cache_seqs);
+    if (past_len < 0 || past_len + n > p->args.max_seq)
+        return exl_set_err(EXL_ERR_ARG, "decode_step_multi: past_len %d + n %d outside the cache (max_seq %d): rows [%d, %d) must fit", past_len, n, p->args.max_seq, past_len, past_len + n);
+    if (p->args.lm_head && !logits) return exl_set_err(EXL_ERR_ARG, "decode_step_multi: the plan has an lm_head, logits must be given");
+    DeviceGuard guard(p->device);
+    StepArgs a = p->args;
+    a.x_in = (const half*)x_in; a.x_out = (half*)x_out; a.logits = (float*)logits; a.past_len = past_len;
+    a.bsz = n; a.seq = seq;
+    for (int b = 0; b < n; b++) a.past_lens[b] = past_len;
+    return launch_step(p, a, multi_kernel(), att_needs_reset_multi(a.heads, a.kv_heads, past_len, p->grid), stream_);
 }

@@ -101,6 +101,29 @@ DS_HD int stage_area_bytes(int xstages, int n_rep)
     const int b = xstages * (256 + 32), g = gqa_scratch_bytes(n_rep);
     return b > g ? b : ((g + 31) & ~31);
 }
+// Multi-token plans (ntok consecutive tokens of one sequence) run the grouped-query attention path for any n_rep: a KV head's stage
+// serves its n_rep * ntok query vectors (token t, query head r of the group at t * n_rep + r), and the segment keeps the ntok new k
+// and v rows in fp32 ([2][ntok][128] each) -- the launch's own tokens are the causal tail of every query vector.
+DS_HD int gqa_scratch_bytes_multi(int n_rep, int ntok) { return gqa_kn_off(n_rep * ntok) + 2 * 2 * ntok * TILE * 4; }
+DS_HD int stage_area_bytes_multi(int xstages, int n_rep, int ntok)
+{
+    const int b = xstages * (256 + 32), g = gqa_scratch_bytes_multi(n_rep, ntok);
+    return b > g ? b : ((g + 31) & ~31);
+}
+// The multi-token ATT phase: (KV head, 16-position chunk) units over the kv_heads real KV heads at the shared context past_len (the
+// history every token of the launch attends), and the grouped-query cap on CTAs per KV head -- a unit does the math of n_rep * ntok
+// query vectors.  Every other phase is phase_of's (the GEMV phases do not depend on the token count; HEAD neither).
+template <class A>
+DS_HD Phase phase_of_multi(const A& a, int kind, int grid)
+{
+    Phase p = phase_of(a, kind, grid);
+    if (kind == PH_ATT) {
+        p.G = grid;
+        const int kvh = kv_heads_of(a);
+        if (kvh * ATT_CTAS_PER_KV_HEAD < grid) p.G = kvh * ATT_CTAS_PER_KV_HEAD;
+    }
+    return p;
+}
 
 // ---- host side (exl_decode_plan_create / exl_decode_step) ----
 // Short contexts: with fewer attention units than participating CTAs (U < G) some CTAs between the first and the last CTA of a
@@ -181,6 +204,46 @@ static inline int max_batch_for(int H, int HQ, int I, int heads, int kv_heads, b
         if (b * (n_rep > 1 ? kv_heads : heads) > grid || b * heads > DS_MAX_HEADS) break;
         if (ring_depth_for(dev_smem, smem_fixed_bytes(H, HQ, I, act, n_rep, b, xst)) < 2) break;
         best = b;
+    }
+    return best;
+}
+
+// ---- multi-token plans (exl_decode_plan_create_multi / exl_decode_step_multi): 1 .. max_tokens consecutive tokens of ONE sequence ----
+// The GEMV, norm and head phases are the batch's with nb = n tokens; ATT is phase_of_multi's.  Its slot table, reset predicate and
+// shared memory follow.  tests/decode_sched_check_multi.cpp proves them for every token count and context.
+// Exact: with fewer units than CTAs every CTA holds at most one unit, so a KV head's range has an idle CTA exactly when it spans more
+// CTAs than the head has units (the plain U < G test also fires at contexts where every range happens to be dense).
+static inline bool att_needs_reset_multi(int heads, int kv_heads, int past_len, int grid)
+{
+    AttDims a = {};
+    a.heads = heads; a.kv_heads = kv_heads; a.past_len = past_len;
+    const Phase p = phase_of_multi(a, PH_ATT, grid);
+    if (p.U >= p.G || p.tpm < 2) return false;
+    for (int kvh = 0; kvh < kv_heads; kvh++)
+        if (cta_of((long long)(kvh + 1) * p.tpm - 1, p.U, p.G) - cta_of((long long)kvh * p.tpm, p.U, p.G) + 1 > p.tpm) return true;
+    return false;
+}
+// slots of att_part per virtual query head (token t, head h): one per CTA that can hold a piece of its KV head, + 2
+static inline int att_slots_multi(int grid, int kv_heads)
+{
+    return (grid < ATT_CTAS_PER_KV_HEAD * kv_heads ? grid / kv_heads : ATT_CTAS_PER_KV_HEAD) + 2;
+}
+// as smem_fixed_bytes for a batch of max_tokens, with the multi-token attention scratch sharing the staging area
+static inline size_t smem_fixed_bytes_multi(int H, int n_rep, int max_tokens, int xstages)
+{
+    const size_t tail = (size_t)(2 * 17 * PART_LD + 6 * TILE) * 4 + (size_t)2 * TILE * 2 /* fp16 q */ + (size_t)H * 2 /* wnorm */ + SMEM_STATIC_ALLOWANCE;
+    return 1024 + (size_t)stage_area_bytes_multi(max_tokens * xstages, n_rep, max_tokens) + (size_t)max_tokens * H * 2 + tail;
+}
+// The most tokens (<= MAX_BATCH) a multi-token plan can take: >= 2 ring stages per pipeline, every KV head a CTA of its own (at most 2
+// head segments per CTA), and max_tokens * heads virtual query heads in the CTA-range table.  0: not even one fits.
+static inline int max_tokens_for(int H, int HQ, int I, int heads, int kv_heads, size_t dev_smem, int grid)
+{
+    const int xst = batch_xstages(H, HQ, kv_heads * TILE, I, grid);
+    int best = 0;
+    for (int k = 1; k <= MAX_BATCH; k++) {
+        if (kv_heads > grid || k * heads > DS_MAX_HEADS) break;
+        if (ring_depth_for(dev_smem, smem_fixed_bytes_multi(H, heads / kv_heads, k, xst)) < 2) break;
+        best = k;
     }
     return best;
 }

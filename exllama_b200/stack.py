@@ -286,16 +286,24 @@ class DecodeStack:
         return torch.matmul(hn.view(-1, s.hidden), self.lm_head.t()).float()
 
     # ---- decode: the whole token as ONE persistent kernel (csrc/decode_step.cu; SURVEY.md 8f-4 / 8f-2) -------------------
-    def make_plan(self, with_head=True):
-        """Build the exl_decode_plan over this stack's handles, norms, caches and tables (borrowed)."""
+    def make_plan(self, with_head=True, max_tokens=None):
+        """Build the exl_decode_plan over this stack's handles, norms, caches and tables (borrowed).  max_tokens (1..4): a
+        multi-token plan instead, for decode_step_fused_multi (up to max_tokens consecutive tokens of one cache sequence per launch)."""
         from . import capi
         hs = [[L.q.q4, L.k.q4, L.v.q4, L.o.q4, L.gate.q4, L.up.q4, L.down.q4] for L in self.layers]
         head = self.lm_head if with_head else None
+        multi = max_tokens is not None
+        if multi and self.lora is not None:
+            raise NotImplementedError("LoRA adapters in the multi-token step are not implemented: use prefill")
         self.dplan = capi.DecodePlan(hs, [L.ln1 for L in self.layers], [L.ln2 for L in self.layers], self.key_cache, self.value_cache,
                                     self.sin, self.cos, self.local_heads, self.shape.head_dim, self.max_seq, self.shape.eps,
                                     final_norm=self.norm if head is not None else None, lm_head=head,
-                                    tp_rank=self.tp_rank, tp_world=self.tp_size, num_kv_heads=self.local_kv_heads, max_batch=self.batch,
-                                    lora=self._plan_lora())
+                                    tp_rank=self.tp_rank, tp_world=self.tp_size, num_kv_heads=self.local_kv_heads,
+                                    max_batch=1 if multi else self.batch, lora=None if multi else self._plan_lora(), max_tokens=max_tokens)
+        if multi:
+            self._plan_xout = torch.empty((max_tokens, self.shape.hidden), dtype=torch.float16, device=self.device)
+            self._plan_logits = torch.empty((max_tokens, self.shape.vocab), dtype=torch.float32, device=self.device) if head is not None else None
+            return self.dplan
         if self.tp_size > 1:
             # exchange the cudaIpc handles of the regions the peers reduce into (acc_o, acc_d, cross-barrier counter)
             import torch.distributed as dist
@@ -329,6 +337,17 @@ class DecodeStack:
         lg = self._plan_logits
         self.dplan.step_batch(hidden, past_lens, x_out=xo, logits=lg)
         return lg[:bsz] if lg is not None else xo[:bsz]
+
+    def decode_step_fused_multi(self, hidden, past_len, seq=0):
+        """n <= max_tokens consecutive tokens of cache sequence seq in one launch (a plan from make_plan(max_tokens=...)): hidden
+        [n, 1, hidden] fp16 (read only), token t at position past_len + t attending rows [0, past_len) and tokens 0..t of the
+        launch -- what prefill(hidden.view(1, n, -1), past_len, seq=seq, last_only=False) computes.  Returns logits [n, vocab] fp32
+        (or the final hidden states without a head); the final pre-norm hidden states are left in self._plan_xout[:n]."""
+        n = hidden.shape[0]
+        assert hidden.numel() == n * self.shape.hidden and hidden.is_contiguous(), hidden.shape
+        lg = self._plan_logits
+        self.dplan.step_multi(hidden, past_len, seq=seq, x_out=self._plan_xout, logits=lg)
+        return lg[:n] if lg is not None else self._plan_xout[:n]
 
     def _o_input(self, attn_local):
         """o_proj input of this rank: its own heads' output, or -- act-order + TP -- the rows of its group range out of the

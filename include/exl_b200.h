@@ -299,6 +299,22 @@ int exl_decode_step(exl_decode_plan* plan, const void* x_in, int past_len, void*
 int exl_decode_step_batch(exl_decode_plan* plan, const void* x_in, int bsz, const int* past_len_host, void* x_out, void* logits,
                           void* stream);
 
+/* Multi-token steps: a plan whose launches carry 1 .. max_tokens (<= 4) consecutive tokens of ONE sequence -- a speculative draft
+   to verify, or a short chunk such as a follow-up turn's first tokens -- in one pass over the weights; the history's K/V rows are
+   read once for all of them.  The caches are [cache_seqs, num_kv_heads, max_seq_len, head_dim].  EXL_ERR_ARG for max_tokens outside
+   1..4 or more than fit this model (the message names the largest that fits), act-order matrices, tp_world > 1, cache_seqs < 1.
+   A multi-token plan is stepped by exl_decode_step_multi only; exl_decode_step / exl_decode_step_batch reject it. */
+int exl_decode_plan_create_multi(const exl_decode_desc* desc, int max_tokens, int cache_seqs, exl_decode_plan** out_plan);
+/* n (1 .. max_tokens) tokens x_in half [n][hidden] of cache sequence seq: token t sits at position past_len + t, attends cache rows
+   [0, past_len) and the launch's own tokens 0 .. t, and writes row past_len + t; no other row is written, and no row at or past
+   past_len is read (a speculative caller that accepts a < n tokens starts its next step at past_len + a + 1 over the stale rows).
+   x_out (optional) half [n][hidden] receives the final hidden states before the final norm, logits float [n][vocab] every row
+   (required iff the plan has an lm_head).  n, seq and past_len are read on the host (baked into a CUDA-graph capture).
+   EXL_ERR_ARG for n outside 1..max_tokens, seq outside [0, cache_seqs), past_len < 0 or past_len + n > max_seq_len, a NULL x_in, a
+   NULL logits with a head, and a plan not made by exl_decode_plan_create_multi. */
+int exl_decode_step_multi(exl_decode_plan* plan, const void* x_in, int n, int seq, int past_len, void* x_out, void* logits,
+                          void* stream);
+
 /* --- tensor-parallel variants (new functionality; the reference has no tensor parallelism, SURVEY.md 8e) ----- */
 
 /* As exl_q4_attn_2 / exl_q4_mlp, but with add_residual == 0 the row-parallel projection OVERWRITES x with this rank's

@@ -74,6 +74,7 @@ SIGNATURES = {
     "exl_rep_penalty": (i32, [i32, vp, vp, f32, i32, i32, i32]),
     "exl_apply_rep_penalty": (i32, [i32, vp, f32, i32, i32, i32, vp]),
     "exl_sample": (i32, [vp, i32, i32, i64, vp, i64, C.POINTER(i32), C.POINTER(ExlSampleParams), vp, vp, vp, vp, vp]),
+    "exl_spec_verify": (i32, [vp, i32, i32, i64, vp, vp, i64, vp, i32, C.POINTER(ExlSampleParams), vp, vp, vp, vp, vp, vp]),
     "exl_q4_matmul_host": (i32, [vp, i32, vp, vp, vp, vp, vp]),
     "exl_decode_plan_create": (i32, [vp, C.POINTER(vp)]),
     "exl_decode_plan_create_batch": (i32, [vp, i32, C.POINTER(vp)]),

@@ -76,8 +76,9 @@ int exl_own_scratch(ExlDevice* ds, int role, int64_t numel, half** out)
 extern "C" {
 
 const char* exl_last_error(void) { return t_err; }
-int exl_version(void) { return 106; }             // 101: exl_decode_desc.num_kv_heads; 102: batched decode plans and steps; 103: LoRA plans;
-                                                  // 104: exl_prefill_attn; 105: exl_prefill_attn_ragged, exl_rope_cache_ragged; 106: exl_sample
+int exl_version(void) { return 107; }             // 101: exl_decode_desc.num_kv_heads; 102: batched decode plans and steps; 103: LoRA plans;
+                                                  // 104: exl_prefill_attn; 105: exl_prefill_attn_ragged, exl_rope_cache_ragged; 106: exl_sample;
+                                                  // 107: exl_spec_verify
 int64_t exl_launch_count(void) { return g_launches.load(); }
 const char* exl_last_q4_path(void) { return g_last_q4_path; }
 
@@ -623,6 +624,14 @@ int exl_sample(const float* logits, int bsz, int vocab, int64_t logits_ld, const
 {
     return exl_sample_launch(logits, bsz, vocab, logits_ld, history, hist_ld, hist_len_host, p, u, tokens, probs, dist,
                              (cudaStream_t)stream);
+}
+
+int exl_spec_verify(const float* target_logits, int k, int vocab, int64_t logits_ld, const int64_t* draft_tokens,
+                    const float* draft_dist, int64_t dist_ld, const int64_t* history, int hist_len_host, const exl_sample_params* p,
+                    const float* u, float* work, int* n_accepted, int64_t* tokens, float* probs, void* stream)
+{
+    return exl_spec_verify_launch(target_logits, k, vocab, logits_ld, draft_tokens, draft_dist, dist_ld, history, hist_len_host, p, u,
+                                  work, n_accepted, tokens, probs, (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------

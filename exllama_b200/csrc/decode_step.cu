@@ -1766,7 +1766,12 @@ static int plan_create(const exl_decode_desc* d, int max_batch, const exl_decode
     p->smem = smem_dynamic_bytes(fixed, depth);
     if ((size_t)H * 2 > (size_t)a.spt_max * 256) return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: internal: head staging does not fit"));
     const void* kfn = multi ? multi_kernel() : step_kernel_for(any_act, d->tp_world > 1, a.n_rep > 1, max_batch > 1, lora != nullptr);
-    cudaError_t e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem);
+    // the attribute belongs to the kernel, not the plan: it only grows, so that plans of one kernel with different shared memory
+    // (a speculative target and its draft) can be stepped in any order
+    cudaFuncAttributes fa{};
+    cudaError_t e = cudaFuncGetAttributes(&fa, kfn);
+    if (e == cudaSuccess && (size_t)fa.maxDynamicSharedSizeBytes < p->smem)
+        e = cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem);
     if (e != cudaSuccess) return plan_fail(p, exl_set_err(EXL_ERR_CUDA, "decode_plan: smem attribute (%zu B): %s", p->smem, cudaGetErrorString(e)));
     int per_sm = 0;
     e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kfn, DS_THREADS, p->smem);

@@ -169,9 +169,14 @@ int exl_prefill_attn_ragged_launch(const half* q, const half* kc, const half* vc
 int exl_ragged_validate(const exl_ragged* r, int num_cache_seqs, int max_seq, const char* who);
 
 // sample.cu
+// tail (with a history): every row reads history row 0, and row b's history is its hist_len[0] tokens followed by tail[0 .. b)
 int exl_sample_launch(const float* logits, int bsz, int vocab, int64_t logits_ld, const int64_t* history, int64_t hist_ld,
                       const int* hist_len, const exl_sample_params* p, const float* u, int64_t* tokens, float* probs, float* dist,
-                      cudaStream_t stream);
+                      cudaStream_t stream, const int64_t* tail = nullptr);
+int exl_spec_verify_launch(const float* target_logits, int k, int vocab, int64_t logits_ld, const int64_t* draft_tokens,
+                           const float* draft_dist, int64_t dist_ld, const int64_t* history, int hist_len,
+                           const exl_sample_params* p, const float* u, float* work, int* n_accepted, int64_t* tokens, float* probs,
+                           cudaStream_t stream);
 
 // half_matmul.cu
 int exl_half_matmul_cublas_launch(ExlDevice* ds, const half* x, const half* w, half* out, int M, int K, int N, bool no_zero, cudaStream_t stream);

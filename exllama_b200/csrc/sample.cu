@@ -42,6 +42,7 @@ static_assert(2 * SP_BINS == 4 * SP_THREADS, "each thread scans two bins");
 struct SampleArgs {
     const float* logits; int64_t ld; int vocab; int slice;
     const int64_t* hist; int64_t hist_ld; int hist_len[EXL_RAGGED_MAX_SEQ];
+    const int64_t* tail; int tail_at;            // history positions >= tail_at read tail[pos - tail_at] (tail NULL: none)
     float temperature; int top_k; float top_p, min_p, typical;
     float pmax; int sustain, decay, bos;
     const int* banned; int n_banned;
@@ -291,7 +292,8 @@ __global__ void __cluster_dims__(SP_CL, 1, 1) __launch_bounds__(SP_THREADS, 1) s
         __syncthreads();
         const int64_t* h = a.hist + (int64_t)row * a.hist_ld;
         for (long long j = threadIdx.x; j < W; j += SP_THREADS) {
-            const int64_t t = h[len - 1 - j];
+            const long long pos = len - 1 - j;
+            const int64_t t = a.tail && pos >= a.tail_at ? a.tail[pos - a.tail_at] : h[pos];
             if (t < 0 || t >= a.vocab) { bad = 1; continue; }
             if (t >= lo && t < lo + n) atomicMin(&s_int[t - lo], (int)j);
         }
@@ -463,13 +465,107 @@ __global__ void __cluster_dims__(SP_CL, 1, 1) __launch_bounds__(SP_THREADS, 1) s
     cluster.sync();                                                  // keep this CTA's exchange slot alive until every CTA has read it
 }
 
+// ---- speculative verification (exl_spec_verify): the acceptance walk and the residual draw --------------------------------------
+constexpr int SV_THREADS = 512;
+
+struct VerifyArgs {
+    const float* p;              // [k + 1][vocab]: sample_kernel's final distributions of the target rows
+    const float* q; int64_t q_ld;
+    const int64_t* drafts; const float* u;
+    int k, vocab;
+    int* n_acc; int64_t* tokens; float* probs;    // tokens / probs hold sample_kernel's draws of the target rows on entry
+};
+
+// One CTA.  Thread 0 walks the drafts (u_{j-1} q_j(d_j) < p_{j-1}(d_j) accepts d_j); after a rejection the block draws the
+// correction from max(0, p_{j-1} - q_j) -- from p_{j-1} if rounding left that empty -- with u_k: thread t owns the contiguous
+// run [t * per, (t + 1) * per) of the vocabulary, masses in the sampler's 2^-60 fixed point, integer scans only.
+__global__ void __launch_bounds__(SV_THREADS, 1) spec_residual_kernel(const __grid_constant__ VerifyArgs a)
+{
+    __shared__ int s_acc, s_state, s_pick;
+    __shared__ int64_t s_bonus; __shared__ float s_bonus_p;
+    __shared__ unsigned long long s_m[SV_THREADS / 32];
+    __shared__ int s_l[SV_THREADS / 32];
+    if (threadIdx.x == 0) {
+        int n = 0, state = 0;                                        // 0: all accepted, 1: d_{n+1} rejected, -1: undefined
+        for (; n < a.k; n++) {
+            if (a.tokens[n] < 0) { state = -1; break; }              // p_n undefined
+            const int64_t d = a.drafts[n];
+            if (d < 0 || d >= a.vocab) { state = -1; break; }
+            const float qd = a.q[(int64_t)n * a.q_ld + d];
+            if (!(qd > 0.0f) || !isfinite(qd)) { state = -1; break; }
+            if (!(__fmul_rn(a.u[n], qd) < a.p[(int64_t)n * a.vocab + d])) { state = 1; break; }
+        }
+        if (state == 0 && a.tokens[a.k] < 0) state = -1;
+        s_acc = n; s_state = state; s_pick = -1;
+        s_bonus = a.tokens[a.k]; s_bonus_p = a.probs[a.k];
+    }
+    __syncthreads();
+    const int n = s_acc;
+    int state = s_state;
+    if (state == 1) {
+        const float* p = a.p + (int64_t)n * a.vocab;
+        const float* q = a.q + (int64_t)n * a.q_ld;
+        const int per = (a.vocab + SV_THREADS - 1) / SV_THREADS;
+        const int i0 = min(a.vocab, (int)threadIdx.x * per), i1 = min(a.vocab, i0 + per);
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+        for (int resid = 1; resid >= 0; resid--) {                   // the same decision in every thread: total is block-wide
+            auto mass = [&](int i) { return fix60(resid ? fmaxf(p[i] - q[i], 0.0f) : p[i]); };
+            unsigned long long mine = 0;
+            int last = -1;
+            for (int i = i0; i < i1; i++) { const unsigned long long m = mass(i); mine += m; if (m) last = i; }
+            unsigned long long incl = mine;
+            for (int o = 1; o < 32; o <<= 1) { const unsigned long long v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
+            int lk = last;
+            for (int o = 16; o; o >>= 1) lk = max(lk, __shfl_xor_sync(0xffffffffu, lk, o));
+            __syncthreads();
+            if (lane == 31) s_m[warp] = incl;
+            if (lane == 0) s_l[warp] = lk;
+            __syncthreads();
+            unsigned long long base = incl - mine, total = 0;
+            int row_last = -1;
+            for (int w = 0; w < SV_THREADS / 32; w++) {
+                if (w < warp) base += s_m[w];
+                total += s_m[w];
+                row_last = max(row_last, s_l[w]);
+            }
+            if (total == 0) continue;                                // only rounding empties the residual: draw from p_n
+            const unsigned long long U = (unsigned long long)((double)a.u[a.k] * (double)total);
+            if (U >= total) {                                        // rounding left u at or above the total: the largest id with mass
+                if (threadIdx.x == 0) s_pick = row_last;
+            } else if (base <= U && U < base + mine) {
+                unsigned long long cum = base;
+                for (int i = i0; i < i1; i++) {
+                    cum += mass(i);
+                    if (cum > U) { s_pick = i; break; }
+                }
+            }
+            break;
+        }
+        __syncthreads();
+        if (s_pick < 0) state = -1;                                  // no mass at all: a defined p row always has some
+    }
+    if (threadIdx.x == 0) {
+        const int emitted = state < 0 ? 0 : n + 1;                   // tokens written before the -1 tail
+        for (int j = 0; j <= a.k; j++) {
+            int64_t t = -1; float pr = NAN;
+            if (j < emitted) {
+                if (j < n) t = a.drafts[j];
+                else t = state == 0 ? s_bonus : (int64_t)s_pick;
+                pr = j < n || state == 1 ? a.p[(int64_t)j * a.vocab + t] : s_bonus_p;
+            }
+            a.tokens[j] = t; a.probs[j] = pr;
+        }
+        *a.n_acc = state < 0 ? -1 : n;
+    }
+}
+
 bool g_sample_attr[EXL_MAX_DEVICES];
 
 } // namespace
 
 int exl_sample_launch(const float* logits, int bsz, int vocab, int64_t logits_ld, const int64_t* history, int64_t hist_ld,
                       const int* hist_len, const exl_sample_params* p, const float* u, int64_t* tokens, float* probs, float* dist,
-                      cudaStream_t stream)
+                      cudaStream_t stream, const int64_t* tail)
 {
     if (!p) return exl_set_err(EXL_ERR_ARG, "sample: params is NULL");
     if (!logits || !u || !tokens || !probs)
@@ -491,13 +587,14 @@ int exl_sample_launch(const float* logits, int bsz, int vocab, int64_t logits_ld
     SampleArgs a{};
     if (history) {
         if (!hist_len) return exl_set_err(EXL_ERR_ARG, "sample: history without hist_len_host");
-        for (int b = 0; b < bsz; b++)
+        for (int b = 0; b < (tail ? 1 : bsz); b++)
             if (hist_len[b] < 0 || hist_len[b] > hist_ld)
                 return exl_set_err(EXL_ERR_ARG, "sample: hist_len[%d] %d outside [0, hist_ld %lld]", b, hist_len[b], (long long)hist_ld);
-        for (int b = 0; b < bsz; b++) a.hist_len[b] = hist_len[b];
+        for (int b = 0; b < bsz; b++) a.hist_len[b] = tail ? hist_len[0] + b : hist_len[b];
+        if (tail) { a.tail = tail; a.tail_at = hist_len[0]; }
     }
     a.logits = logits; a.ld = logits_ld; a.vocab = vocab; a.slice = (vocab + SP_CL - 1) / SP_CL;
-    a.hist = history; a.hist_ld = hist_ld;
+    a.hist = history; a.hist_ld = tail ? 0 : hist_ld;
     a.temperature = p->temperature; a.top_k = p->top_k; a.top_p = p->top_p; a.min_p = p->min_p; a.typical = p->typical;
     a.pmax = p->rep_penalty_max; a.sustain = p->rep_sustain; a.decay = p->rep_decay; a.bos = p->bos_token_id;
     a.banned = p->banned; a.n_banned = p->n_banned;
@@ -513,5 +610,27 @@ int exl_sample_launch(const float* logits, int bsz, int vocab, int64_t logits_ld
     const size_t smem = (size_t)a.slice * sizeof(float);
     sample_kernel<<<dim3(SP_CL, bsz), SP_THREADS, smem, stream>>>(a);
     EXL_CHECK_LAUNCH("sample_kernel");
+    return EXL_OK;
+}
+
+int exl_spec_verify_launch(const float* target_logits, int k, int vocab, int64_t logits_ld, const int64_t* draft_tokens,
+                           const float* draft_dist, int64_t dist_ld, const int64_t* history, int hist_len,
+                           const exl_sample_params* p, const float* u, float* work, int* n_accepted, int64_t* tokens, float* probs,
+                           cudaStream_t stream)
+{
+    if (k < 1 || k > EXL_RAGGED_MAX_SEQ - 1) return exl_set_err(EXL_ERR_ARG, "spec_verify: k %d outside [1, %d]", k, EXL_RAGGED_MAX_SEQ - 1);
+    if (dist_ld < vocab) return exl_set_err(EXL_ERR_ARG, "spec_verify: dist_ld %lld < vocab %d", (long long)dist_ld, vocab);
+    if (!draft_tokens || !draft_dist || !u || !work || !n_accepted || !tokens || !probs)
+        return exl_set_err(EXL_ERR_ARG, "spec_verify: NULL pointer (draft_tokens %p, draft_dist %p, u %p, work %p, n_accepted %p, "
+                           "tokens %p, probs %p)", (const void*)draft_tokens, (const void*)draft_dist, (const void*)u, (void*)work,
+                           (void*)n_accepted, (void*)tokens, (void*)probs);
+    // p_0 .. p_k: every target row through the sampler, row j's history followed by d_1 .. d_j; each row's draw with u_j lands in
+    // tokens[j] / probs[j] (row k's is the bonus token), and -1 there marks an undefined row
+    const int rc = exl_sample_launch(target_logits, k + 1, vocab, logits_ld, history, hist_len, history ? &hist_len : nullptr, p, u,
+                                     tokens, probs, work, stream, draft_tokens);
+    if (rc != EXL_OK) return rc;
+    VerifyArgs a{work, draft_dist, dist_ld, draft_tokens, u, k, vocab, n_accepted, tokens, probs};
+    spec_residual_kernel<<<1, SV_THREADS, 0, stream>>>(a);
+    EXL_CHECK_LAUNCH("spec_residual_kernel");
     return EXL_OK;
 }

@@ -29,6 +29,26 @@ class Settings:
     token_repetition_penalty_decay = 128
 
 
+def params(settings: Settings, dev, bos_token_id=None, banned=None):
+    """(exl_sample_params of settings, the banned ids as an int32 device tensor or None -- keep it alive until the call is made)."""
+    ban = None
+    if banned is not None:
+        ban = torch.as_tensor(banned, dtype=torch.int32).reshape(-1).to(dev)
+    p = capi.ExlSampleParams()
+    p.temperature = settings.temperature
+    p.top_k = settings.top_k
+    p.top_p = settings.top_p
+    p.min_p = settings.min_p
+    p.typical = settings.typical
+    p.rep_penalty_max = settings.token_repetition_penalty_max
+    p.rep_sustain = settings.token_repetition_penalty_sustain
+    p.rep_decay = settings.token_repetition_penalty_decay
+    p.bos_token_id = -1 if bos_token_id is None else int(bos_token_id)
+    p.banned = ban.data_ptr() if ban is not None and ban.numel() else None
+    p.n_banned = ban.numel() if ban is not None else 0
+    return p, ban
+
+
 def sample(logits, settings: Settings, history=None, hist_lens=None, u=None, generator=None, bos_token_id=None, banned=None,
            dist=None):
     """One token per row of logits [bsz, vocab] fp32 (CUDA, unit stride along vocab; left unchanged).
@@ -62,21 +82,7 @@ def sample(logits, settings: Settings, history=None, hist_lens=None, u=None, gen
             raise ValueError(f"sample: {len(hl)} hist_lens for {bsz} rows")
         lens = (C.c_int * bsz)(*hl)
         hist_ptr = C.c_void_p(history.data_ptr())
-    ban = None
-    if banned is not None:
-        ban = torch.as_tensor(banned, dtype=torch.int32).reshape(-1).to(dev)
-    p = capi.ExlSampleParams()
-    p.temperature = settings.temperature
-    p.top_k = settings.top_k
-    p.top_p = settings.top_p
-    p.min_p = settings.min_p
-    p.typical = settings.typical
-    p.rep_penalty_max = settings.token_repetition_penalty_max
-    p.rep_sustain = settings.token_repetition_penalty_sustain
-    p.rep_decay = settings.token_repetition_penalty_decay
-    p.bos_token_id = -1 if bos_token_id is None else int(bos_token_id)
-    p.banned = ban.data_ptr() if ban is not None and ban.numel() else None
-    p.n_banned = ban.numel() if ban is not None else 0
+    p, ban = params(settings, dev, bos_token_id, banned)
     tokens = torch.empty(bsz, dtype=torch.int64, device=dev)
     probs = torch.empty(bsz, dtype=torch.float32, device=dev)
     if dist is not None and (dist.shape != (bsz, vocab) or dist.dtype != torch.float32 or not dist.is_contiguous()):

@@ -394,6 +394,34 @@ int exl_sample(const float* logits, int bsz, int vocab, int64_t logits_ld,
                const int64_t* history, int64_t hist_ld, const int* hist_len_host,
                const exl_sample_params* p, const float* u, int64_t* tokens, float* probs, float* dist, void* stream);
 
+/* Speculative sampling (new functionality; the reference has no speculative decoding): verify k draft tokens d_1 .. d_k of one
+   sequence against the target's logits so that the emitted tokens follow exactly the target's distribution (Leviathan et al.
+   2023, Chen et al. 2023).
+   Inputs: target_logits fp32 [k + 1][logits_ld], row j the target's logits after the prefix and d_1 .. d_j (exl_decode_step_multi
+   over [last token, d_1 .. d_k]); draft_tokens int64 [k]; draft_dist fp32 [k][dist_ld], q_j = the final distribution d_j was drawn
+   from (exl_sample's dist of the draft); optional history int64 [hist_len_host] (newest last); u fp32 [k + 1] uniforms in [0, 1):
+   u_0 .. u_{k-1} decide the acceptances, u_k the one draw; work fp32 [k + 1][vocab], caller-provided scratch.
+   The rule:
+     1. p_j = row j's final distribution under p, exactly as exl_sample computes it (same kernel), with the repetition-penalty
+        history history[0 .. hist_len_host) followed by d_1 .. d_j (no history: no penalty);
+     2. for j = 1 .. k: accept d_j iff u_{j-1} * q_j(d_j) < p_{j-1}(d_j) (fp32 product); stop at the first rejection;
+     3. d_j rejected: the correction is drawn from r = max(0, p_{j-1} - q_j) with u_k, masses in 2^-60 fixed point: the smallest id
+        whose inclusive cumulative mass, in ascending id order, exceeds floor(u_k * total) (computed in double); the largest id with
+        mass if rounding leaves that at or above the total; if r has no mass at all (rounding only), the same draw over p_{j-1};
+     4. all k accepted: the bonus token is exl_sample's draw of p_k with u_k.
+   Outputs: *n_accepted (int32) = a in 0 .. k; tokens int64 [k + 1] = d_1 .. d_a, the correction or bonus token, then -1;
+   probs fp32 [k + 1] = p of each emitted token (what sample() returns), NaN after them.  Rows past the first rejection are not
+   read.  A row the walk reaches that is undefined -- p_j undefined in exl_sample's sense, d_j outside [0, vocab), q_j(d_j) not
+   finite and positive -- gives *n_accepted = -1, every token -1 and every probability NaN.  k and hist_len_host are read on the
+   host (baked into a CUDA-graph capture).  Two launches (exl_sample over the k + 1 rows, then spec_residual_kernel); no
+   allocation, no floating-point atomics: two calls are bitwise equal.
+   EXL_ERR_ARG for everything exl_sample rejects (hist_len_host < 0 included), k outside 1 .. EXL_RAGGED_MAX_SEQ - 1,
+   dist_ld < vocab, or a NULL draft_tokens, draft_dist, u, work, n_accepted, tokens or probs. */
+int exl_spec_verify(const float* target_logits, int k, int vocab, int64_t logits_ld,
+                    const int64_t* draft_tokens, const float* draft_dist, int64_t dist_ld,
+                    const int64_t* history, int hist_len_host, const exl_sample_params* p, const float* u, float* work,
+                    int* n_accepted, int64_t* tokens, float* probs, void* stream);
+
 /* --- host-buffer entry point (end-to-end measurement and non-torch callers) ----- */
 
 /* q4_matmul with HOST x / out: copies x H2D, runs exl_q4_matmul, copies out D2H, synchronises `stream`.

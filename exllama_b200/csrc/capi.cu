@@ -76,9 +76,9 @@ int exl_own_scratch(ExlDevice* ds, int role, int64_t numel, half** out)
 extern "C" {
 
 const char* exl_last_error(void) { return t_err; }
-int exl_version(void) { return 107; }             // 101: exl_decode_desc.num_kv_heads; 102: batched decode plans and steps; 103: LoRA plans;
+int exl_version(void) { return 108; }             // 101: exl_decode_desc.num_kv_heads; 102: batched decode plans and steps; 103: LoRA plans;
                                                   // 104: exl_prefill_attn; 105: exl_prefill_attn_ragged, exl_rope_cache_ragged; 106: exl_sample;
-                                                  // 107: exl_spec_verify
+                                                  // 107: exl_spec_verify; 108: exl_token_logprobs
 int64_t exl_launch_count(void) { return g_launches.load(); }
 const char* exl_last_q4_path(void) { return g_last_q4_path; }
 

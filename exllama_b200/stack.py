@@ -358,13 +358,18 @@ class DecodeStack:
         return full.index_select(1, self.o_rows)
 
     # ---- prefill: unfused path (model.py:532-550) --------------------------------------------------------------
-    def prefill(self, hidden, past_len=0, last_only=True, seq=0):
+    def prefill(self, hidden, past_len=0, last_only=True, seq=0, targets=None):
         """hidden: [bsz, q_len, hidden] fp16; sequence b fills rows [past_len, past_len + q_len) of cache sequence seq + b and attends
         rows [0, past_len + t] of it (a prompt chunk, or a follow-up turn appended to a live cache).  Returns logits [bsz, vocab] of
         the last position (last_only) or [bsz * q_len, vocab].  At past_len 0 attention is torch's causal SDPA (model.py's
-        prompt path); at past_len > 0 it is csrc/prefill_attn.cu over the cache in place."""
+        prompt path); at past_len > 0 it is csrc/prefill_attn.cu over the cache in place.
+        targets: int64 token ids [bsz, q_len] (or any shape of bsz * q_len).  Then the head is rms_norm + exl_token_logprobs over every
+        position (last_only does not apply) and the call returns (logprob fp32 [bsz * q_len], greedy int64 [bsz * q_len]) instead of
+        logits (scoring.token_logprobs)."""
         s = self.shape
         bsz, q_len, _ = hidden.shape
+        if targets is not None:
+            self._check_targets(targets, bsz * q_len)
         if bsz > self.batch:
             raise ValueError(f"prefill of {bsz} sequences into caches that hold {self.batch} (DecodeStack(..., batch=))")
         if seq < 0 or seq + bsz > self.batch:
@@ -414,21 +419,37 @@ class DecodeStack:
             hidden = residual + y
         if self.lm_head is None:
             return hidden
+        if targets is not None:
+            return self._token_logprobs(hidden, targets)
         if last_only:
             hidden = hidden[:, -1:, :].contiguous()
         hn = cuda_ext.ext_rms_norm(hidden, self.norm, s.eps)
         return torch.matmul(hn.view(-1, s.hidden), self.lm_head.t()).float()
 
+    def _check_targets(self, targets, n):
+        if self.lm_head is None:
+            raise ValueError("targets given to a stack without a head (with_head=False)")
+        if not isinstance(targets, torch.Tensor) or targets.dtype != torch.int64 or targets.numel() != n or targets.device != self.device:
+            raise ValueError(f"targets must be an int64 tensor of {n} token ids on {self.device}, got "
+                             f"{getattr(targets, 'dtype', type(targets))} {tuple(getattr(targets, 'shape', ()))}")
+
+    def _token_logprobs(self, hidden, targets):
+        """The head of prefill(targets=) / prefill_ragged(targets=): rms_norm of every position, then exl_token_logprobs."""
+        from . import scoring
+        hn = cuda_ext.ext_rms_norm(hidden, self.norm, self.shape.eps)
+        return scoring.token_logprobs(hn.view(-1, self.shape.hidden), self.lm_head, targets.reshape(-1).contiguous())
+
     RAGGED_MAX_SEQ = 64                        # EXL_RAGGED_MAX_SEQ: sequences of one prefill_ragged call
 
-    def prefill_ragged(self, hidden, q_lens, past_lens, seqs=None, last_only=True):
+    def prefill_ragged(self, hidden, q_lens, past_lens, seqs=None, last_only=True, targets=None):
         """n prompts or follow-up turns of different lengths at different past_lens in one call.  hidden: [T, hidden] fp16, the
         sequences' tokens packed in order (sequence i owns rows [sum(q_lens[:i]), + q_lens[i])); sequence i fills rows
         [past_lens[i], past_lens[i] + q_lens[i]) of cache sequence seqs[i] (default 0 .. n-1, distinct) and attends rows
         [0, past_lens[i] + t] of it.  The same results as n prefill(x_i, past_lens[i], seq=seqs[i]) calls except for the GEMM route:
         the q4 GEMMs run once per layer on all T rows.  Per layer one rope_cache_ragged and one prefill_attn_ragged launch
         (csrc/elementwise.cu, csrc/prefill_attn.cu).  Returns the logits [n, vocab] of each sequence's last token (last_only) or
-        [T, vocab]."""
+        [T, vocab].  targets: int64 token ids [T], packed as hidden is; then the call returns (logprob fp32 [T], greedy int64 [T]) of
+        every position instead of logits, as prefill(targets=) does."""
         s = self.shape
         if self.tp_size > 1:
             raise NotImplementedError("prefill_ragged under tensor parallelism is not implemented")
@@ -451,6 +472,8 @@ class DecodeStack:
         T = sum(q_lens)
         if hidden.dim() != 2 or tuple(hidden.shape) != (T, s.hidden):
             raise ValueError(f"prefill_ragged: hidden {tuple(hidden.shape)} is not [sum(q_lens) = {T}, {s.hidden}]")
+        if targets is not None:
+            self._check_targets(targets, T)
         hq = self.local_heads * s.head_dim
         kvh = self.local_kv_heads
         ad = lambda i, n: (self.lora[i] or {}).get(n) if self.lora is not None else None      # (A, B) or None
@@ -474,6 +497,8 @@ class DecodeStack:
             hidden = residual + L.down.forward(y, ad(i, "down"))
         if self.lm_head is None:
             return hidden.view(T, s.hidden)
+        if targets is not None:
+            return self._token_logprobs(hidden, targets)
         if last_only:
             ends, t = [], 0
             for ql in q_lens:

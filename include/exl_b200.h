@@ -422,6 +422,24 @@ int exl_spec_verify(const float* target_logits, int k, int vocab, int64_t logits
                     const int64_t* history, int hist_len_host, const exl_sample_params* p, const float* u, float* work,
                     int* n_accepted, int64_t* tokens, float* probs, void* stream);
 
+/* --- token log-probabilities (exllama_b200/csrc/logprob.cu; the reference: matmul + log_softmax + gather, perplexity.py:118-121) --- */
+
+/* Per row t of the final-normed hidden states hn fp16 [T][H] (row-major) against lm_head fp16 [V][H] (row-major) and targets int64
+   [T], with logit[t][v] = sum_k hn[t][k] * lm_head[v][k] accumulated in fp32 from exact fp16 products (never rounded to fp16, never
+   written to memory):
+     logprob[t] = logit[t][targets[t]] - logsumexp_v logit[t][v]   (fp32)
+     greedy[t]  = argmax_v logit[t][v], ties to the lower id         (int64)
+   A target outside [0, V) gives logprob NaN; a NaN or inf in row t of hn gives logprob NaN and greedy -1.  Other rows are unaffected,
+   and nothing past T is written.  work: caller-provided device scratch of at least exl_token_logprobs_work_size bytes (per-row
+   partials of each vocab chunk).  Two launches (the fused GEMM + per-chunk softmax statistics, then a fixed-order merge); no
+   allocation, no host synchronisation and no atomics: two calls are bitwise equal, and the call can be captured in a CUDA graph.
+   EXL_ERR_ARG for T < 1, V < 1, H not a positive multiple of 64, a NULL or non-16-byte-aligned pointer, work_bytes too small, or
+   operands on different devices.  No GPU: EXL_ERR_CUDA (there is no CPU fallback). */
+int exl_token_logprobs(const void* hn, int T, int H, const void* lm_head, int V, const int64_t* targets, float* logprob,
+                       int64_t* greedy, void* work, int64_t work_bytes, void* stream);
+/* *bytes = the work exl_token_logprobs needs for T rows and V ids on device `device` (it depends on the SM count). */
+int exl_token_logprobs_work_size(int T, int V, int device, int64_t* bytes);
+
 /* --- host-buffer entry point (end-to-end measurement and non-torch callers) ----- */
 
 /* q4_matmul with HOST x / out: copies x H2D, runs exl_q4_matmul, copies out D2H, synchronises `stream`.

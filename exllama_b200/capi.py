@@ -35,6 +35,19 @@ class ExlSampleParams(C.Structure):
                 ("rep_penalty_max", f32), ("rep_sustain", i32), ("rep_decay", i32), ("bos_token_id", i32),
                 ("banned", vp), ("n_banned", i32)]
 
+class ExlKvCopyPair(C.Structure):
+    """exl_kv_copy_pair: rows [row_lo, row_hi) of cache sequence src copied to cache sequence dst."""
+    _fields_ = [("src", i32), ("dst", i32), ("row_lo", i32), ("row_hi", i32)]
+
+
+BEAM_EXPAND, BEAM_FIRST = 0, 1                  # EXL_BEAM_EXPAND / EXL_BEAM_FIRST
+
+
+def beam_work_bytes(rows, beams):
+    """EXL_BEAM_WORK_BYTES(rows, beams): the scratch exl_beam_select needs."""
+    return rows * beams * 8 + rows * 4
+
+
 # name -> (restype, argtypes); mirrors include/exl_b200.h one to one
 SIGNATURES = {
     "exl_last_error": (C.c_char_p, []),
@@ -77,6 +90,8 @@ SIGNATURES = {
     "exl_spec_verify": (i32, [vp, i32, i32, i64, vp, vp, i64, vp, i32, C.POINTER(ExlSampleParams), vp, vp, vp, vp, vp, vp]),
     "exl_token_logprobs": (i32, [vp, i32, i32, vp, i32, vp, vp, vp, vp, i64, vp]),
     "exl_token_logprobs_work_size": (i32, [i32, i32, i32, C.POINTER(i64)]),
+    "exl_beam_select": (i32, [vp, i32, i32, i64, C.POINTER(C.c_double), i32, i32, vp, vp, i64, vp, vp, vp, vp, vp, vp]),
+    "exl_kv_copy_rows": (i32, [C.POINTER(vp), C.POINTER(vp), i32, i32, i32, i32, i32, C.POINTER(ExlKvCopyPair), i32, vp]),
     "exl_q4_matmul_host": (i32, [vp, i32, vp, vp, vp, vp, vp]),
     "exl_decode_plan_create": (i32, [vp, C.POINTER(vp)]),
     "exl_decode_plan_create_batch": (i32, [vp, i32, C.POINTER(vp)]),

@@ -76,9 +76,10 @@ int exl_own_scratch(ExlDevice* ds, int role, int64_t numel, half** out)
 extern "C" {
 
 const char* exl_last_error(void) { return t_err; }
-int exl_version(void) { return 108; }             // 101: exl_decode_desc.num_kv_heads; 102: batched decode plans and steps; 103: LoRA plans;
+int exl_version(void) { return 109; }             // 101: exl_decode_desc.num_kv_heads; 102: batched decode plans and steps; 103: LoRA plans;
                                                   // 104: exl_prefill_attn; 105: exl_prefill_attn_ragged, exl_rope_cache_ragged; 106: exl_sample;
-                                                  // 107: exl_spec_verify; 108: exl_token_logprobs
+                                                  // 107: exl_spec_verify; 108: exl_token_logprobs;
+                                                  // 109: exl_beam_select, exl_kv_copy_rows
 int64_t exl_launch_count(void) { return g_launches.load(); }
 const char* exl_last_q4_path(void) { return g_last_q4_path; }
 
@@ -632,6 +633,20 @@ int exl_spec_verify(const float* target_logits, int k, int vocab, int64_t logits
 {
     return exl_spec_verify_launch(target_logits, k, vocab, logits_ld, draft_tokens, draft_dist, dist_ld, history, hist_len_host, p, u,
                                   work, n_accepted, tokens, probs, (cudaStream_t)stream);
+}
+
+int exl_beam_select(const float* dist, int rows, int vocab, int64_t dist_ld, const double* score_host, int beams, int mode, const float* u,
+                    void* work, int64_t work_bytes, int* parent, int64_t* token, float* prob, double* score, int* count, void* stream)
+{
+    return exl_beam_select_launch(dist, rows, vocab, dist_ld, score_host, beams, mode, u, work, work_bytes, parent, token, prob, score,
+                                  count, (cudaStream_t)stream);
+}
+
+int exl_kv_copy_rows(void* const* k_caches, void* const* v_caches, int n_layers, int num_cache_seqs, int num_kv_heads, int max_seq_len,
+                     int head_dim, const exl_kv_copy_pair* pairs, int n_pairs, void* stream)
+{
+    return exl_kv_copy_rows_launch(k_caches, v_caches, n_layers, num_cache_seqs, num_kv_heads, max_seq_len, head_dim, pairs, n_pairs,
+                                   (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------

@@ -178,6 +178,13 @@ int exl_spec_verify_launch(const float* target_logits, int k, int vocab, int64_t
                            const exl_sample_params* p, const float* u, float* work, int* n_accepted, int64_t* tokens, float* probs,
                            cudaStream_t stream);
 
+// beam.cu
+int exl_beam_select_launch(const float* dist, int rows, int vocab, int64_t dist_ld, const double* score_host, int beams, int mode,
+                           const float* u, void* work, int64_t work_bytes, int* parent, int64_t* token, float* prob, double* score,
+                           int* count, cudaStream_t stream);
+int exl_kv_copy_rows_launch(void* const* k_caches, void* const* v_caches, int n_layers, int num_cache_seqs, int num_kv_heads,
+                            int max_seq_len, int head_dim, const exl_kv_copy_pair* pairs, int n_pairs, cudaStream_t stream);
+
 // half_matmul.cu
 int exl_half_matmul_cublas_launch(ExlDevice* ds, const half* x, const half* w, half* out, int M, int K, int N, bool no_zero, cudaStream_t stream);
 int exl_half_matmul_custom_launch(const half* x, const half* w, half* out, int M, int K, int N, cudaStream_t stream);

@@ -422,6 +422,51 @@ int exl_spec_verify(const float* target_logits, int k, int vocab, int64_t logits
                     const int64_t* history, int hist_len_host, const exl_sample_params* p, const float* u, float* work,
                     int* n_accepted, int64_t* tokens, float* probs, void* stream);
 
+/* --- beam search (exllama_b200/csrc/beam.cu; the reference: ExLlamaGenerator.beam_search, generator.py:497-700) ------------- */
+
+#define EXL_BEAM_EXPAND 0
+#define EXL_BEAM_FIRST 1
+/* scratch exl_beam_select needs for `rows` rows and `beams` beams */
+#define EXL_BEAM_WORK_BYTES(rows, beams) ((int64_t)(rows) * (beams) * 8 + (int64_t)(rows) * 4)
+
+/* Choose beams from the rows' final distributions dist fp32 [rows][dist_ld] (exl_sample's dist rows: 0 outside the kept set).
+   A candidate is a (row r, token t) with dist[r][t] > 0; its score is score_host[r] + log((double)dist[r][t]) (float64;
+   score_host: host array of rows window scores, the sum of the log-probabilities of each beam's window).
+     EXL_BEAM_EXPAND: the best K = min(beams, #candidates) candidates under (score descending, row ascending, token ascending),
+                      written in the order (row ascending, score descending, token ascending).
+     EXL_BEAM_FIRST:  rows == 1; K = min(beams, #candidates) draws without replacement with u[0 .. K) (device fp32 uniforms in
+                      [0, 1)): draw j takes the smallest remaining id whose inclusive cumulative mass, in ascending id order and the
+                      sampler's 2^-60 fixed point, exceeds floor(u[j] * remaining total) (computed in double), or the largest
+                      remaining positive id if rounding leaves that at or above the total; the draws are written sorted by id.
+   Outputs (device, beams entries each): parent int32 (the row), token int64, prob fp32 (dist of that token), score float64; entries
+   past K get -1 / -1 / NaN / NaN.  *count (int32) = K, or -1 when a row is undefined: it holds a NaN, negative or infinite entry, or
+   no positive one (exl_sample writes a NaN row for a distribution it marks undefined); every entry is then -1 / -1 / NaN / NaN.
+   work: device scratch of at least EXL_BEAM_WORK_BYTES(rows, beams) bytes, 16-byte aligned.  rows, beams, mode and score_host are
+   read on the host (baked into a CUDA-graph capture).  Two launches in expand mode (one cluster per row, one merging CTA), one in
+   first mode; no allocation, no floating-point atomics: two calls are bitwise equal.
+   EXL_ERR_ARG (naming the value) for rows or beams outside 1 .. EXL_RAGGED_MAX_SEQ, rows != 1 in first mode, vocab outside
+   1 .. 262144, dist_ld < vocab, a mode that is neither, a NaN or +inf score_host entry, work_bytes too small, a misaligned work, or
+   a NULL pointer (dist, score_host, work, parent, token, prob, score, count; u in first mode). */
+int exl_beam_select(const float* dist, int rows, int vocab, int64_t dist_ld, const double* score_host, int beams, int mode, const float* u,
+                    void* work, int64_t work_bytes, int* parent, int64_t* token, float* prob, double* score, int* count, void* stream);
+
+#define EXL_KV_COPY_MAX_LAYERS 128
+/* Rows [row_lo, row_hi) of cache sequence src, copied to the same rows of cache sequence dst. */
+typedef struct { int src, dst, row_lo, row_hi; } exl_kv_copy_pair;
+
+/* Copy KV-cache rows between cache sequences, every layer, K and V, in one launch: for each of the n_pairs (1 .. EXL_RAGGED_MAX_SEQ)
+   host entries of pairs, rows [row_lo, row_hi) of sequence src go to the same rows of sequence dst in k_caches[l] and v_caches[l]
+   for l < n_layers (host arrays of device pointers to fp16 caches [num_cache_seqs][num_kv_heads][max_seq_len][head_dim], 16-byte
+   aligned).  Nothing else is written.  No sequence may be both a source and a destination and no destination may appear twice, so
+   the order of the copies does not matter.  An empty range copies nothing.  One CTA per (layer, K or V, KV head, pair), each a
+   contiguous run copied with 16-byte loads and stores.
+   EXL_ERR_ARG (naming the value) for n_layers outside 1 .. EXL_KV_COPY_MAX_LAYERS, n_pairs outside 1 .. EXL_RAGGED_MAX_SEQ,
+   num_cache_seqs < 2, num_kv_heads < 1, max_seq_len < 1, head_dim not a positive multiple of 8, a sequence outside
+   [0, num_cache_seqs), a range outside 0 <= row_lo <= row_hi <= max_seq_len, a sequence that is both a source and a destination
+   (src == dst included), a destination named twice, or a NULL or misaligned pointer. */
+int exl_kv_copy_rows(void* const* k_caches, void* const* v_caches, int n_layers, int num_cache_seqs, int num_kv_heads, int max_seq_len,
+                     int head_dim, const exl_kv_copy_pair* pairs, int n_pairs, void* stream);
+
 /* --- token log-probabilities (exllama_b200/csrc/logprob.cu; the reference: matmul + log_softmax + gather, perplexity.py:118-121) --- */
 
 /* Per row t of the final-normed hidden states hn fp16 [T][H] (row-major) against lm_head fp16 [V][H] (row-major) and targets int64

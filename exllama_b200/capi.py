@@ -35,6 +35,10 @@ class ExlSampleParams(C.Structure):
                 ("rep_penalty_max", f32), ("rep_sustain", i32), ("rep_decay", i32), ("bos_token_id", i32),
                 ("banned", vp), ("n_banned", i32)]
 
+GEN_MAX_STOP = 8                                # EXL_GEN_MAX_STOP
+GEN_LIVE, GEN_STOPPED, GEN_ERROR = 0, 1, 4      # EXL_GEN_LIVE / EXL_GEN_STOPPED / EXL_GEN_ERROR
+
+
 class ExlKvCopyPair(C.Structure):
     """exl_kv_copy_pair: rows [row_lo, row_hi) of cache sequence src copied to cache sequence dst."""
     _fields_ = [("src", i32), ("dst", i32), ("row_lo", i32), ("row_hi", i32)]
@@ -87,6 +91,9 @@ SIGNATURES = {
     "exl_rep_penalty": (i32, [i32, vp, vp, f32, i32, i32, i32]),
     "exl_apply_rep_penalty": (i32, [i32, vp, f32, i32, i32, i32, vp]),
     "exl_sample": (i32, [vp, i32, i32, i64, vp, i64, C.POINTER(i32), C.POINTER(ExlSampleParams), vp, vp, vp, vp, vp]),
+    "exl_sample_rows": (i32, [vp, i32, i32, i64, vp, i64, C.POINTER(i32), C.POINTER(ExlSampleParams), vp, vp, vp, vp, vp]),
+    "exl_gen_advance": (i32, [vp, vp, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), vp, i64, vp, vp, vp, i32, vp, i32, i32, vp, vp,
+                              vp, vp, i64, vp]),
     "exl_spec_verify": (i32, [vp, i32, i32, i64, vp, vp, i64, vp, i32, C.POINTER(ExlSampleParams), vp, vp, vp, vp, vp, vp]),
     "exl_token_logprobs": (i32, [vp, i32, i32, vp, i32, vp, vp, vp, vp, i64, vp]),
     "exl_token_logprobs_work_size": (i32, [i32, i32, i32, C.POINTER(i64)]),

@@ -76,10 +76,10 @@ int exl_own_scratch(ExlDevice* ds, int role, int64_t numel, half** out)
 extern "C" {
 
 const char* exl_last_error(void) { return t_err; }
-int exl_version(void) { return 109; }             // 101: exl_decode_desc.num_kv_heads; 102: batched decode plans and steps; 103: LoRA plans;
+int exl_version(void) { return 110; }             // 101: exl_decode_desc.num_kv_heads; 102: batched decode plans and steps; 103: LoRA plans;
                                                   // 104: exl_prefill_attn; 105: exl_prefill_attn_ragged, exl_rope_cache_ragged; 106: exl_sample;
                                                   // 107: exl_spec_verify; 108: exl_token_logprobs;
-                                                  // 109: exl_beam_select, exl_kv_copy_rows
+                                                  // 109: exl_beam_select, exl_kv_copy_rows; 110: exl_sample_rows, exl_gen_advance
 int64_t exl_launch_count(void) { return g_launches.load(); }
 const char* exl_last_q4_path(void) { return g_last_q4_path; }
 
@@ -625,6 +625,24 @@ int exl_sample(const float* logits, int bsz, int vocab, int64_t logits_ld, const
 {
     return exl_sample_launch(logits, bsz, vocab, logits_ld, history, hist_ld, hist_len_host, p, u, tokens, probs, dist,
                              (cudaStream_t)stream);
+}
+
+int exl_sample_rows(const float* logits, int bsz, int vocab, int64_t logits_ld, const int64_t* history, int64_t hist_ld,
+                    const int* hist_len_host, const exl_sample_params* p_rows, const float* u, int64_t* tokens, float* probs, float* dist,
+                    void* stream)
+{
+    return exl_sample_rows_launch(logits, bsz, vocab, logits_ld, history, hist_ld, hist_len_host, p_rows, u, tokens, probs, dist,
+                                  (cudaStream_t)stream);
+}
+
+int exl_gen_advance(const int64_t* tokens, const float* probs, int rows, const int* slot_host, const int* pos_host, const int* j_host,
+                    int64_t* hist, int64_t hist_ld, int* status, const int64_t* stop_ids, const uint64_t* seeds, int n_slots,
+                    const void* embed, int vocab, int hidden, void* x_next, float* u_next, int64_t* out_tokens, float* out_probs,
+                    int64_t out_ld, void* stream)
+{
+    return exl_gen_advance_launch(tokens, probs, rows, slot_host, pos_host, j_host, hist, hist_ld, status, stop_ids, seeds, n_slots,
+                                  (const half*)embed, vocab, hidden, (half*)x_next, u_next, out_tokens, out_probs, out_ld,
+                                  (cudaStream_t)stream);
 }
 
 int exl_spec_verify(const float* target_logits, int k, int vocab, int64_t logits_ld, const int64_t* draft_tokens,

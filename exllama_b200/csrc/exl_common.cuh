@@ -173,10 +173,19 @@ int exl_ragged_validate(const exl_ragged* r, int num_cache_seqs, int max_seq, co
 int exl_sample_launch(const float* logits, int bsz, int vocab, int64_t logits_ld, const int64_t* history, int64_t hist_ld,
                       const int* hist_len, const exl_sample_params* p, const float* u, int64_t* tokens, float* probs, float* dist,
                       cudaStream_t stream, const int64_t* tail = nullptr);
+int exl_sample_rows_launch(const float* logits, int bsz, int vocab, int64_t logits_ld, const int64_t* history, int64_t hist_ld,
+                           const int* hist_len, const exl_sample_params* p_rows, const float* u, int64_t* tokens, float* probs,
+                           float* dist, cudaStream_t stream);
 int exl_spec_verify_launch(const float* target_logits, int k, int vocab, int64_t logits_ld, const int64_t* draft_tokens,
                            const float* draft_dist, int64_t dist_ld, const int64_t* history, int hist_len,
                            const exl_sample_params* p, const float* u, float* work, int* n_accepted, int64_t* tokens, float* probs,
                            cudaStream_t stream);
+
+// generate.cu
+int exl_gen_advance_launch(const int64_t* tokens, const float* probs, int rows, const int* slot_host, const int* pos_host,
+                           const int* j_host, int64_t* hist, int64_t hist_ld, int* status, const int64_t* stop_ids,
+                           const uint64_t* seeds, int n_slots, const half* embed, int vocab, int hidden, half* x_next, float* u_next,
+                           int64_t* out_tokens, float* out_probs, int64_t out_ld, cudaStream_t stream);
 
 // beam.cu
 int exl_beam_select_launch(const float* dist, int rows, int vocab, int64_t dist_ld, const double* score_host, int beams, int mode,

@@ -18,18 +18,26 @@
 // Draw       inverse CDF in ascending token-id order over the kept set, in the same fixed point.
 #include "sample_select.cuh"
 #include <cmath>
+#include <cstdio>
 
 namespace {
+
+// One row's settings: exl_sample_params without its padding.  exl_sample gives every row the same; exl_sample_rows its own.
+struct RowParams {
+    float temperature; int top_k; float top_p, min_p, typical;
+    float pmax; int sustain, decay, bos, n_banned;
+    const int* banned;
+};
 
 struct SampleArgs {
     const float* logits; int64_t ld; int vocab; int slice;
     const int64_t* hist; int64_t hist_ld; int hist_len[EXL_RAGGED_MAX_SEQ];
     const int64_t* tail; int tail_at;            // history positions >= tail_at read tail[pos - tail_at] (tail NULL: none)
-    float temperature; int top_k; float top_p, min_p, typical;
-    float pmax; int sustain, decay, bos;
-    const int* banned; int n_banned;
     const float* u; int64_t* tokens; float* probs; float* dist;
+    RowParams rp[EXL_RAGGED_MAX_SEQ];            // a cluster is one row, so every branch on a row's settings is uniform in it
 };
+static_assert(sizeof(RowParams) == 48, "RowParams layout");
+static_assert(sizeof(SampleArgs) <= 4096, "SampleArgs must fit the classic 4 KB kernel parameter space");
 
 __device__ float penalty_value(const Shared& sh, long long j, long long s0, float dv)
 {
@@ -53,20 +61,21 @@ __global__ void __cluster_dims__(SP_CL, 1, 1) __launch_bounds__(SP_THREADS, 1) s
     const int n = max(0, min(a.slice, a.vocab - lo));
     int ph = 0;
     int bad = 0;
+    const RowParams& rs = a.rp[row];
 
     // 1. repetition penalty: newest window position of each token of the slice
-    const bool pen = a.hist != nullptr && a.pmax != 1.0f && a.hist_len[row] > 0;
+    const bool pen = a.hist != nullptr && rs.pmax != 1.0f && a.hist_len[row] > 0;
     long long s0 = 0, W = 0;
-    const float dv = a.decay ? (1.0f - a.pmax) / (float)a.decay : 0.0f;
+    const float dv = rs.decay ? (1.0f - rs.pmax) / (float)rs.decay : 0.0f;
     if (pen) {
         const long long len = a.hist_len[row];
-        s0 = a.sustain == -1 ? len : a.sustain;
-        const long long beg = max(0LL, len - s0 - a.decay);
+        s0 = rs.sustain == -1 ? len : rs.sustain;
+        const long long beg = max(0LL, len - s0 - rs.decay);
         W = len - beg;
         for (int i = threadIdx.x; i < n; i += SP_THREADS) s_int[i] = INT_MAX;
         if (threadIdx.x == 0) {
             const long long kmax = min((long long)SP_VTAB - 1, max(0LL, W - 1 - s0));
-            float v = a.pmax;
+            float v = rs.pmax;
             sh.vtab[0] = v;
             for (long long k = 1; k <= kmax; k++) { v += dv; sh.vtab[k] = v; }
         }
@@ -91,12 +100,12 @@ __global__ void __cluster_dims__(SP_CL, 1, 1) __launch_bounds__(SP_THREADS, 1) s
                 x = x > 0.0f ? __fdiv_rn(x, v) : x * v;
             }
         }
-        if (lo + i == a.bos) x = -10000.0f;
+        if (lo + i == rs.bos) x = -10000.0f;
         s_row[i] = x;
     }
     __syncthreads();
-    for (int k = threadIdx.x; k < a.n_banned; k += SP_THREADS) {
-        const int t = a.banned[k];
+    for (int k = threadIdx.x; k < rs.n_banned; k += SP_THREADS) {
+        const int t = rs.banned[k];
         if (t < 0 || t >= a.vocab) { bad = 1; continue; }
         if (t >= lo && t < lo + n) s_row[t - lo] = -INFINITY;
     }
@@ -104,7 +113,7 @@ __global__ void __cluster_dims__(SP_CL, 1, 1) __launch_bounds__(SP_THREADS, 1) s
     // 3. temperature, + 1e-8, softmax
     float mx = -INFINITY;
     for (int i = threadIdx.x; i < n; i += SP_THREADS) {
-        const float y = __fadd_rn(__fdiv_rn(s_row[i], a.temperature), 1e-8f);
+        const float y = __fadd_rn(__fdiv_rn(s_row[i], rs.temperature), 1e-8f);
         s_row[i] = y;
         if (isnan(y)) bad = 1;
         mx = fmaxf(mx, y);
@@ -133,22 +142,22 @@ __global__ void __cluster_dims__(SP_CL, 1, 1) __launch_bounds__(SP_THREADS, 1) s
     Row R;
     unsigned len = (unsigned)a.vocab;                                // length of the ordered list at the current stage
     // 4. top-k, then L1 normalisation
-    if (a.top_k > 0) {
-        R.kk = radix_descent(sh, ph, R, s_row, n, lo, 1, false, (unsigned)a.top_k, 0).key;
-        len = (unsigned)a.top_k;
+    if (rs.top_k > 0) {
+        R.kk = radix_descent(sh, ph, R, s_row, n, lo, 1, false, (unsigned)rs.top_k, 0).key;
+        len = (unsigned)rs.top_k;
         float s = 0.f;
         for (int i = threadIdx.x; i < n; i += SP_THREADS) if (desc_key(s_row[i], lo + i) >= R.kk) s += s_row[i];
         R.sk = fmaxf(cluster_sum_f(sh, ph, s), 1e-12f);
     }
     // 5. top-p with its min_p test, then renormalise
-    if (a.top_p > 0.0f) {
-        const unsigned long long T = (unsigned long long)((double)fminf(a.top_p, 2.0f) * SP_FIX);
+    if (rs.top_p > 0.0f) {
+        const unsigned long long T = (unsigned long long)((double)fminf(rs.top_p, 2.0f) * SP_FIX);
         const Descent c = radix_descent(sh, ph, R, s_row, n, lo, 1, true, 0, T);
         const unsigned n_p = c.found ? c.before : len;
         unsigned cm = 0;
         for (int i = threadIdx.x; i < n; i += SP_THREADS) {
             const Tok t = eval(R, s_row[i], lo + i, 1);
-            cm += (t.in && t.w >= a.min_p) ? 1u : 0u;
+            cm += (t.in && t.w >= rs.min_p) ? 1u : 0u;
         }
         cm = cluster_sum_c(sh, ph, cm);
         const unsigned keep = max(1u, min(min(n_p, cm), len));
@@ -164,14 +173,14 @@ __global__ void __cluster_dims__(SP_CL, 1, 1) __launch_bounds__(SP_THREADS, 1) s
         R.sp = fmaxf(cluster_sum_f(sh, ph, s), 1e-12f);
     }
     // 6. typical: order by |sum p log(p + eps) - log(p + eps)| ascending, the same prefix rule without min_p, renormalise
-    if (a.typical > 0.0f) {
+    if (rs.typical > 0.0f) {
         float s = 0.f;
         for (int i = threadIdx.x; i < n; i += SP_THREADS) {
             const Tok t = eval(R, s_row[i], lo + i, 2);
             if (t.in) s += t.w * logf(t.w + 1e-10f);
         }
         R.negent = cluster_sum_f(sh, ph, s);
-        const unsigned long long T = (unsigned long long)((double)fminf(a.typical, 2.0f) * SP_FIX);
+        const unsigned long long T = (unsigned long long)((double)fminf(rs.typical, 2.0f) * SP_FIX);
         const Descent c = radix_descent(sh, ph, R, s_row, n, lo, 3, true, 0, T);
         const unsigned n_t = c.found ? c.before : len;
         const unsigned keep = max(1u, min(n_t, len));
@@ -185,7 +194,7 @@ __global__ void __cluster_dims__(SP_CL, 1, 1) __launch_bounds__(SP_THREADS, 1) s
         }
         R.st = fmaxf(cluster_sum_f(sh, ph, s2), 1e-12f);
     }
-    const int level = a.typical > 0.0f ? 3 : (a.top_p > 0.0f ? 2 : 1);
+    const int level = rs.typical > 0.0f ? 3 : (rs.top_p > 0.0f ? 2 : 1);
 
     // 7. final distribution and the draw: thread t owns the contiguous run [t * per, (t + 1) * per) of the slice
     const int per = (n + SP_THREADS - 1) / SP_THREADS;
@@ -344,27 +353,41 @@ bool g_sample_attr[EXL_MAX_DEVICES];
 
 } // namespace
 
-int exl_sample_launch(const float* logits, int bsz, int vocab, int64_t logits_ld, const int64_t* history, int64_t hist_ld,
-                      const int* hist_len, const exl_sample_params* p, const float* u, int64_t* tokens, float* probs, float* dist,
-                      cudaStream_t stream, const int64_t* tail)
+// Checks one parameter set the way exl_sample always has; who is "sample" or "sample: row <b>" (exl_sample_rows names the row).
+static int check_params(const exl_sample_params* p, int vocab, const char* who)
 {
-    if (!p) return exl_set_err(EXL_ERR_ARG, "sample: params is NULL");
+    if (!std::isfinite(p->temperature) || !(p->temperature > 0.0f))
+        return exl_set_err(EXL_ERR_ARG, "%s: temperature %g is not finite and positive", who, (double)p->temperature);
+    if (p->top_k < 0 || p->top_k > vocab) return exl_set_err(EXL_ERR_ARG, "%s: top_k %d outside [0, vocab %d]", who, p->top_k, vocab);
+    if (!(p->top_p >= 0.0f)) return exl_set_err(EXL_ERR_ARG, "%s: top_p %g is negative", who, (double)p->top_p);
+    if (!(p->min_p >= 0.0f)) return exl_set_err(EXL_ERR_ARG, "%s: min_p %g is negative", who, (double)p->min_p);
+    if (!(p->typical >= 0.0f)) return exl_set_err(EXL_ERR_ARG, "%s: typical %g is negative", who, (double)p->typical);
+    if (p->rep_sustain < -1) return exl_set_err(EXL_ERR_ARG, "%s: rep_sustain %d < -1", who, p->rep_sustain);
+    if (p->rep_decay < 0) return exl_set_err(EXL_ERR_ARG, "%s: rep_decay %d < 0", who, p->rep_decay);
+    if (p->n_banned < 0 || (p->n_banned > 0 && !p->banned))
+        return exl_set_err(EXL_ERR_ARG, "%s: n_banned %d with banned %p", who, p->n_banned, (const void*)p->banned);
+    return EXL_OK;
+}
+
+// per_row: row b uses p[b] (exl_sample_rows); else every row uses p[0]
+static int sample_launch(const float* logits, int bsz, int vocab, int64_t logits_ld, const int64_t* history, int64_t hist_ld,
+                         const int* hist_len, const exl_sample_params* p, bool per_row, const float* u, int64_t* tokens, float* probs,
+                         float* dist, cudaStream_t stream, const int64_t* tail)
+{
+    if (!p) return exl_set_err(EXL_ERR_ARG, per_row ? "sample: p_rows is NULL" : "sample: params is NULL");
     if (!logits || !u || !tokens || !probs)
         return exl_set_err(EXL_ERR_ARG, "sample: NULL pointer (logits %p, u %p, tokens %p, probs %p)", (const void*)logits,
                            (const void*)u, (void*)tokens, (void*)probs);
     if (bsz < 1 || bsz > EXL_RAGGED_MAX_SEQ) return exl_set_err(EXL_ERR_ARG, "sample: bsz %d outside [1, %d]", bsz, EXL_RAGGED_MAX_SEQ);
     if (vocab < 1 || vocab > SP_MAX_VOCAB) return exl_set_err(EXL_ERR_ARG, "sample: vocab %d outside [1, %d]", vocab, SP_MAX_VOCAB);
     if (logits_ld < vocab) return exl_set_err(EXL_ERR_ARG, "sample: logits_ld %lld < vocab %d", (long long)logits_ld, vocab);
-    if (!std::isfinite(p->temperature) || !(p->temperature > 0.0f))
-        return exl_set_err(EXL_ERR_ARG, "sample: temperature %g is not finite and positive", (double)p->temperature);
-    if (p->top_k < 0 || p->top_k > vocab) return exl_set_err(EXL_ERR_ARG, "sample: top_k %d outside [0, vocab %d]", p->top_k, vocab);
-    if (!(p->top_p >= 0.0f)) return exl_set_err(EXL_ERR_ARG, "sample: top_p %g is negative", (double)p->top_p);
-    if (!(p->min_p >= 0.0f)) return exl_set_err(EXL_ERR_ARG, "sample: min_p %g is negative", (double)p->min_p);
-    if (!(p->typical >= 0.0f)) return exl_set_err(EXL_ERR_ARG, "sample: typical %g is negative", (double)p->typical);
-    if (p->rep_sustain < -1) return exl_set_err(EXL_ERR_ARG, "sample: rep_sustain %d < -1", p->rep_sustain);
-    if (p->rep_decay < 0) return exl_set_err(EXL_ERR_ARG, "sample: rep_decay %d < 0", p->rep_decay);
-    if (p->n_banned < 0 || (p->n_banned > 0 && !p->banned))
-        return exl_set_err(EXL_ERR_ARG, "sample: n_banned %d with banned %p", p->n_banned, (const void*)p->banned);
+    for (int b = 0; b < (per_row ? bsz : 1); b++) {
+        char who[32];
+        if (per_row) snprintf(who, sizeof who, "sample: row %d", b);
+        else snprintf(who, sizeof who, "sample");
+        const int rc = check_params(p + b, vocab, who);
+        if (rc != EXL_OK) return rc;
+    }
     SampleArgs a{};
     if (history) {
         if (!hist_len) return exl_set_err(EXL_ERR_ARG, "sample: history without hist_len_host");
@@ -376,9 +399,11 @@ int exl_sample_launch(const float* logits, int bsz, int vocab, int64_t logits_ld
     }
     a.logits = logits; a.ld = logits_ld; a.vocab = vocab; a.slice = (vocab + SP_CL - 1) / SP_CL;
     a.hist = history; a.hist_ld = tail ? 0 : hist_ld;
-    a.temperature = p->temperature; a.top_k = p->top_k; a.top_p = p->top_p; a.min_p = p->min_p; a.typical = p->typical;
-    a.pmax = p->rep_penalty_max; a.sustain = p->rep_sustain; a.decay = p->rep_decay; a.bos = p->bos_token_id;
-    a.banned = p->banned; a.n_banned = p->n_banned;
+    for (int b = 0; b < bsz; b++) {
+        const exl_sample_params* q = per_row ? p + b : p;
+        a.rp[b] = RowParams{q->temperature, q->top_k, q->top_p, q->min_p, q->typical, q->rep_penalty_max, q->rep_sustain, q->rep_decay,
+                            q->bos_token_id, q->n_banned, q->banned};
+    }
     a.u = u; a.tokens = tokens; a.probs = probs; a.dist = dist;
 
     int dev = 0;
@@ -392,6 +417,21 @@ int exl_sample_launch(const float* logits, int bsz, int vocab, int64_t logits_ld
     sample_kernel<<<dim3(SP_CL, bsz), SP_THREADS, smem, stream>>>(a);
     EXL_CHECK_LAUNCH("sample_kernel");
     return EXL_OK;
+}
+
+int exl_sample_launch(const float* logits, int bsz, int vocab, int64_t logits_ld, const int64_t* history, int64_t hist_ld,
+                      const int* hist_len, const exl_sample_params* p, const float* u, int64_t* tokens, float* probs, float* dist,
+                      cudaStream_t stream, const int64_t* tail)
+{
+    return sample_launch(logits, bsz, vocab, logits_ld, history, hist_ld, hist_len, p, false, u, tokens, probs, dist, stream, tail);
+}
+
+int exl_sample_rows_launch(const float* logits, int bsz, int vocab, int64_t logits_ld, const int64_t* history, int64_t hist_ld,
+                           const int* hist_len, const exl_sample_params* p_rows, const float* u, int64_t* tokens, float* probs,
+                           float* dist, cudaStream_t stream)
+{
+    return sample_launch(logits, bsz, vocab, logits_ld, history, hist_ld, hist_len, p_rows, true, u, tokens, probs, dist, stream,
+                         nullptr);
 }
 
 int exl_spec_verify_launch(const float* target_logits, int k, int vocab, int64_t logits_ld, const int64_t* draft_tokens,

@@ -1,0 +1,428 @@
+"""Batched generation on the device: many requests, each with its own settings, seed, stop ids, bos id and banned list, through the
+stack's cache sequences, with a slot refilled as soon as its request finishes (continuous batching; DESIGN.md §4g).
+
+    gen = generate.BatchGenerator(stack, embed)
+    rid = gen.submit(generate.Request(prompt_ids, max_new_tokens=128, settings=s, stop_ids=[eos], seed=7))
+    results = gen.run()                          # {id: Result(tokens, probs, finish, t_first)}
+
+Cache sequence s of the stack is slot s.  Each step() steps every live request by one token, then admits waiting requests into the
+lowest free slots (their prompts in one prefill_ragged, their first tokens through one exl_sample_rows and one exl_gen_advance).  A
+step is one decode_step_fused_batch over slots 0 .. highest live slot (or one prefill_ragged when the stack has no fused plan), one
+exl_sample_rows with each row's own settings and one exl_gen_advance, which appends the tokens, tests the stop ids and writes the
+next step's input rows and uniforms on the device.  The host never waits on the step in flight: length and cache-full finishes are
+decided on the host, and the device status (stop, error) of step k - 1 is read after step k has been launched.  A request that
+stopped at step k - 1 is therefore stepped once more; exl_gen_advance ignores that row (the status is sticky), and its slot is
+freed one step late.
+
+Token j of a request is what sampling.sample returns for its logits row with the request's settings, bos id and banned list,
+history = prompt + tokens 0 .. j - 1, and u = uniform(seed, j) (include/exl_b200.h U), so a request's tokens do not depend on
+which other requests share its steps.
+"""
+from __future__ import annotations
+
+import collections
+import copy
+import ctypes as C
+import time
+
+import torch
+
+from . import capi, sampling
+
+MAX_STOP = capi.GEN_MAX_STOP
+_M64 = (1 << 64) - 1
+
+
+def uniform(seed, j):
+    """U(seed, j) of include/exl_b200.h: splitmix64 output j (0-based) of the stream seeded with seed, top 24 bits / 2^24 (a float
+    that fp32 holds exactly)."""
+    x = (int(seed) + (int(j) + 1) * 0x9E3779B97F4A7C15) & _M64
+    x = ((x ^ (x >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    x = ((x ^ (x >> 27)) * 0x94D049BB133111EB) & _M64
+    x ^= x >> 31
+    return (x >> 40) / float(1 << 24)
+
+
+class Request:
+    """One completion to generate.  prompt_ids: a non-empty 1-D list or tensor of ids; max_new_tokens >= 1; settings: a
+    sampling.Settings (default its defaults), used as given; stop_ids: up to MAX_STOP ids that end the request (the stop token is
+    kept); seed: the request's uniforms are uniform(seed, j); bos_token_id, banned: as sampling.sample."""
+
+    def __init__(self, prompt_ids, max_new_tokens, settings=None, stop_ids=(), seed=0, bos_token_id=None, banned=None):
+        self.prompt = [int(t) for t in torch.as_tensor(prompt_ids, dtype=torch.int64).reshape(-1).tolist()]
+        self.max_new_tokens = int(max_new_tokens)
+        self.settings = settings if settings is not None else sampling.Settings()
+        self.stop_ids = [int(t) for t in stop_ids]
+        self.seed = int(seed) & _M64
+        self.bos_token_id = bos_token_id
+        self.banned = None if banned is None else [int(t) for t in banned]
+        if not self.prompt:
+            raise ValueError("Request: the prompt is empty")
+        if self.max_new_tokens < 1:
+            raise ValueError(f"Request: max_new_tokens {self.max_new_tokens} must be at least 1")
+        if len(self.stop_ids) > MAX_STOP:
+            raise ValueError(f"Request: {len(self.stop_ids)} stop ids, at most {MAX_STOP}")
+
+
+class Result:
+    """tokens, probs: host lists of the generated tokens and their final probabilities; finish: "stop" (the last token is a stop
+    id), "length" (max_new_tokens), "max_seq" (the cache sequence is full) or "error" (an undefined distribution: NaN logits, or
+    every token masked; tokens then holds the ones before it); t_first: seconds from submit() to the host's first sight of the
+    first token (one step after it was drawn, as every status read)."""
+
+    def __init__(self):
+        self.tokens, self.probs, self.finish, self.t_first = [], [], None, None
+        self._fetch, self._n = None, None
+
+    def _settle(self):
+        if self._fetch is not None:
+            ev, tok, prob = self._fetch
+            ev.synchronize()
+            t, p = tok.tolist(), prob.tolist()
+            n = t.index(-1) if -1 in t else len(t)
+            self.tokens, self.probs = t[:n], p[:n]
+            self._fetch = None
+
+
+class _Live:
+    __slots__ = ("rid", "req", "slot", "L", "n", "t0", "host_finish")
+
+    def __init__(self, rid, req, slot, t0):
+        self.rid, self.req, self.slot, self.L, self.n, self.t0 = rid, req, slot, len(req.prompt), 0, t0
+        self.host_finish = None
+
+
+class Scheduler:
+    """The host side of batched generation: admission, slots, positions and finishes.  dev carries out the device work (_Device for
+    a DecodeStack; tests substitute a fake): admit(lives), step(lives), copy_status() -> i (an index), read_status(i) -> the status of every slot when copy i was made (host int array), fetch(live, n)
+    -> (event, tokens, probs), release(slot)."""
+
+    def __init__(self, dev, n_slots, max_seq):
+        self.dev, self.n_slots, self.max_seq = dev, int(n_slots), int(max_seq)
+        self.waiting = collections.deque()
+        self.slots = [None] * self.n_slots
+        self.results = {}
+        self.order = []                     # (iteration, "admit" | "step" | "release" | "finish", ...) events, for tests
+        self._next_id = 0
+        self._lag = None                    # (copy index, [(live, tokens issued)]) of the previous status copy, not read yet
+        self._k = 0
+
+    def submit(self, req):
+        if len(req.prompt) + 1 > self.max_seq:
+            raise ValueError(f"submit: a prompt of {len(req.prompt)} tokens leaves no room for a token in max_seq {self.max_seq}")
+        rid = self._next_id
+        self._next_id += 1
+        self.waiting.append((rid, req, time.perf_counter()))
+        self.results[rid] = Result()
+        return rid
+
+    def _limit(self, lv):
+        """The host's finish of lv after its tokens so far, or None."""
+        if lv.n >= lv.req.max_new_tokens:
+            return "length"
+        if lv.L + lv.n >= self.max_seq:
+            return "max_seq"
+        return None
+
+    def _fetch(self, lv, n):
+        res = self.results[lv.rid]
+        if res._n != n:                     # an earlier fetch of a different count is replaced before the slot can be reused
+            res._fetch, res._n = self.dev.fetch(lv, n), n
+
+    def _finish(self, lv, reason, n):
+        self.results[lv.rid].finish = reason
+        self._fetch(lv, n)
+        if self.slots[lv.slot] is lv:
+            self._release(lv)
+        self.order.append((self._k, "finish", lv.rid, lv.slot, reason))
+
+    def _release(self, lv):
+        self.slots[lv.slot] = None
+        self.dev.release(lv.slot)
+        self.order.append((self._k, "release", lv.rid, lv.slot))
+
+    def step(self):
+        """One iteration: one step of the live requests, admissions (prompt and first token), the status read of the previous iteration.  Returns
+        False when nothing was left to do."""
+        live = [lv for lv in self.slots if lv is not None]
+        if not self.waiting and not live and self._lag is None:
+            return False
+        adm, tokens = [], 0
+        # waiting requests in order into the lowest free slots, at most max_seq prompt tokens in one admission (the prefill's
+        # scratch is sized for max_seq rows); the first one always goes
+        while self.waiting and None in self.slots and (not adm or tokens + len(self.waiting[0][1].prompt) <= self.max_seq):
+            rid, req, t0 = self.waiting.popleft()
+            tokens += len(req.prompt)
+            s = self.slots.index(None)
+            lv = _Live(rid, req, s, t0)
+            self.slots[s] = lv
+            adm.append(lv)
+        run = live
+        # the step first: a fused step covers free slots at past_len 0 and writes their row 0, which the admission's prefill then
+        # overwrites
+        if run:
+            self.dev.step(run)
+            for lv in run:
+                lv.n += 1
+            self.order.append((self._k, "step", [(lv.slot, lv.L + lv.n - 2) for lv in run]))
+        if adm:
+            self.dev.admit(adm)
+            for lv in adm:
+                lv.n = 1
+            self.order.append((self._k, "admit", [(lv.rid, lv.slot) for lv in adm]))
+        snap = []
+        for lv in adm + run:
+            snap.append((lv, lv.n))
+            lv.host_finish = self._limit(lv)
+        copy = self.dev.copy_status() if snap else None
+        # a request the host has finished is stepped no more: free its slot now (a stop or error in its last token is settled from
+        # the status read that covers it)
+        for lv in adm + run:
+            if lv.host_finish is not None:
+                self._fetch(lv, lv.n)
+                self._release(lv)
+        if self._lag is not None:
+            status = self.dev.read_status(self._lag[0])
+            now = time.perf_counter()
+            for lv, n in self._lag[1]:
+                res = self.results[lv.rid]
+                if res.t_first is None:
+                    res.t_first = now - lv.t0
+                if res.finish is not None:
+                    continue
+                st = int(status[lv.slot])
+                if st == capi.GEN_STOPPED:
+                    self._finish(lv, "stop", n)
+                elif st == capi.GEN_ERROR:
+                    self._finish(lv, "error", n)
+                elif lv.host_finish is not None and n == lv.n:
+                    self._finish(lv, lv.host_finish, n)
+        self._lag = (copy, snap) if snap else None
+        self._k += 1
+        return True
+
+    def run(self):
+        """step() until every submitted request has finished; returns {id: Result}."""
+        while self.step():
+            pass
+        for res in self.results.values():
+            res._settle()
+        return self.results
+
+
+def fused_rows(lives):
+    """The rows of a fused step over the requests lives: slots 0 .. highest live slot, each live slot's request (its last token at
+    position L + n - 1, the past_len it is stepped at), None and past_len 0 for a free slot (its row reads no history and the next
+    prefill into that slot overwrites the row it writes).  Returns (rows, past_lens)."""
+    by_slot = {lv.slot: lv for lv in lives}
+    rows = [by_slot.get(s) for s in range(max(by_slot) + 1)]
+    return rows, [lv.L + lv.n - 1 if lv is not None else 0 for lv in rows]
+
+
+class _Device:
+    """The device side of BatchGenerator over a DecodeStack: per-slot history, status, stop ids, seeds, next inputs, uniforms and
+    output rows, and the launches of an admission and of a step."""
+
+    def __init__(self, stack, embed, owner):
+        st = self.st = stack
+        self.emb, self.owner = embed, owner
+        self.dev = embed.device
+        n, ms, H, V = stack.batch, stack.max_seq, stack.shape.hidden, stack.shape.vocab
+        self.n_slots, self.max_seq, self.H, self.V = n, ms, H, V
+        z = lambda shape, dt: torch.zeros(shape, dtype=dt, device=self.dev)
+        self.hist = z((n, ms), torch.int64)
+        self.status = torch.full((n,), capi.GEN_STOPPED, dtype=torch.int32, device=self.dev)
+        self.stop = torch.full((n, MAX_STOP), -1, dtype=torch.int64, device=self.dev)
+        self.seeds = z((n,), torch.int64)                    # uint64 bit patterns
+        self.x_next = z((n, H), torch.float16)
+        self.u_next = z((n,), torch.float32)
+        self.out_tok = z((n, ms), torch.int64)
+        self.out_prob = z((n, ms), torch.float32)
+        self.tokens = z((n,), torch.int64)
+        self.probs = z((n,), torch.float32)
+        self.pin = torch.zeros((2, n), dtype=torch.int32).pin_memory()
+        self.pin_ev = [None, None]
+        self.copies = 0
+        self.rowp = (capi.ExlSampleParams * n)()             # each slot's sampler settings (slot order: the fused route's rows)
+        self.keep = [None] * n                               # the banned tensors rowp points into
+        for s in range(n):
+            self.release(s)
+        if getattr(stack, "dplan", None) is not None:
+            stack.dplan.close()
+            stack.dplan = None
+        try:
+            stack.make_plan()
+            self.fused = True
+        except capi.ExlError:
+            stack.dplan = None
+            self.fused = False
+
+    def _up(self, values, dtype):
+        """values (host) on the device without a host synchronisation: a pinned copy, which torch keeps until the copy is done."""
+        return torch.tensor(values, dtype=dtype).pin_memory().to(self.dev, non_blocking=True)
+
+    def release(self, s):
+        self.rowp[s], _ = sampling.params(sampling.Settings(), self.dev)
+        self.keep[s] = None
+
+    def _advance(self, rows, slots, pos, js):
+        n = len(slots)
+        arr = lambda v: (C.c_int * n)(*[int(x) for x in v])
+        capi.check(capi.lib().exl_gen_advance(capi._ptr(self.tokens), capi._ptr(self.probs), n, arr(slots), arr(pos), arr(js),
+                                              capi._ptr(self.hist), self.max_seq, capi._ptr(self.status), capi._ptr(self.stop),
+                                              capi._ptr(self.seeds), self.n_slots, capi._ptr(self.emb), self.V, self.H,
+                                              capi._ptr(self.x_next), capi._ptr(self.u_next), capi._ptr(self.out_tok),
+                                              capi._ptr(self.out_prob), self.max_seq, capi._stream()))
+
+    def _sample(self, logits, params, history, hist_lens, u):
+        n = logits.shape[0]
+        lens = (C.c_int * n)(*hist_lens)
+        capi.check(capi.lib().exl_sample_rows(capi._ptr(logits), n, self.V, logits.stride(0) if n > 1 else self.V,
+                                              capi._ptr(history), self.max_seq, lens, params, capi._ptr(u), capi._ptr(self.tokens),
+                                              capi._ptr(self.probs), None, capi._stream()))
+
+    def _trace(self, kind, logits, lives, u):
+        tr = self.owner.trace
+        if tr is not None:
+            tr.append(dict(kind=kind, logits=logits.cpu().numpy().copy(), rids=[lv.rid for lv in lives],
+                           slots=[lv.slot for lv in lives], j=[lv.n for lv in lives], u=u.cpu().numpy().copy()))
+
+    def admit(self, lives):
+        n = len(lives)
+        slots = [lv.slot for lv in lives]
+        ids = self._up([t for lv in lives for t in lv.req.prompt], torch.int64)
+        idx = self._up(slots, torch.int64)
+        meta = self._up([lv.req.stop_ids + [-1] * (MAX_STOP - len(lv.req.stop_ids)) + [lv.req.seed - (1 << 64) if lv.req.seed >> 63 else
+                                                                                     lv.req.seed] for lv in lives], torch.int64)
+        self.stop[idx] = meta[:, :MAX_STOP]
+        self.seeds[idx] = meta[:, MAX_STOP]
+        self.status[idx] = capi.GEN_LIVE
+        off = 0
+        for lv in lives:
+            self.hist[lv.slot, :lv.L] = ids[off:off + lv.L]
+            off += lv.L
+            ban = self._up(lv.req.banned, torch.int32) if lv.req.banned else None
+            p, ban = sampling.params(lv.req.settings, self.dev, lv.req.bos_token_id, ban)
+            self.rowp[lv.slot], self.keep[lv.slot] = p, ban
+        params = (capi.ExlSampleParams * n)(*[self.rowp[s] for s in slots])
+        u = self._up([uniform(lv.req.seed, 0) for lv in lives], torch.float32)
+        logits = self.st.prefill_ragged(self.emb[ids], [lv.L for lv in lives], [0] * n, seqs=slots, last_only=True)
+        self._trace("admit", logits, lives, u)
+        self._sample(logits, params, self.hist.index_select(0, idx), [lv.L for lv in lives], u)
+        self._advance(n, slots, [lv.L for lv in lives], [0] * n)
+
+    def step(self, lives):
+        ev = None
+        if self.owner.timings is not None:
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+            ev[0].record()
+        st = self.st
+        by_slot = {lv.slot: lv for lv in lives}
+        if self.fused:
+            rows, pasts = fused_rows(lives)
+            hi = len(rows)
+            x = self.x_next[:hi].view(hi, 1, self.H)
+            logits = st.decode_step_fused(x, pasts[0]).view(1, -1) if st.batch == 1 else st.decode_step_fused_batch(x, pasts)
+            params, history, u = self.rowp, self.hist, self.u_next
+        else:
+            slots = sorted(by_slot)
+            idx = self._up(slots, torch.int64)
+            rows = [by_slot[s] for s in slots]
+            logits = st.prefill_ragged(self.x_next.index_select(0, idx), [1] * len(rows), [lv.L + lv.n - 1 for lv in rows], seqs=slots,
+                                       last_only=False)
+            params = (capi.ExlSampleParams * len(rows))(*[self.rowp[s] for s in slots])
+            history, u = self.hist.index_select(0, idx), self.u_next.index_select(0, idx)
+        if ev:
+            ev[1].record()
+        if self.owner.trace is not None:
+            live_rows = [lv for lv in rows if lv is not None]
+            tr_u = u[:len(rows)]
+            self._trace("step", logits[[i for i, lv in enumerate(rows) if lv is not None]], live_rows,
+                        tr_u[[i for i, lv in enumerate(rows) if lv is not None]])
+        self._sample(logits, params, history, [lv.L + lv.n if lv is not None else 0 for lv in rows], u)
+        if ev:
+            ev[2].record()
+        self._advance(len(rows), [lv.slot if lv is not None else -1 for lv in rows], [lv.L + lv.n if lv is not None else 0 for lv in rows],
+                      [lv.n if lv is not None else 0 for lv in rows])
+        if ev:
+            ev[3].record()
+            self.owner.timings.append((ev, len(lives)))
+
+    def copy_status(self):
+        """Copy the status into pinned buffer i % 2 behind an event; copy i is read (read_status(i)) before copy i + 2 is made."""
+        i = self.copies
+        self.pin[i % 2].copy_(self.status, non_blocking=True)
+        self.pin_ev[i % 2] = torch.cuda.Event()
+        self.pin_ev[i % 2].record()
+        self.copies += 1
+        return i
+
+    def read_status(self, i):
+        self.pin_ev[i % 2].synchronize()
+        return self.pin[i % 2].numpy().copy()
+
+    def fetch(self, lv, n):
+        tok = torch.empty(n, dtype=torch.int64).pin_memory()
+        prob = torch.empty(n, dtype=torch.float32).pin_memory()
+        tok.copy_(self.out_tok[lv.slot, :n], non_blocking=True)
+        prob.copy_(self.out_prob[lv.slot, :n], non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record()
+        return ev, tok, prob
+
+
+class BatchGenerator(Scheduler):
+    """Batched generation over one DecodeStack (module docstring; DESIGN.md §4g).
+
+    stack   a DecodeStack with an lm_head; its batch cache sequences are the slots, its max_seq bounds prompt + completion
+    embed   fp16 [vocab, hidden]: maps a token to the stack's input
+
+    submit(Request) -> id; step() runs one iteration; run() steps until every request has finished and returns {id: Result}.
+    The step is decode_step_fused_batch when stack.make_plan() succeeds (fused is then True), else prefill_ragged with one token per
+    live slot (act-order, or more slots than the fused plan takes).  trace: set to a list to record every admission's and step's
+    logits rows with their request ids, slots, token indices and uniforms (tests).  timings: set to a list to record, per step,
+    four CUDA events (start, after the step, the sampler, the advance) and the number of requests stepped (tools/generate_bench.py)."""
+
+    def __init__(self, stack, embed):
+        if stack.tp_size > 1:
+            raise NotImplementedError("batched generation under tensor parallelism is not implemented")
+        if stack.lm_head is None:
+            raise ValueError("BatchGenerator: the stack has no lm_head")
+        if stack.batch > MAX_SLOTS:
+            raise ValueError(f"BatchGenerator: the stack holds {stack.batch} cache sequences, at most {MAX_SLOTS}")
+        if embed.dtype != torch.float16 or tuple(embed.shape) != (stack.shape.vocab, stack.shape.hidden) or not embed.is_contiguous():
+            raise ValueError(f"BatchGenerator: embed must be contiguous fp16 [{stack.shape.vocab}, {stack.shape.hidden}], got "
+                             f"{embed.dtype} {tuple(embed.shape)}")
+        self.trace = None
+        self.timings = None
+        super().__init__(_Device(stack, embed, self), stack.batch, stack.max_seq)
+        self.fused = self.dev.fused
+
+    def submit(self, req):
+        v = self.dev.V
+        bad = [t for t in req.prompt + req.stop_ids if not 0 <= t < v]
+        if bad:
+            raise ValueError(f"submit: token id {bad[0]} outside the vocabulary [0, {v})")
+        return super().submit(req)
+
+
+MAX_SLOTS = 64                                          # EXL_RAGGED_MAX_SEQ: rows of one exl_sample_rows / exl_gen_advance
+
+
+def generate_simple(stack, embed, prompts, max_new_tokens=128, settings=None, eos_token_id=None, bos_token_id=None, banned=None,
+                    seed=0):
+    """ExLlamaGenerator.generate_simple over a list of prompts (lists of ids): each prompt is one request with min_p 0 and the bos
+    mask, as gen_single_token samples (generator.py:355,366), seed seed + i for prompt i, max_new_tokens clipped to max_seq - the
+    prompt's length, and eos_token_id as its stop id.  One difference from the reference: a row ends at its own EOS, where the
+    reference steps every row until all of them have one.  Returns each prompt followed by its tokens (host lists of ids)."""
+    s = copy.copy(settings if settings is not None else sampling.Settings())
+    s.min_p = 0.0
+    gen = BatchGenerator(stack, embed)
+    ids = []
+    for i, p in enumerate(prompts):
+        req = Request(p, 1, s, stop_ids=() if eos_token_id is None else (eos_token_id,), seed=seed + i, bos_token_id=bos_token_id,
+                      banned=banned)
+        req.max_new_tokens = max(1, min(int(max_new_tokens), stack.max_seq - len(req.prompt)))
+        ids.append((req.prompt, gen.submit(req)))
+    res = gen.run()
+    return [prompt + res[rid].tokens for prompt, rid in ids]

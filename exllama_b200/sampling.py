@@ -1,5 +1,6 @@
 """Token sampling on the device: the generator's repetition penalty, bos mask, temperature, top-k, top-p (with min-p) and typical
-filters and the draw, for every row of a logits batch in one launch (csrc/sample.cu, include/exl_b200.h exl_sample).
+filters and the draw, for every row of a logits batch in one launch (csrc/sample.cu, include/exl_b200.h exl_sample, and
+exl_sample_rows when each row has its own settings).
 
     tokens, probs = sampling.sample(logits, sampling.Settings(), history=ids, hist_lens=lens, bos_token_id=1)
 
@@ -49,9 +50,29 @@ def params(settings: Settings, dev, bos_token_id=None, banned=None):
     return p, ban
 
 
-def sample(logits, settings: Settings, history=None, hist_lens=None, u=None, generator=None, bos_token_id=None, banned=None,
-           dist=None):
+def row_params(settings, bsz, dev, bos_token_id=None, banned=None):
+    """(a ctypes array of bsz exl_sample_params, the banned tensors to keep alive) for exl_sample_rows: settings is a list of bsz
+    Settings; bos_token_id None, one id for every row, or a list of bsz (None or an id); banned None or a list of bsz (None or ids)."""
+    settings = list(settings)
+    if len(settings) != bsz:
+        raise ValueError(f"sample: {len(settings)} settings for {bsz} rows")
+    bos = bos_token_id if isinstance(bos_token_id, (list, tuple)) else [bos_token_id] * bsz
+    ban = [None] * bsz if banned is None else list(banned)
+    if len(bos) != bsz or len(ban) != bsz:
+        raise ValueError(f"sample: {len(bos)} bos ids and {len(ban)} banned lists for {bsz} rows")
+    arr = (capi.ExlSampleParams * bsz)()
+    keep = []
+    for b in range(bsz):
+        arr[b], t = params(settings[b], dev, bos[b], ban[b])
+        keep.append(t)
+    return arr, keep
+
+
+def sample(logits, settings, history=None, hist_lens=None, u=None, generator=None, bos_token_id=None, banned=None, dist=None):
     """One token per row of logits [bsz, vocab] fp32 (CUDA, unit stride along vocab; left unchanged).
+
+    settings  a Settings for every row (exl_sample), or a list of bsz Settings, row b using settings[b] (exl_sample_rows); with a
+              list, bos_token_id may also be a list of bsz ids (None: untouched) and banned a list of bsz id lists (None: none)
 
     history   int64 [bsz, hist_ld] token ids on the logits' device, newest last, or None (no penalty)
     hist_lens the tokens of each history row to use (host ints, default hist_ld each)
@@ -82,13 +103,18 @@ def sample(logits, settings: Settings, history=None, hist_lens=None, u=None, gen
             raise ValueError(f"sample: {len(hl)} hist_lens for {bsz} rows")
         lens = (C.c_int * bsz)(*hl)
         hist_ptr = C.c_void_p(history.data_ptr())
-    p, ban = params(settings, dev, bos_token_id, banned)
+    per_row = isinstance(settings, (list, tuple))
+    if per_row:
+        p, ban = row_params(settings, bsz, dev, bos_token_id, banned)
+    else:
+        p, ban = params(settings, dev, bos_token_id, banned)
     tokens = torch.empty(bsz, dtype=torch.int64, device=dev)
     probs = torch.empty(bsz, dtype=torch.float32, device=dev)
     if dist is not None and (dist.shape != (bsz, vocab) or dist.dtype != torch.float32 or not dist.is_contiguous()):
         raise ValueError(f"sample: dist must be contiguous fp32 [{bsz}, {vocab}], got {dist.dtype} {tuple(dist.shape)}")
     ld = logits.stride(0) if bsz > 1 else vocab          # a one-row view may carry any stride along rows
+    fn = capi.lib().exl_sample_rows if per_row else capi.lib().exl_sample
     with torch.cuda.device(dev):
-        capi.check(capi.lib().exl_sample(capi._ptr(logits), bsz, vocab, ld, hist_ptr, hist_ld, lens, C.byref(p),
-                                         capi._ptr(u), capi._ptr(tokens), capi._ptr(probs), capi._ptr(dist), capi._stream()))
+        capi.check(fn(capi._ptr(logits), bsz, vocab, ld, hist_ptr, hist_ld, lens, p if per_row else C.byref(p), capi._ptr(u),
+                      capi._ptr(tokens), capi._ptr(probs), capi._ptr(dist), capi._stream()))
     return tokens, probs

@@ -394,6 +394,14 @@ int exl_sample(const float* logits, int bsz, int vocab, int64_t logits_ld,
                const int64_t* history, int64_t hist_ld, const int* hist_len_host,
                const exl_sample_params* p, const float* u, int64_t* tokens, float* probs, float* dist, void* stream);
 
+/* exl_sample with one parameter set per row: row b uses p_rows[b] (host array of bsz entries, read during the call and carried in the
+   kernel parameters, so a captured graph replays the same call) -- its temperature, filters, penalty triple, bos id and banned list.
+   Everything else is exl_sample's, and exl_sample(..., p, ...) is this call with every p_rows[b] = *p, bitwise.  EXL_ERR_ARG as
+   exl_sample; a bad parameter set is reported with its row ("sample: row 3: top_k 0 ..."). */
+int exl_sample_rows(const float* logits, int bsz, int vocab, int64_t logits_ld,
+                    const int64_t* history, int64_t hist_ld, const int* hist_len_host,
+                    const exl_sample_params* p_rows, const float* u, int64_t* tokens, float* probs, float* dist, void* stream);
+
 /* Speculative sampling (new functionality; the reference has no speculative decoding): verify k draft tokens d_1 .. d_k of one
    sequence against the target's logits so that the emitted tokens follow exactly the target's distribution (Leviathan et al.
    2023, Chen et al. 2023).
@@ -466,6 +474,37 @@ typedef struct { int src, dst, row_lo, row_hi; } exl_kv_copy_pair;
    (src == dst included), a destination named twice, or a NULL or misaligned pointer. */
 int exl_kv_copy_rows(void* const* k_caches, void* const* v_caches, int n_layers, int num_cache_seqs, int num_kv_heads, int max_seq_len,
                      int head_dim, const exl_kv_copy_pair* pairs, int n_pairs, void* stream);
+
+/* --- batched generation (exllama_b200/csrc/generate.cu; exllama_b200/generate.py schedules requests into cache slots) ------------- */
+
+#define EXL_GEN_MAX_STOP  8   /* stop ids per slot */
+#define EXL_GEN_LIVE      0   /* slot status: still generating */
+#define EXL_GEN_STOPPED   1   /* the last token stored is one of the slot's stop ids (it is kept) */
+#define EXL_GEN_ERROR     4   /* the sampler returned -1 for the slot's row (undefined distribution) */
+
+/* The uniform of draw j of a request with seed s:
+     U(s, j) = (z >> 40) / 2^24,  z = splitmix64 output j (0-based) of the stream seeded with s:
+       x = s + (j + 1) * 0x9E3779B97F4A7C15;  x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9;  x = (x ^ (x >> 27)) * 0x94D049BB133111EB;
+       z = x ^ (x >> 31)                     (all mod 2^64)
+   exactly representable in fp32, in [0, 1).  A request's draws depend only on its seed and its token index. */
+
+/* The tail of one generation step, after exl_sample(_rows) drew tokens[rows] / probs[rows].  Row r belongs to cache slot
+   slot_host[r] (-1: the row is ignored); it is the request's token j_host[r], appended at history position pos_host[r].  Per slot s
+   (device arrays of n_slots rows): hist int64 [n_slots][hist_ld], status int32 [n_slots], stop_ids int64 [n_slots][EXL_GEN_MAX_STOP]
+   (-1 pads), seeds uint64 [n_slots]; outputs x_next fp16 [n_slots][hidden], u_next fp32 [n_slots], out_tokens int64 and out_probs
+   fp32 [n_slots][out_ld].  For each row whose slot's status is EXL_GEN_LIVE:
+     token t in [0, vocab): hist[s][pos] = t, out_tokens[s][j] = t, out_probs[s][j] = probs[r], status[s] = EXL_GEN_STOPPED if t is
+       one of stop_ids[s], x_next[s] = embed[t] (fp16 [vocab][hidden], 16-byte loads and stores), u_next[s] = U(seeds[s], j + 1);
+     else (the sampler's -1): out_tokens[s][j] = -1, out_probs[s][j] = NaN, status[s] = EXL_GEN_ERROR, nothing else.
+   A row whose slot is not live writes nothing: a non-zero status is sticky until the caller resets it.  One CTA per row, no atomics:
+   bitwise reproducible.  slot_host, pos_host and j_host are read on the host (baked into a CUDA-graph capture).
+   EXL_ERR_ARG (naming the value) for rows outside 1 .. EXL_RAGGED_MAX_SEQ, n_slots outside 1 .. EXL_RAGGED_MAX_SEQ, a slot outside
+   [-1, n_slots) or named twice, pos outside [0, hist_ld), j outside [0, out_ld), vocab < 1, hidden not a positive multiple of 8, a
+   NULL or (embed, x_next) non-16-byte-aligned pointer. */
+int exl_gen_advance(const int64_t* tokens, const float* probs, int rows, const int* slot_host, const int* pos_host, const int* j_host,
+                    int64_t* hist, int64_t hist_ld, int* status, const int64_t* stop_ids, const uint64_t* seeds, int n_slots,
+                    const void* embed, int vocab, int hidden, void* x_next, float* u_next, int64_t* out_tokens, float* out_probs,
+                    int64_t out_ld, void* stream);
 
 /* --- token log-probabilities (exllama_b200/csrc/logprob.cu; the reference: matmul + log_softmax + gather, perplexity.py:118-121) --- */
 

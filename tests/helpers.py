@@ -92,34 +92,54 @@ def oracle_mm(oracle, xin, lin, ab=None, acc=None, recons=False):
 
 
 def oracle_qkv(oracle, st, i, x, past):
-    """Layer i of a DecodeStack on the fp16 layer input x [1, hidden], as oracle_decode_step computes it: (normed x, roped fp16 q
-    [heads * hd], roped fp16 k [kv_heads, hd], fp16 v [kv_heads, hd]) of the new token at position `past`."""
+    """Layer i of a DecodeStack on the fp16 layer inputs x [n, hidden] of n consecutive tokens, token t at position past + t, as
+    oracle_decode_step computes them: (normed x [n, hidden], roped fp16 q [n, heads * hd], roped fp16 k [n, kv_heads, hd], fp16 v
+    [n, kv_heads, hd]).  One token (n = 1): q [heads * hd], k and v [kv_heads, hd]."""
     s = st.shape
     hd, heads, kvh = s.head_dim, s.heads, s.kv_heads
     sin = st.sin.view(-1, hd).cpu().numpy(); cos = st.cos.view(-1, hd).cpu().numpy()
     L = st.layers[i]
+    x = np.asarray(x, np.float16).reshape(-1, s.hidden)
+    n = x.shape[0]
     xn, _ = oracle.rms_norm(x, _np(L.ln1), s.eps)
-    q, k, v = (oracle_mm(oracle, xn, getattr(L, n), adapter_of(st, i, n)).astype(np.float16) for n in ("q", "k", "v"))
-    q = oracle.rope(q.reshape(1, heads, hd), sin, cos, 1, heads, hd, heads, past).reshape(-1)
-    k = oracle.rope(k.reshape(1, kvh, hd), sin, cos, 1, kvh, hd, kvh, past).reshape(kvh, hd)
-    return xn, q, k, v.reshape(kvh, hd)
+    q, k, v = (oracle_mm(oracle, xn, getattr(L, m), adapter_of(st, i, m)).astype(np.float16) for m in ("q", "k", "v"))
+    # the oracle's rope puts row r at position past + r // num_heads: token t's heads at past + t
+    q = oracle.rope(q.reshape(1, n * heads, hd), sin, cos, 1, n * heads, hd, heads, past).reshape(n, heads * hd)
+    k = oracle.rope(k.reshape(1, n * kvh, hd), sin, cos, 1, n * kvh, hd, kvh, past).reshape(n, kvh, hd)
+    v = v.reshape(n, kvh, hd)
+    return (xn, q[0], k[0], v[0]) if n == 1 else (xn, q, k, v)
 
 
-def oracle_decode_step(oracle, st, snap, x, past, seq=0, n_layers=None):
-    """float64/fp16 restatement of one decode token of a DecodeStack (grouped-query attention, cache sequence `seq`, the stack's
-    adapter) on the cache snapshot `snap` (per layer (key_cache, value_cache) tensors): (final hidden fp16, logits float64 or None
-    for a stack without a head, new k/v rows per layer).  n_layers: stop after that many layers (hidden state after them, no
-    logits)."""
+def causal_attn(oracle, st, q, kc, vc, past):
+    """Attention of n consecutive tokens of one sequence: q [n, heads, hd] fp16 (token t at position past + t), kc / vc [kv_heads,
+    max_seq, hd] fp16 holding the launch's own rows at past .. past + n - 1.  Token t reads rows [0, past + t]: one decode query
+    of oracle.decode_attn_f64 per token.  Returns float64 [n, heads, hd]."""
+    from prefill_oracle import prefill_attn_f64
+    s = st.shape
+    return prefill_attn_f64(oracle, q, kc, vc, s.heads, s.kv_heads, past, st.max_seq, s.head_dim)
+
+
+def oracle_decode_step(oracle, st, snap, x, past, seq=0, n_layers=None, attend=None):
+    """float64/fp16 restatement of one decode launch of a DecodeStack (grouped-query attention, cache sequence `seq`, the stack's
+    adapter) on the cache snapshot `snap` (per layer (key_cache, value_cache) tensors), with the fused step's rounding points:
+    x [n, hidden] holds n consecutive tokens, token t at position past + t.  Per layer every token's k / v rows go into rows
+    past .. past + n - 1 of a copy of the cache, then token t attends rows [0, past + t] (causal_attn).  Returns (final hidden fp16
+    [n, hidden], logits float64 [n, vocab] or None for a stack without a head, new k / v rows per layer: [kv_heads, n, hd] each, or
+    [kv_heads, hd] for one token).  n_layers: stop after that many layers (hidden state after them, no logits).  attend(l, q, kc,
+    vc): the attention of layer l in place of causal_attn (a test emulating a kernel bug)."""
     s = st.shape
     hd, heads, kvh = s.head_dim, s.heads, s.kv_heads
-    x = x.reshape(1, s.hidden).copy()
+    x = np.asarray(x, np.float16).reshape(-1, s.hidden).copy()
+    n = x.shape[0]
     rows = []
     for i, L in enumerate(st.layers):
         _, q, k, v = oracle_qkv(oracle, st, i, x, past)
+        q, k, v = q.reshape(n, heads, hd), k.reshape(n, kvh, hd), v.reshape(n, kvh, hd)
         kc = _np(snap[i][0][seq]).copy(); vc = _np(snap[i][1][seq]).copy()
-        kc[:, past] = k; vc[:, past] = v.reshape(kvh, hd)
-        rows.append((k.copy(), v.reshape(kvh, hd).copy()))
-        attn = oracle.decode_attn_f64(q, kc, vc, heads, kvh, hd, past + 1, st.max_seq).astype(np.float16).reshape(1, -1)
+        kc[:, past:past + n] = k.transpose(1, 0, 2); vc[:, past:past + n] = v.transpose(1, 0, 2)
+        rows.append((k[0].copy(), v[0].copy()) if n == 1 else (kc[:, past:past + n].copy(), vc[:, past:past + n].copy()))
+        a = causal_attn(oracle, st, q, kc, vc, past) if attend is None else attend(i, q, kc, vc)
+        attn = a.astype(np.float16).reshape(n, -1)
         x = oracle_mm(oracle, attn, L.o, adapter_of(st, i, "o"), acc=x).astype(np.float16)
         xn, _ = oracle.rms_norm(x, _np(L.ln2), s.eps)
         act = oracle.silu_mul(oracle_mm(oracle, xn, L.gate, adapter_of(st, i, "gate")).astype(np.float16),
@@ -398,6 +418,35 @@ def attn_probe_stack(shape, layers, max_seq, act=False, batch=1, seed=0, gamma=N
     return st
 
 
+def cpu_probe_stack(oracle, heads, kv, layers, max_seq, gamma=None, seed=0, batch=1):
+    """What the probe helpers read of an attn_probe_stack, on the CPU (hidden heads x 128, inter 512): q / k / v / gate / up /
+    down checkpoint-like, o the identity, ln2 = 0, no head, caches of `batch` sequences.  gamma: k = gamma q as in
+    attn_probe_stack."""
+    import torch
+    from types import SimpleNamespace
+    from exllama_b200.shapes import LlamaShape
+    from stack_harness import sincos
+    hd = 128
+    hidden, inter = heads * hd, 512
+    shape = LlamaShape("cpu-probe", hidden, inter, layers, heads, vocab=32000, kv_heads=kv)
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a))
+    lin = lambda qw, qz, sc: SimpleNamespace(qweight=t(qw), qzeros=t(qz), scales=t(sc), g_idx=None)
+    rng = np.random.default_rng(seed)
+    Ls = []
+    for i in range(layers):
+        mk = lambda K, N, j: lin(*synth_q4_ckpt(K, N, 128, seed=seed * 100 + 10 * i + j, scale=0.2)[:3])
+        L = SimpleNamespace(q=mk(hidden, hidden, 0), k=mk(hidden, kv * hd, 1), v=mk(hidden, kv * hd, 2),
+                            o=lin(*identity_q4(hidden)[:3]), gate=mk(hidden, inter, 3), up=mk(hidden, inter, 4), down=mk(inter, hidden, 5),
+                            ln1=t((1 + 0.05 * rng.standard_normal(hidden)).astype(np.float16)), ln2=t(np.zeros(hidden, np.float16)))
+        if gamma is not None:
+            L.k = lin(*scaled_q_as_k(L.q.qweight.numpy(), L.q.qzeros.numpy(), L.q.scales.numpy(), heads, kv, gamma))
+        Ls.append(L)
+    sin, cos = sincos(max_seq, hd)
+    kc = [torch.zeros((batch, kv, max_seq, hd), dtype=torch.float16) for _ in range(layers)]
+    return SimpleNamespace(shape=shape, layers=Ls, sin=t(sin), cos=t(cos), max_seq=max_seq, lora=None, lm_head=None,
+                           key_cache=kc)
+
+
 def probe_caches(st, seed):
     """Background caches for a probe stack: per layer [key_cache, value_cache] numpy fp16 [batch, kv_heads, max_seq, hd] of
     N(0, 0.25)."""
@@ -426,20 +475,97 @@ def single_positions(past):
     return sorted({p for p in c if 0 <= p < past})
 
 
-def plant_group(q, kc, vc, plants, past, s_new, rng, poison=True):
-    """Plant keys for the query heads of one KV group (numpy, in place).
+def multi_positions(past, j, m):
+    """The dense plateau of query vector j of the m = n n_rep vectors of a KV group in an n-token launch (j = t n_rep + r), each
+    disjoint from the others': m <= 8, dense_positions(past, j, m) (residues {j, 15 - j}); m <= 16, the positions p < past with
+    p mod 16 = j; m > 16 (at most 32), residue j mod 16 on the 16-position chunks of parity j // 16.  past - 1 goes to the vector
+    whose residue (and parity) holds it, or to vector 0 when no vector's does."""
+    if m <= 8:
+        return dense_positions(past, j, m)
+    assert m <= 32, m
+    p = np.arange(past)
+    own = p % 16 + (16 * (p // 16 % 2) if m > 16 else 0)
+    sel = p[own == j]
+    if past > 0 and own[-1] >= m and j == 0:
+        sel = np.append(sel, past - 1)
+    return sel
 
-    q [n_rep, hd] the heads' roped fp16 q; kc / vc [max_seq, hd] the group's cache rows of one sequence; plants[r] the positions
-    (< past) of head r's plateau, or None; s_new [n_rep] the new token's scores.  The key of head r is the least-norm k with
-    q_j . k / sqrt(hd) = T_r for j = r and 0 for the other heads of the group, T_r = max(PROBE_SCORE, 30 + every other score of
-    head r), written in fp16 at every position of plants[r], with a random +-1 V row per position.  poison: row `past` (which
-    the step overwrites with the new token) gets a key scoring POISON_LIFT above everything for every head and V = 100 x a
-    signature, and the rows past it NaN: a kernel that reads either shows it."""
+
+def lone_positions(past, m, off=0):
+    """One planted key for each of m query vectors, at distinct positions: single_positions(past) first, then evenly spread rows
+    of the context, rotated by `off`.  Entry j (None when the context has fewer rows than vectors) is vector j's plateau."""
+    single = single_positions(past)
+    spread = [p for p in np.unique(np.linspace(0, past - 1, 2 * m).astype(np.int64)).tolist() if p not in single] if past else []
+    order = single + spread
+    return [[order[(j + off) % len(order)]] if j < len(order) else None for j in range(m)]
+
+
+def multi_probe_specs(st, n, past, background=False):
+    """Plant specs (plant_probe) of an n-token launch at past_len, by name: "dense" (multi_positions), "lone+0" / "lone+3" (one
+    key per query vector, lone_positions rotated by the offset and the layer) and "newest" (each token's first query head of a
+    group answers with its own new row: a stack whose k is gamma q).  Vector j = t n_rep + r of KV group g is virtual head
+    t * heads + g * n_rep + r.  background: the odd KV groups stay unplanted (one-layer plans: a second layer would carry their
+    loose bound to every head)."""
+    heads = st.shape.heads
+    n_rep = heads // st.shape.kv_heads
+    m = n * n_rep
+
+    def vec(h):
+        t, hh = divmod(h, heads)
+        g, r = divmod(hh, n_rep)
+        return g, t * n_rep + r, r
+
+    def bg(g):
+        return background and g % 2 == 1
+    out = [("dense", lambda l, h: None if bg(vec(h)[0]) else multi_positions(past, vec(h)[1], m))]
+    for off in (0, 3):
+        out.append((f"lone+{off}", lambda l, h, off=off: None if bg(vec(h)[0]) else lone_positions(past, m, off + l)[vec(h)[1]]))
+    out.append(("newest", lambda l, h: "new" if vec(h)[2] == 0 else None))
+    return out
+
+
+def newest_inputs(oracle, st, n, past, seed, margin=PROBE_GAP + 15.0):
+    """Inputs x [n, hidden] (1e-2 N(0, 1)) of a one-layer k = gamma q stack for the "newest" layout: token by token, a draw is
+    kept when each KV group's first query head scores its own new row at least `margin` above the new rows of the tokens before
+    it.  (A q dominated by a few high-scale columns is nearly collinear with the other tokens' q, so a larger earlier q can
+    outscore the token's own row.)"""
+    s = st.shape
+    n_rep = s.heads // s.kv_heads
+    rng = np.random.default_rng(seed)
+    xs = []
+    for t in range(n):
+        for _ in range(200):
+            x = np.stack(xs + [(1e-2 * rng.standard_normal(s.hidden)).astype(np.float16)])
+            _, q, k, _ = oracle_qkv(oracle, st, 0, x, past)
+            q = q.reshape(t + 1, s.heads, s.head_dim)[t, ::n_rep].astype(np.float64)
+            k = k.reshape(t + 1, s.kv_heads, s.head_dim).astype(np.float64)
+            sc = np.einsum("gd,jgd->gj", q, k) / np.sqrt(s.head_dim)
+            if (sc[:, t:] - margin >= sc[:, :t].max(1, initial=-np.inf)[:, None]).all():
+                xs.append(x[t])
+                break
+        else:
+            raise AssertionError(f"no input for token {t} lets its own row dominate")
+    return np.stack(xs)
+
+
+def plant_group(q, kc, vc, plants, past, s_new, rng, poison=True):
+    """Plant keys for the query vectors of one KV group (numpy, in place).
+
+    q [m, hd] the group's roped fp16 query vectors: the n_rep heads of one token, or for a launch of n tokens m = n n_rep vectors,
+    vector j = t n_rep + r token t's head r; kc / vc [max_seq, hd] the group's cache rows of one sequence; plants[j] the positions
+    (< past) of vector j's plateau, or None; s_new [m] or [m, n] the vectors' scores against the launch's n new rows.  The key
+    of vector r is the least-norm k with q_j . k / sqrt(hd) = T_r for j = r and 0 for the other vectors of the group, T_r =
+    max(PROBE_SCORE, 30 + every other score of vector r, the new rows' included), written in fp16 at every position of
+    plants[r], with a random +-1 V row per position.  poison: rows past .. past + n - 1 (which the launch overwrites with its new
+    rows) get a key scoring POISON_LIFT above everything for every vector and V = 100 x a signature, and the rows from past + n
+    on NaN: a kernel that reads either shows it."""
     hd = q.shape[1]
     Q = q.astype(np.float64)
     G = Q @ Q.T
+    s_new = np.asarray(s_new, np.float64).reshape(len(Q), -1)
+    n = s_new.shape[1]
     bg = (kc[:past].astype(np.float64) @ Q.T).max(0) / np.sqrt(hd) if past > 0 else np.full(len(Q), -np.inf)
-    top = np.maximum(bg, s_new)
+    top = np.maximum(bg, s_new.max(1))
     tmax = top.max()
     for r, P in enumerate(plants):
         if P is None or len(P) == 0:
@@ -453,10 +579,12 @@ def plant_group(q, kc, vc, plants, past, s_new, rng, poison=True):
         vc[P] = rng.choice([-1.0, 1.0], (len(P), hd)).astype(np.float16)
     if poison and past < kc.shape[0]:
         t = np.full(len(Q), (tmax + POISON_LIFT) * np.sqrt(hd))
-        kc[past] = (Q.T @ np.linalg.solve(G, t)).astype(np.float16)
-        assert np.isfinite(kc[past]).all(), "poison key overflows fp16"
-        vc[past] = 100 * rng.choice([-1.0, 1.0], hd).astype(np.float16)
-        kc[past + 1:] = np.nan; vc[past + 1:] = np.nan
+        key = (Q.T @ np.linalg.solve(G, t)).astype(np.float16)
+        assert np.isfinite(key).all(), "poison key overflows fp16"
+        for p in range(past, min(past + n, kc.shape[0])):
+            kc[p] = key
+            vc[p] = 100 * rng.choice([-1.0, 1.0], hd).astype(np.float16)
+        kc[past + n:] = np.nan; vc[past + n:] = np.nan
 
 
 def snap_of(caches):
@@ -465,36 +593,43 @@ def snap_of(caches):
 
 
 def plant_probe(oracle, st, caches, x, past, spec, seed, seq=0, poison=True):
-    """Plant every layer of cache sequence `seq` of a probe stack (caches from probe_caches, modified in place), layer by layer:
-    layer l's q depends on the layers below, so they are planted first.  spec(l, h) -> positions of head h's plateau, "new" (the
-    new token dominates: nothing to plant) or None (background).  Returns plants[l] = {head: positions} for probe_expectation."""
+    """Plant every layer of cache sequence `seq` of a probe stack (caches from probe_caches, modified in place) for the launch of
+    x [n, hidden] (token t at position past + t), layer by layer: layer l's q depends on the layers below, so they are planted
+    first.  Query heads are virtual, as the multi-token step numbers them: h = t * heads + h' is token t's query head h' (for one
+    token h = h').  spec(l, h) -> positions of head h's plateau, "new" (the token's own new row, past + t, dominates: nothing to
+    plant) or None (background).  Returns plants[l] = {virtual head: positions} for probe_expectation."""
     s = st.shape
     hd, heads, kvh = s.head_dim, s.heads, s.kv_heads
     n_rep = heads // kvh
     rng = np.random.default_rng(seed)
+    x = np.asarray(x, np.float16).reshape(-1, s.hidden)
+    n = x.shape[0]
     out = []
     for l in range(len(st.layers)):
-        xl = np.asarray(x, np.float16).reshape(1, -1)
+        xl = x
         if l > 0:
             xl = oracle_decode_step(oracle, st, snap_of(caches), x, past, seq, n_layers=l)[0]
         _, q, k, _ = oracle_qkv(oracle, st, l, xl, past)
-        q = q.reshape(heads, hd)
+        q = q.reshape(n, heads, hd); k = k.reshape(n, kvh, hd)
         pl = {}
         for g in range(kvh):
-            qg = q[g * n_rep:(g + 1) * n_rep]
-            s_new = qg.astype(np.float64) @ k[g].astype(np.float64) / np.sqrt(hd)
+            qg = q[:, g * n_rep:(g + 1) * n_rep].reshape(n * n_rep, hd)
+            q64 = qg.astype(np.float64)
+            s_new = np.stack([q64 @ k[t, g].astype(np.float64) for t in range(n)], 1) / np.sqrt(hd)
             ps = []
-            for r in range(n_rep):
-                P = spec(l, g * n_rep + r)
+            for j in range(n * n_rep):
+                t, r = divmod(j, n_rep)
+                hv = t * heads + g * n_rep + r
+                P = spec(l, hv)
                 if isinstance(P, str):
                     assert P == "new"
-                    pl[g * n_rep + r] = np.array([past])
+                    pl[hv] = np.array([past + t])
                     P = None
                 elif P is not None:
                     taken = np.concatenate([np.zeros(0, np.int64)] + [p for p in ps if p is not None])
-                    P = np.setdiff1d(np.asarray(P, np.int64), taken)          # a position serves one head of the group
+                    P = np.setdiff1d(np.asarray(P, np.int64), taken)          # a position serves one vector of the group
                     if len(P):
-                        pl[g * n_rep + r] = P
+                        pl[hv] = P
                     else:
                         P = None
                 ps.append(P)
@@ -516,24 +651,28 @@ def _rope_err(v, e, sin_row, cos_row):
 
 
 def probe_expectation(oracle, st, snap, x, past, plants, kind, seq=0, o_prop=False):
-    """(want, bound): the oracle's final hidden state of a probe stack (oracle_decode_step on the cache snapshot) and a float64
-    bound B >= |kernel - want| per element.
+    """(want, bound): the oracle's final hidden state of a probe stack (oracle_decode_step on the cache snapshot) for the launch
+    of x [n, hidden] (token t at position past + t) and a float64 bound B >= |kernel - want| per element: [n, hidden] each, or
+    [hidden] for one token.
 
-    Per layer, with the layer input known to within bx (0 for layer 0):
+    Per layer and token t, with the layer input known to within bx (0 for layer 0):
       q, k, v  The GEMV error is quant_error_bound(kind) of each projection, plus the oracle's own fp16 rounding 2^-11 |ref|,
                plus the effect of a perturbed input: rms norm moves xn by at most |w| rm (bx + |x| rms(bx) / rms(x)) + 2 ulps,
                contracted with |W| (adapters: the same for x . A, a rounding of x . A, and the 16-bit x grid, contracted with
-               |B|).  Rope adds the propagated error and 2 fp16 ulps (_rope_err): Dq, Dk, Dv.
-      scores   A score q . k_p / sqrt(hd) moves by at most delta_h = max(sum_d Dq_d max_p |k_pd|, sum_d Dq_d |kn_d| +
-               (|q_d| + Dq_d) Dk_d) / sqrt(hd) (cached rows hold the same bits in kernel and oracle; kn is the new token's
-               k), plus 2^-20 of sum_d |q_d| max_p |k_pd| / sqrt(hd) for the fp32 dot product and scale.
+               |B|).  Rope at position past + t adds the propagated error and 2 fp16 ulps (_rope_err): Dq, Dk, Dv.
+      scores   Token t reads the cached rows [0, past) and the launch's new rows j = 0 .. t (kn_j, token j's k).  A score
+               q . k_p / sqrt(hd) moves by at most delta_h = max(sum_d Dq_d max_p |k_pd|, max_j sum_d Dq_d |kn_jd| + (|q_d| +
+               Dq_d) Dk_jd) / sqrt(hd) (cached rows hold the same bits in kernel and oracle), plus 2^-20 of sum_d |q_d| max_p
+               |k_pd| / sqrt(hd) for the fp32 dot product and scale.
       softmax  Scores within delta of the oracle's move every weight by a factor in [e^-2delta, e^2delta], so the output moves by
-               at most (e^{2 delta} - 1) max|V| (and never more than 2 max|V|: both are averages of the same rows).  A planted head (plants[l][h] = P) whose P scores at least gap above every
-               other position has its answer within 2 n e^{-(gap - 2 delta)} max|V| of the mean of V over P in both kernel and
-               oracle (n = past + 1 positions): that bound is used instead, and the setup asserts gap >= PROBE_GAP.  At past = 0 the
-               new row is the only one and has weight 1.  Add Dv of
-               the new row times the most weight it can have (1, or n e^{-(gap - 2 delta)} when it is off the plateau), and (past / 16 + 64) 2^-23 max|V| for fp32 accumulation along a chain of at most past / 16 + 64
-               additions and the exponential approximations.
+               at most (e^{2 delta} - 1) max|V| (and never more than 2 max|V|: both are averages of the same rows).  A planted
+               head (plants[l][h] = P, h the virtual head t * heads + h') whose P scores at least gap above every other position
+               has its answer within 2 n e^{-(gap - 2 delta)} max|V| of the mean of V over P in both kernel and oracle (n = past
+               + t + 1 positions): that bound is used instead, and the setup asserts gap >= PROBE_GAP.  At past = 0 token 0's
+               own row is the only one and has weight 1.  Add the largest Dv of the new rows 0 .. t times the most weight they
+               can have (1, or n e^{-(gap - 2 delta)} when they are off the plateau), and (past / 16 + 64) 2^-23 max|V| for fp32
+               accumulation along a chain of at most past / 16 + 64 additions and the exponential approximations (the causal
+               tail adds at most 4 to the chain).
       o_proj   Two fp16 roundings of the attention output, then the identity o GEMV's x quantisation: quant_error_bound(kind)
                of the identity at an upper bound of |attention| (segments: group and 128-k stage, so a head under plain order).
                o_prop: o_proj is any matrix (no adapter): the attention bound goes through |W_o| instead of unchanged, and the
@@ -543,82 +682,92 @@ def probe_expectation(oracle, st, snap, x, past, plants, kind, seq=0, o_prop=Fal
     s = st.shape
     hd, heads, kvh = s.head_dim, s.heads, s.kv_heads
     n_rep = heads // kvh
-    sin = st.sin.view(-1, hd).cpu().numpy()[past]; cos = st.cos.view(-1, hd).cpu().numpy()[past]
-    x = np.asarray(x, np.float16).reshape(1, -1)
+    sin = st.sin.view(-1, hd).cpu().numpy(); cos = st.cos.view(-1, hd).cpu().numpy()
+    x = np.asarray(x, np.float16).reshape(-1, s.hidden)
+    n = x.shape[0]
     want, _, rows = oracle_decode_step(oracle, st, snap, x, past, seq)
     xs = [x] + [oracle_decode_step(oracle, st, snap, x, past, seq, n_layers=l)[0] for l in range(1, len(st.layers))] + [want]
-    bx = np.zeros(s.hidden)
+    bx = np.zeros((n, s.hidden))
     sq = np.sqrt(hd)
     for l, L in enumerate(st.layers):
-        xl = xs[l].astype(np.float64).reshape(-1)
         xn, q, k, v = oracle_qkv(oracle, st, l, xs[l], past)
-        xn64 = xn.astype(np.float64).reshape(-1)
+        q, k = q.reshape(n, heads, hd), k.reshape(n, kvh, hd)
+        xn64 = xn.astype(np.float64)
         dxn = None
         if bx.any():
             w = np.abs(_np(L.ln1).astype(np.float64))
-            r = np.sqrt(np.mean(xl * xl) + s.eps)
-            dxn = 1.01 * (w / r * (bx + np.abs(xl) * (np.sqrt(np.mean(bx * bx)) / r + 2.0 ** -9)) + 2.0 ** -9 * np.abs(xn64))
+            dxn = np.empty((n, s.hidden))
+            for t in range(n):
+                xl = xs[l][t].astype(np.float64)
+                r = np.sqrt(np.mean(xl * xl) + s.eps)
+                dxn[t] = 1.01 * (w / r * (bx[t] + np.abs(xl) * (np.sqrt(np.mean(bx[t] * bx[t])) / r + 2.0 ** -9)) +
+                                 2.0 ** -9 * np.abs(xn64[t]))
 
         def proj_err(name):
             lin = getattr(L, name)
             xm = None if lin.g_idx is None else oracle.make_x_map(lin.g_idx.numpy(), lin.qzeros.shape[0])
             qw, qz, sc = _np(lin.qweight), _np(lin.qzeros), _np(lin.scales)
             B, ref = quant_error_bound(oracle, xn, qw, qz, sc, xm, kind)
-            e = B[0] + 2.0 ** -11 * np.abs(ref[0]) + FP16_TINY
+            e = B + 2.0 ** -11 * np.abs(ref) + FP16_TINY
             if dxn is not None:
                 W = np.abs(oracle.dequant_f64(qw, qz, sc))
-                e = e + 1.01 * ((dxn if xm is None else dxn[np.asarray(xm, np.int64)]) @ W)
+                e = e + 1.01 * np.stack([(d if xm is None else d[np.asarray(xm, np.int64)]) @ W for d in dxn])
             ab = adapter_of(st, l, name)
             if ab is not None:
                 A, Bm = (np.abs(_np(t).astype(np.float64)) for t in ab)
-                ex = 2.0 ** -9 * np.abs(xn64) + np.abs(xn64).max() / QUANT_Q["step"] + (0 if dxn is None else dxn)
-                t16 = np.abs(oracle.half_matmul_f64(xn, _np(ab[0])))
-                e = e + 1.01 * ((ex @ A + 2.0 ** -10 * t16[0]) @ Bm) + 2.0 ** -10 * (t16[0] @ Bm)
+                for t in range(n):
+                    ex = 2.0 ** -9 * np.abs(xn64[t]) + np.abs(xn64[t]).max() / QUANT_Q["step"] + (0 if dxn is None else dxn[t])
+                    t16 = np.abs(oracle.half_matmul_f64(xn[t:t + 1], _np(ab[0])))
+                    e[t] = e[t] + 1.01 * ((ex @ A + 2.0 ** -10 * t16[0]) @ Bm) + 2.0 ** -10 * (t16[0] @ Bm)
             return e
         eq, ek, ev = proj_err("q"), proj_err("k"), proj_err("v")
-        q = q.reshape(heads, hd)
-        dq = _rope_err(q, eq.reshape(heads, hd), sin, cos)
-        dk = _rope_err(k, ek.reshape(kvh, hd), sin, cos)
-        dv = ev.reshape(kvh, hd)
+        dq = [_rope_err(q[t], eq[t].reshape(heads, hd), sin[past + t], cos[past + t]) for t in range(n)]
+        dk = [_rope_err(k[t], ek[t].reshape(kvh, hd), sin[past + t], cos[past + t]) for t in range(n)]
+        dv = [ev[t].reshape(kvh, hd) for t in range(n)]
         kc = _np(snap[l][0][seq]).copy(); vc = _np(snap[l][1][seq]).copy()
-        kc[:, past] = rows[l][0]; vc[:, past] = rows[l][1]
-        attn = oracle.decode_attn_f64(q.reshape(-1), kc, vc, heads, kvh, hd, past + 1, st.max_seq).reshape(heads, hd)
-        K = kc[:, :past + 1].astype(np.float64); V = vc[:, :past + 1].astype(np.float64)
-        q64 = q.astype(np.float64)
-        bh = np.zeros(heads)
-        for h in range(heads):
-            g = h // n_rep
-            kmax = np.abs(K[g]).max(0)
-            kold = np.abs(K[g, :past]).max(0) if past > 0 else np.zeros(hd)
-            kn = np.abs(K[g, past])
-            delta = max(dq[h] @ kold, dq[h] @ kn + (np.abs(q64[h]) + dq[h]) @ dk[g]) / sq
-            delta = delta * (1 + 2.0 ** -10) + 2.0 ** -20 * (np.abs(q64[h]) @ kmax) / sq
-            vmax = np.abs(V[g]).max() + dv[g].max()
-            P = plants[l].get(h) if plants is not None else None
-            if P is not None:
-                sc_h = K[g] @ q64[h] / sq
-                inP = np.zeros(past + 1, bool); inP[P] = True
-                assert len(set(sc_h[inP].tolist())) == 1 or P.tolist() == [past], f"layer {l} head {h}: planted keys differ"
-                gap = sc_h[inP].min() - sc_h[~inP].max() if (~inP).any() else np.inf
-                assert gap >= PROBE_GAP, f"layer {l} head {h}: plateau only {gap:.2f} above the other scores"
-                w_off = min(1.0, (past + 1) * np.exp(min(50.0, 2 * delta - gap))) if np.isfinite(gap) else 0.0
-                t = 2 * w_off * vmax + dv[g].max() * (1.0 if inP[past] else w_off)
-            elif past == 0:
-                t = dv[g].max()                                   # one row: weight 1 whatever the scores
-            else:
-                t = min(2.0, np.expm1(min(50.0, 2 * delta))) * vmax + dv[g].max()
-            bh[h] = t + (past / 16 + 64) * 2.0 ** -23 * vmax
-        battn = (bh[:, None] + 2.0 ** -10 * np.abs(attn) + 2 * FP16_TINY).reshape(-1)
+        kc[:, past:past + n] = rows[l][0].reshape(kvh, n, hd); vc[:, past:past + n] = rows[l][1].reshape(kvh, n, hd)
+        attn = causal_attn(oracle, st, q, kc, vc, past)
+        battn = np.empty((n, s.hidden))
+        for t in range(n):
+            npos = past + t + 1
+            K = kc[:, :npos].astype(np.float64); V = vc[:, :npos].astype(np.float64)
+            q64 = q[t].astype(np.float64)
+            bh = np.zeros(heads)
+            for h in range(heads):
+                g = h // n_rep
+                kmax = np.abs(K[g]).max(0)
+                kold = np.abs(K[g, :past]).max(0) if past > 0 else np.zeros(hd)
+                dnew = [dq[t][h] @ np.abs(K[g, past + j]) + (np.abs(q64[h]) + dq[t][h]) @ dk[j][g] for j in range(t + 1)]
+                delta = max([dq[t][h] @ kold] + dnew) / sq
+                delta = delta * (1 + 2.0 ** -10) + 2.0 ** -20 * (np.abs(q64[h]) @ kmax) / sq
+                dvn = max(dv[j][g].max() for j in range(t + 1))
+                vmax = np.abs(V[g]).max() + dvn
+                P = plants[l].get(t * heads + h) if plants is not None else None
+                if P is not None:
+                    sc_h = K[g] @ q64[h] / sq
+                    inP = np.zeros(npos, bool); inP[P] = True
+                    assert len(set(sc_h[inP].tolist())) == 1 or P.tolist() == [past + t], f"layer {l} token {t} head {h}: planted keys differ"
+                    gap = sc_h[inP].min() - sc_h[~inP].max() if (~inP).any() else np.inf
+                    assert gap >= PROBE_GAP, f"layer {l} token {t} head {h}: plateau only {gap:.2f} above the other scores"
+                    w_off = min(1.0, npos * np.exp(min(50.0, 2 * delta - gap))) if np.isfinite(gap) else 0.0
+                    b = 2 * w_off * vmax + dvn * (1.0 if inP[past:].any() else w_off)
+                elif past == 0 and t == 0:
+                    b = dvn                                       # one row: weight 1 whatever the scores
+                else:
+                    b = min(2.0, np.expm1(min(50.0, 2 * delta))) * vmax + dvn
+                bh[h] = b + (past / 16 + 64) * 2.0 ** -23 * vmax
+            battn[t] = (bh[:, None] + 2.0 ** -10 * np.abs(attn[t]) + 2 * FP16_TINY).reshape(-1)
+        attn = attn.reshape(n, -1)
         lin = L.o
         xm = None if lin.g_idx is None else oracle.make_x_map(lin.g_idx.numpy(), lin.qzeros.shape[0])
-        amax = ((np.abs(attn).reshape(-1) + battn) * (1 + 2.0 ** -9)).astype(np.float16)
-        Bo, _ = quant_error_bound(oracle, amax[None], _np(lin.qweight), _np(lin.qzeros), _np(lin.scales), xm, kind)
+        amax = ((np.abs(attn) + battn) * (1 + 2.0 ** -9)).astype(np.float16)
+        Bo, _ = quant_error_bound(oracle, amax, _np(lin.qweight), _np(lin.qzeros), _np(lin.scales), xm, kind)
         if o_prop:
             assert adapter_of(st, l, "o") is None, "o_prop carries no adapter on o"
-            battn = (battn if xm is None else battn[np.asarray(xm, np.int64)]) @ np.abs(
-                oracle.dequant_f64(_np(lin.qweight), _np(lin.qzeros), _np(lin.scales)))
-        bx = bx + battn + Bo[0] + 2.0 ** -10 * np.abs(xs[l + 1].astype(np.float64).reshape(-1)) + 2 * FP16_TINY
-    return want.reshape(-1), bx
+            Wo = np.abs(oracle.dequant_f64(_np(lin.qweight), _np(lin.qzeros), _np(lin.scales)))
+            battn = np.stack([(b if xm is None else b[np.asarray(xm, np.int64)]) @ Wo for b in battn])
+        bx = bx + battn + Bo + 2.0 ** -10 * np.abs(xs[l + 1].astype(np.float64)) + 2 * FP16_TINY
+    return (want.reshape(-1), bx[0]) if n == 1 else (want, bx)
 
 
 class RefLib:

@@ -1,12 +1,10 @@
 """The attention probe's construction (tests/helpers.py, "Attention probe") checked with the float64 oracle alone, so that a
 failure of tests/test_gpu_decode_attn_probe.py points at a kernel, not at the harness."""
-from types import SimpleNamespace
-
 import numpy as np
 import pytest
 
-from helpers import (PROBE_GAP, dense_positions, identity_q4, plant_group, plant_probe, probe_expectation, scaled_q_as_k,
-                     single_positions, snap_of, synth_q4_ckpt)
+from helpers import (PROBE_GAP, cpu_probe_stack as _cpu_stack, dense_positions, identity_q4, plant_group, plant_probe,
+                     probe_expectation, scaled_q_as_k, single_positions, snap_of, synth_q4_ckpt)
 from stack_harness import sincos
 
 
@@ -76,33 +74,7 @@ def test_planted_cache_answer_is_plateau_mean(oracle, n_rep, past, layout):
         assert np.abs(got[h] - mean).max() <= margin, (h, np.abs(got[h] - mean).max(), margin)
 
 
-# ---- the whole probe on a CPU stand-in of a DecodeStack ------------------------------------------------------------------------
-def _cpu_stack(oracle, heads, kv, layers, max_seq, gamma=None, seed=0):
-    """What the probe helpers read of a DecodeStack, on the CPU: q / k / v / gate / up / down checkpoint-like, o the identity,
-    ln2 = 0, no head."""
-    import torch
-    from exllama_b200.shapes import LlamaShape
-    hd = 128
-    hidden, inter = heads * hd, 512
-    shape = LlamaShape("cpu-probe", hidden, inter, layers, heads, vocab=32000, kv_heads=kv)
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a))
-    lin = lambda qw, qz, sc: SimpleNamespace(qweight=t(qw), qzeros=t(qz), scales=t(sc), g_idx=None)
-    rng = np.random.default_rng(seed)
-    Ls = []
-    for i in range(layers):
-        mk = lambda K, N, j: lin(*synth_q4_ckpt(K, N, 128, seed=seed * 100 + 10 * i + j, scale=0.2)[:3])
-        L = SimpleNamespace(q=mk(hidden, hidden, 0), k=mk(hidden, kv * hd, 1), v=mk(hidden, kv * hd, 2),
-                            o=lin(*identity_q4(hidden)[:3]), gate=mk(hidden, inter, 3), up=mk(hidden, inter, 4), down=mk(inter, hidden, 5),
-                            ln1=t((1 + 0.05 * rng.standard_normal(hidden)).astype(np.float16)), ln2=t(np.zeros(hidden, np.float16)))
-        if gamma is not None:
-            L.k = lin(*scaled_q_as_k(L.q.qweight.numpy(), L.q.qzeros.numpy(), L.q.scales.numpy(), heads, kv, gamma))
-        Ls.append(L)
-    sin, cos = sincos(max_seq, hd)
-    kc = [torch.zeros((1, kv, max_seq, hd), dtype=torch.float16) for _ in range(layers)]
-    return SimpleNamespace(shape=shape, layers=Ls, sin=t(sin), cos=t(cos), max_seq=max_seq, lora=None, lm_head=None,
-                           key_cache=kc)
-
-
+# ---- the whole probe on a CPU stand-in of a DecodeStack (helpers.cpu_probe_stack) ------------------------------------------
 @pytest.mark.parametrize("heads,kv", [(2, 2), (4, 1)])
 def test_probe_bound_is_tight_and_sees_a_dropped_chunk(oracle, heads, kv):
     """probe_expectation on planted caches: the bound of a planted head is far below what one 16-position chunk read as

@@ -35,6 +35,14 @@ class ExlSampleParams(C.Structure):
                 ("rep_penalty_max", f32), ("rep_sustain", i32), ("rep_decay", i32), ("bos_token_id", i32),
                 ("banned", vp), ("n_banned", i32)]
 
+CFG_MAX_PAIRS = 32                              # EXL_CFG_MAX_PAIRS
+
+
+class ExlCfgPair(C.Structure):
+    """exl_cfg_pair: logits rows a and b mixed with weight alpha, penalised with the triple."""
+    _fields_ = [("a", i32), ("b", i32), ("alpha", C.c_double), ("rep_penalty_max", f32), ("rep_sustain", i32), ("rep_decay", i32)]
+
+
 GEN_MAX_STOP = 8                                # EXL_GEN_MAX_STOP
 GEN_LIVE, GEN_STOPPED, GEN_ERROR = 0, 1, 4      # EXL_GEN_LIVE / EXL_GEN_STOPPED / EXL_GEN_ERROR
 
@@ -92,6 +100,7 @@ SIGNATURES = {
     "exl_apply_rep_penalty": (i32, [i32, vp, f32, i32, i32, i32, vp]),
     "exl_sample": (i32, [vp, i32, i32, i64, vp, i64, C.POINTER(i32), C.POINTER(ExlSampleParams), vp, vp, vp, vp, vp]),
     "exl_sample_rows": (i32, [vp, i32, i32, i64, vp, i64, C.POINTER(i32), C.POINTER(ExlSampleParams), vp, vp, vp, vp, vp]),
+    "exl_cfg_mix": (i32, [vp, i32, i32, i64, vp, i64, C.POINTER(i32), C.POINTER(ExlCfgPair), i32, vp]),
     "exl_gen_advance": (i32, [vp, vp, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), vp, i64, vp, vp, vp, i32, vp, i32, i32, vp, vp,
                               vp, vp, i64, vp]),
     "exl_spec_verify": (i32, [vp, i32, i32, i64, vp, vp, i64, vp, i32, C.POINTER(ExlSampleParams), vp, vp, vp, vp, vp, vp]),

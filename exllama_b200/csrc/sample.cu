@@ -39,16 +39,6 @@ struct SampleArgs {
 static_assert(sizeof(RowParams) == 48, "RowParams layout");
 static_assert(sizeof(SampleArgs) <= 4096, "SampleArgs must fit the classic 4 KB kernel parameter space");
 
-__device__ float penalty_value(const Shared& sh, long long j, long long s0, float dv)
-{
-    long long k = j - s0;
-    if (k <= 0) return sh.vtab[0];
-    if (k < SP_VTAB) return sh.vtab[k];
-    float v = sh.vtab[SP_VTAB - 1];
-    for (long long i = SP_VTAB - 1; i < k; i++) v += dv;
-    return v;
-}
-
 __global__ void __cluster_dims__(SP_CL, 1, 1) __launch_bounds__(SP_THREADS, 1) sample_kernel(const __grid_constant__ SampleArgs a)
 {
     extern __shared__ __align__(16) float s_row[];
@@ -65,41 +55,16 @@ __global__ void __cluster_dims__(SP_CL, 1, 1) __launch_bounds__(SP_THREADS, 1) s
 
     // 1. repetition penalty: newest window position of each token of the slice
     const bool pen = a.hist != nullptr && rs.pmax != 1.0f && a.hist_len[row] > 0;
-    long long s0 = 0, W = 0;
+    long long s0 = 0;
     const float dv = rs.decay ? (1.0f - rs.pmax) / (float)rs.decay : 0.0f;
-    if (pen) {
-        const long long len = a.hist_len[row];
-        s0 = rs.sustain == -1 ? len : rs.sustain;
-        const long long beg = max(0LL, len - s0 - rs.decay);
-        W = len - beg;
-        for (int i = threadIdx.x; i < n; i += SP_THREADS) s_int[i] = INT_MAX;
-        if (threadIdx.x == 0) {
-            const long long kmax = min((long long)SP_VTAB - 1, max(0LL, W - 1 - s0));
-            float v = rs.pmax;
-            sh.vtab[0] = v;
-            for (long long k = 1; k <= kmax; k++) { v += dv; sh.vtab[k] = v; }
-        }
-        __syncthreads();
-        const int64_t* h = a.hist + (int64_t)row * a.hist_ld;
-        for (long long j = threadIdx.x; j < W; j += SP_THREADS) {
-            const long long pos = len - 1 - j;
-            const int64_t t = a.tail && pos >= a.tail_at ? a.tail[pos - a.tail_at] : h[pos];
-            if (t < 0 || t >= a.vocab) { bad = 1; continue; }
-            if (t >= lo && t < lo + n) atomicMin(&s_int[t - lo], (int)j);
-        }
-        __syncthreads();
-    }
+    if (pen)
+        s0 = penalty_scan(sh, s_int, a.hist + (int64_t)row * a.hist_ld, a.tail, a.tail_at, a.hist_len[row], rs.pmax, rs.sustain, rs.decay,
+                          dv, a.vocab, lo, n, bad);
     // 2. penalised logits, bos, banned
     const float* lg = a.logits + (int64_t)row * a.ld + lo;
     for (int i = threadIdx.x; i < n; i += SP_THREADS) {
         float x = lg[i];
-        if (pen) {
-            const int j = s_int[i];
-            if (j != INT_MAX) {
-                const float v = penalty_value(sh, j, s0, dv);
-                x = x > 0.0f ? __fdiv_rn(x, v) : x * v;
-            }
-        }
+        if (pen) x = penalise(sh, x, s_int[i], s0, dv);
         if (lo + i == rs.bos) x = -10000.0f;
         s_row[i] = x;
     }

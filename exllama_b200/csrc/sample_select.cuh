@@ -1,4 +1,4 @@
-// sample_select.cuh -- the sampler's order keys and radix selector (csrc/sample.cu), shared with csrc/beam.cu.
+// sample_select.cuh -- the sampler's order keys, radix selector and repetition penalty (csrc/sample.cu), shared with csrc/beam.cu and csrc/cfg.cu.
 //
 // One thread-block cluster of SP_CL CTAs per row; CTA r keeps the slice [r * slice, (r + 1) * slice) of the row in shared memory.
 // Tokens are ordered by 50-bit keys (the float's bits above the inverted token id, so keys are unique and a tie goes to the lower
@@ -128,6 +128,55 @@ __device__ unsigned cluster_sum_c(Shared& sh, int& ph, unsigned v)
     Part p{}; p.c = block_sum_c(v, sh);
     cluster_exchange(sh, ph, p, [](const Part* ps, Part& o) { unsigned s = 0; for (int r = 0; r < SP_CL; r++) s += ps[r].c; o.c = s; });
     return sh.bc.c;
+}
+
+// ---- the repetition penalty of one row (apply_rep_penalty_cpu, bit-exact with exl_apply_rep_penalty), used by csrc/sample.cu and
+// csrc/cfg.cu.  penalty_scan leaves in s_int[i] the newest position j (0 = newest) in the history window of token lo + i of the slice
+// (INT_MAX: not in the window) and in sh.vtab the first SP_VTAB factors of the fp32 recurrence v += dv; it sets bad for a history
+// id outside [0, vocab) and returns s0, the sustain length.  h is the row's history, len its length (> 0); positions >= tail_at
+// read tail[pos - tail_at] when tail is not NULL.  Ends with a block barrier.
+__device__ __forceinline__ long long penalty_scan(Shared& sh, int* s_int, const int64_t* h, const int64_t* tail, long long tail_at,
+                                                  long long len, float pmax, int sustain, int decay, float dv, int vocab, int lo, int n,
+                                                  int& bad)
+{
+    const long long s0 = sustain == -1 ? len : sustain;
+    const long long beg = max(0LL, len - s0 - decay);
+    const long long W = len - beg;
+    for (int i = threadIdx.x; i < n; i += SP_THREADS) s_int[i] = INT_MAX;
+    if (threadIdx.x == 0) {
+        const long long kmax = min((long long)SP_VTAB - 1, max(0LL, W - 1 - s0));
+        float v = pmax;
+        sh.vtab[0] = v;
+        for (long long k = 1; k <= kmax; k++) { v += dv; sh.vtab[k] = v; }
+    }
+    __syncthreads();
+    for (long long j = threadIdx.x; j < W; j += SP_THREADS) {
+        const long long pos = len - 1 - j;
+        const int64_t t = tail && pos >= tail_at ? tail[pos - tail_at] : h[pos];
+        if (t < 0 || t >= vocab) { bad = 1; continue; }
+        if (t >= lo && t < lo + n) atomicMin(&s_int[t - lo], (int)j);
+    }
+    __syncthreads();
+    return s0;
+}
+
+// the factor at window position j (penalty_scan's s_int entry)
+__device__ __forceinline__ float penalty_value(const Shared& sh, long long j, long long s0, float dv)
+{
+    long long k = j - s0;
+    if (k <= 0) return sh.vtab[0];
+    if (k < SP_VTAB) return sh.vtab[k];
+    float v = sh.vtab[SP_VTAB - 1];
+    for (long long i = SP_VTAB - 1; i < k; i++) v += dv;
+    return v;
+}
+
+// logit x of a token at window position j (INT_MAX: none) after the penalty
+__device__ __forceinline__ float penalise(const Shared& sh, float x, int j, long long s0, float dv)
+{
+    if (j == INT_MAX) return x;
+    const float v = penalty_value(sh, j, s0, dv);
+    return x > 0.0f ? __fdiv_rn(x, v) : x * v;
 }
 
 // The row's filter state: each stage's cut (a key threshold; 0 keeps everything) and normaliser (1 until the stage has run, and for

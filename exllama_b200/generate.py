@@ -17,12 +17,20 @@ freed one step late.
 Token j of a request is what sampling.sample returns for its logits row with the request's settings, bos id and banned list,
 history = prompt + tokens 0 .. j - 1, and u = uniform(seed, j) (include/exl_b200.h U), so a request's tokens do not depend on
 which other requests share its steps.
+
+A guided request (Request(cfg_prompt=, cfg_alpha=), classifier-free guidance, DESIGN.md §4h) owns two slots: its prompt's and a
+shadow slot for cfg_prompt, stepped with the same tokens.  Between the step and the sampler, exl_cfg_mix penalises each of its two
+rows over its own slot's history and writes (1 - cfg_alpha) * l_prompt + cfg_alpha * l_cfg (log-softmaxed rows) to both; its
+token j is then sampling.sample of that mixed row with the request's settings, bos id and banned list, no history (the penalty
+was applied in the mix) and u = uniform(seed, j).  Both slots carry the same sampler settings and seed, so both rows draw the same
+token and exl_gen_advance appends it to both.
 """
 from __future__ import annotations
 
 import collections
 import copy
 import ctypes as C
+import math
 import time
 
 import torch
@@ -46,9 +54,12 @@ def uniform(seed, j):
 class Request:
     """One completion to generate.  prompt_ids: a non-empty 1-D list or tensor of ids; max_new_tokens >= 1; settings: a
     sampling.Settings (default its defaults), used as given; stop_ids: up to MAX_STOP ids that end the request (the stop token is
-    kept); seed: the request's uniforms are uniform(seed, j); bos_token_id, banned: as sampling.sample."""
+    kept); seed: the request's uniforms are uniform(seed, j); bos_token_id, banned: as sampling.sample.  cfg_prompt: None, or a
+    non-empty list or tensor of ids, the guidance prompt of classifier-free guidance with weight cfg_alpha (a finite float; 0 gives
+    the prompt's log-probabilities, 1 the guidance prompt's); the request then takes two slots (module docstring)."""
 
-    def __init__(self, prompt_ids, max_new_tokens, settings=None, stop_ids=(), seed=0, bos_token_id=None, banned=None):
+    def __init__(self, prompt_ids, max_new_tokens, settings=None, stop_ids=(), seed=0, bos_token_id=None, banned=None, cfg_prompt=None,
+                 cfg_alpha=0.0):
         self.prompt = [int(t) for t in torch.as_tensor(prompt_ids, dtype=torch.int64).reshape(-1).tolist()]
         self.max_new_tokens = int(max_new_tokens)
         self.settings = settings if settings is not None else sampling.Settings()
@@ -56,6 +67,12 @@ class Request:
         self.seed = int(seed) & _M64
         self.bos_token_id = bos_token_id
         self.banned = None if banned is None else [int(t) for t in banned]
+        self.cfg_prompt = None if cfg_prompt is None else [int(t) for t in torch.as_tensor(cfg_prompt, dtype=torch.int64).reshape(-1).tolist()]
+        self.cfg_alpha = float(cfg_alpha)
+        if self.cfg_prompt is not None and not self.cfg_prompt:
+            raise ValueError("Request: the cfg_prompt is empty")
+        if not math.isfinite(self.cfg_alpha):
+            raise ValueError(f"Request: cfg_alpha {self.cfg_alpha} is not finite")
         if not self.prompt:
             raise ValueError("Request: the prompt is empty")
         if self.max_new_tokens < 1:
@@ -85,11 +102,15 @@ class Result:
 
 
 class _Live:
-    __slots__ = ("rid", "req", "slot", "L", "n", "t0", "host_finish")
+    """A request in a slot.  A guided request has two: the primary (its prompt; it decides finishes and holds the tokens fetched)
+    and a shadow (cfg_prompt), linked through pair; a plain request's pair is None."""
+    __slots__ = ("rid", "req", "slot", "L", "n", "t0", "host_finish", "prompt", "pair", "shadow")
 
-    def __init__(self, rid, req, slot, t0):
-        self.rid, self.req, self.slot, self.L, self.n, self.t0 = rid, req, slot, len(req.prompt), 0, t0
+    def __init__(self, rid, req, slot, t0, shadow=False):
+        self.prompt = req.cfg_prompt if shadow else req.prompt
+        self.rid, self.req, self.slot, self.L, self.n, self.t0 = rid, req, slot, len(self.prompt), 0, t0
         self.host_finish = None
+        self.pair, self.shadow = None, shadow
 
 
 class Scheduler:
@@ -110,6 +131,11 @@ class Scheduler:
     def submit(self, req):
         if len(req.prompt) + 1 > self.max_seq:
             raise ValueError(f"submit: a prompt of {len(req.prompt)} tokens leaves no room for a token in max_seq {self.max_seq}")
+        if req.cfg_prompt is not None:
+            if self.n_slots < 2:
+                raise ValueError(f"submit: a guided request takes two slots, the stack has {self.n_slots}")
+            if len(req.cfg_prompt) + 1 > self.max_seq:
+                raise ValueError(f"submit: a cfg_prompt of {len(req.cfg_prompt)} tokens leaves no room for a token in max_seq {self.max_seq}")
         rid = self._next_id
         self._next_id += 1
         self.waiting.append((rid, req, time.perf_counter()))
@@ -120,7 +146,7 @@ class Scheduler:
         """The host's finish of lv after its tokens so far, or None."""
         if lv.n >= lv.req.max_new_tokens:
             return "length"
-        if lv.L + lv.n >= self.max_seq:
+        if max(lv.L, lv.pair.L if lv.pair is not None else 0) + lv.n >= self.max_seq:      # a guided request: its longer prompt
             return "max_seq"
         return None
 
@@ -137,9 +163,10 @@ class Scheduler:
         self.order.append((self._k, "finish", lv.rid, lv.slot, reason))
 
     def _release(self, lv):
-        self.slots[lv.slot] = None
-        self.dev.release(lv.slot)
-        self.order.append((self._k, "release", lv.rid, lv.slot))
+        for x in (lv, lv.pair) if lv.pair is not None else (lv,):
+            self.slots[x.slot] = None
+            self.dev.release(x.slot)
+            self.order.append((self._k, "release", x.rid, x.slot))
 
     def step(self):
         """One iteration: one step of the live requests, admissions (prompt and first token), the status read of the previous iteration.  Returns
@@ -148,15 +175,25 @@ class Scheduler:
         if not self.waiting and not live and self._lag is None:
             return False
         adm, tokens = [], 0
-        # waiting requests in order into the lowest free slots, at most max_seq prompt tokens in one admission (the prefill's
-        # scratch is sized for max_seq rows); the first one always goes
-        while self.waiting and None in self.slots and (not adm or tokens + len(self.waiting[0][1].prompt) <= self.max_seq):
+        # waiting requests in order into the lowest free slots (a guided request into the two lowest, and nothing overtakes one
+        # that waits for them), at most max_seq prompt tokens in one admission (the prefill's scratch is sized for max_seq rows);
+        # the first one always goes
+        while self.waiting:
+            req = self.waiting[0][1]
+            free = [s for s, x in enumerate(self.slots) if x is None]
+            cost = len(req.prompt) + (len(req.cfg_prompt) if req.cfg_prompt is not None else 0)
+            if len(free) < (1 if req.cfg_prompt is None else 2) or (adm and tokens + cost > self.max_seq):
+                break
             rid, req, t0 = self.waiting.popleft()
-            tokens += len(req.prompt)
-            s = self.slots.index(None)
-            lv = _Live(rid, req, s, t0)
-            self.slots[s] = lv
+            tokens += cost
+            lv = _Live(rid, req, free[0], t0)
+            self.slots[free[0]] = lv
             adm.append(lv)
+            if req.cfg_prompt is not None:
+                sh = _Live(rid, req, free[1], t0, shadow=True)
+                lv.pair, sh.pair = sh, lv
+                self.slots[free[1]] = sh
+                adm.append(sh)
         run = live
         # the step first: a fused step covers free slots at past_len 0 and writes their row 0, which the admission's prefill then
         # overwrites
@@ -172,12 +209,14 @@ class Scheduler:
             self.order.append((self._k, "admit", [(lv.rid, lv.slot) for lv in adm]))
         snap = []
         for lv in adm + run:
+            if lv.shadow:
+                continue                    # a guided request finishes through its primary
             snap.append((lv, lv.n))
             lv.host_finish = self._limit(lv)
         copy = self.dev.copy_status() if snap else None
-        # a request the host has finished is stepped no more: free its slot now (a stop or error in its last token is settled from
-        # the status read that covers it)
-        for lv in adm + run:
+        # a request the host has finished is stepped no more: free its slot(s) now (a stop or error in its last token is settled
+        # from the status read that covers it)
+        for lv, _ in snap:
             if lv.host_finish is not None:
                 self._fetch(lv, lv.n)
                 self._release(lv)
@@ -281,16 +320,35 @@ class _Device:
                                               capi._ptr(history), self.max_seq, lens, params, capi._ptr(u), capi._ptr(self.tokens),
                                               capi._ptr(self.probs), None, capi._stream()))
 
+    def _mix(self, logits, rows, history, hist_lens):
+        """exl_cfg_mix over the guided requests among rows (logits row i belongs to rows[i], a _Live or None), each row penalised
+        over history[i][0 .. hist_lens[i]); returns the sampler's history lengths, 0 for a guided row (it is penalised here)."""
+        at = {id(lv): i for i, lv in enumerate(rows) if lv is not None}
+        pairs = [(i, at[id(lv.pair)]) for i, lv in enumerate(rows) if lv is not None and lv.pair is not None and not lv.shadow]
+        if not pairs:
+            return hist_lens
+        n = logits.shape[0]
+        arr = (capi.ExlCfgPair * len(pairs))()
+        for k, (a, b) in enumerate(pairs):
+            req = rows[a].req
+            s = req.settings
+            arr[k] = capi.ExlCfgPair(a, b, req.cfg_alpha, s.token_repetition_penalty_max, s.token_repetition_penalty_sustain,
+                                     s.token_repetition_penalty_decay)
+        capi.check(capi.lib().exl_cfg_mix(capi._ptr(logits), n, self.V, logits.stride(0) if n > 1 else self.V, capi._ptr(history),
+                                          self.max_seq, (C.c_int * n)(*hist_lens), arr, len(pairs), capi._stream()))
+        return [0 if lv is not None and lv.pair is not None else h for lv, h in zip(rows, hist_lens)]
+
     def _trace(self, kind, logits, lives, u):
         tr = self.owner.trace
         if tr is not None:
             tr.append(dict(kind=kind, logits=logits.cpu().numpy().copy(), rids=[lv.rid for lv in lives],
-                           slots=[lv.slot for lv in lives], j=[lv.n for lv in lives], u=u.cpu().numpy().copy()))
+                           slots=[lv.slot for lv in lives], j=[lv.n for lv in lives], u=u.cpu().numpy().copy(),
+                           shadow=[lv.shadow for lv in lives]))
 
     def admit(self, lives):
         n = len(lives)
         slots = [lv.slot for lv in lives]
-        ids = self._up([t for lv in lives for t in lv.req.prompt], torch.int64)
+        ids = self._up([t for lv in lives for t in lv.prompt], torch.int64)
         idx = self._up(slots, torch.int64)
         meta = self._up([lv.req.stop_ids + [-1] * (MAX_STOP - len(lv.req.stop_ids)) + [lv.req.seed - (1 << 64) if lv.req.seed >> 63 else
                                                                                      lv.req.seed] for lv in lives], torch.int64)
@@ -306,9 +364,23 @@ class _Device:
             self.rowp[lv.slot], self.keep[lv.slot] = p, ban
         params = (capi.ExlSampleParams * n)(*[self.rowp[s] for s in slots])
         u = self._up([uniform(lv.req.seed, 0) for lv in lives], torch.float32)
-        logits = self.st.prefill_ragged(self.emb[ids], [lv.L for lv in lives], [0] * n, seqs=slots, last_only=True)
+        # at most max_seq prompt tokens per prefill (its scratch rows): only a guided request's two prompts can exceed that alone
+        chunks, off = [[]], 0
+        for i, lv in enumerate(lives):
+            if chunks[-1] and sum(lives[k].L for k in chunks[-1]) + lv.L > self.max_seq:
+                chunks.append([])
+            chunks[-1].append(i)
+        parts = []
+        for ch in chunks:
+            T = sum(lives[i].L for i in ch)
+            parts.append(self.st.prefill_ragged(self.emb[ids[off:off + T]], [lives[i].L for i in ch], [0] * len(ch),
+                                                seqs=[slots[i] for i in ch], last_only=True))
+            off += T
+        logits = parts[0] if len(parts) == 1 else torch.cat(parts)
         self._trace("admit", logits, lives, u)
-        self._sample(logits, params, self.hist.index_select(0, idx), [lv.L for lv in lives], u)
+        history = self.hist.index_select(0, idx)
+        lens = self._mix(logits, lives, history, [lv.L for lv in lives])
+        self._sample(logits, params, history, lens, u)
         self._advance(n, slots, [lv.L for lv in lives], [0] * n)
 
     def step(self, lives):
@@ -339,7 +411,8 @@ class _Device:
             tr_u = u[:len(rows)]
             self._trace("step", logits[[i for i, lv in enumerate(rows) if lv is not None]], live_rows,
                         tr_u[[i for i, lv in enumerate(rows) if lv is not None]])
-        self._sample(logits, params, history, [lv.L + lv.n if lv is not None else 0 for lv in rows], u)
+        lens = self._mix(logits, rows, history, [lv.L + lv.n if lv is not None else 0 for lv in rows])
+        self._sample(logits, params, history, lens, u)
         if ev:
             ev[2].record()
         self._advance(len(rows), [lv.slot if lv is not None else -1 for lv in rows], [lv.L + lv.n if lv is not None else 0 for lv in rows],

@@ -430,6 +430,32 @@ int exl_spec_verify(const float* target_logits, int k, int vocab, int64_t logits
                     const int64_t* history, int hist_len_host, const exl_sample_params* p, const float* u, float* work,
                     int* n_accepted, int64_t* tokens, float* probs, void* stream);
 
+/* --- classifier-free guidance (exllama_b200/csrc/cfg.cu; the reference: example_cfg.py:69-75) ------------------------------- */
+
+#define EXL_CFG_MAX_PAIRS 32
+/* One guided pair: logits rows a and b (the prompt and the guidance prompt), the mix weight alpha, and the repetition-penalty
+   triple both rows use (exl_sample_params' rep_penalty_max / rep_sustain / rep_decay). */
+typedef struct { int a, b; double alpha; float rep_penalty_max; int rep_sustain, rep_decay; } exl_cfg_pair;
+
+/* In place on fp32 logits [rows][ld], for each of the n_pairs (1 .. EXL_CFG_MAX_PAIRS) host entries of pairs_host, pair (a, b):
+     1. row a penalised over history[a][0 .. hist_len_host[a]) and row b over history[b][0 .. hist_len_host[b]) with the pair's
+        triple, bit-exact with exl_apply_rep_penalty (exl_sample's rule; none when rep_penalty_max == 1, history == NULL or the
+        length is 0);
+     2. each penalised row x': lse = m + log sum exp(x' - m) (m its maximum; exp and the sum in float64 in one fixed order), rounded
+        to fp32, and l = x' - lse in fp32;
+     3. w_a = (float)(1 - alpha), w_b = (float)alpha (computed in double), mixed = w_a * l_a + w_b * l_b with each product and the
+        sum rounded to fp32 (no contraction), written to both row a and row b.
+   Then exl_sample(_rows) of either row with no history draws the guided token (the reference's sample_current(mixed)).  If either
+   row is undefined in exl_sample's sense (a NaN logit, every logit -inf, a history id outside [0, vocab) in the penalty window),
+   both rows are written all-NaN, so the sampler returns -1 for both; a NaN the mix itself produces (0 * -inf) is written as is.
+   Rows in no pair are not touched.  Everything host-side is read during the call (baked into a CUDA-graph capture).  One launch,
+   one cluster per pair; no allocation, no floating-point atomics: two calls are bitwise equal.
+   EXL_ERR_ARG (naming the value) for rows outside 1 .. EXL_RAGGED_MAX_SEQ, vocab outside 1 .. 262144, ld < vocab, n_pairs outside
+   1 .. EXL_CFG_MAX_PAIRS, a pair row outside [0, rows), a == b, a row named in two pairs, a non-finite alpha, rep_sustain < -1,
+   rep_decay < 0, history without hist_len_host, hist_len_host[r] outside 0 .. hist_ld, or a NULL logits or pairs_host. */
+int exl_cfg_mix(float* logits, int rows, int vocab, int64_t ld, const int64_t* history, int64_t hist_ld, const int* hist_len_host,
+                const exl_cfg_pair* pairs_host, int n_pairs, void* stream);
+
 /* --- beam search (exllama_b200/csrc/beam.cu; the reference: ExLlamaGenerator.beam_search, generator.py:497-700) ------------- */
 
 #define EXL_BEAM_EXPAND 0

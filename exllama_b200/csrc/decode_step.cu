@@ -1176,7 +1176,7 @@ __global__ void __launch_bounds__(DS_THREADS, 1) decode_step_kernel(const __grid
             const float scale = rsqrtf((float)TILE);
             const int l16 = lane & 15, sub = lane >> 4;
             const int h0 = u1 > u0 ? u0 / nph : 0;
-            const int nseg = u1 > u0 ? (u1 - 1) / nph - h0 + 1 : 0;            // <= 2 (heads <= grid, checked on the host)
+            const int nseg = u1 > u0 ? (u1 - 1) / nph - h0 + 1 : 0;            // <= 2 (heads <= grid: exl_decode_plan_create checks it against the plan's grid)
             if constexpr (GQA || MULTI) att_gqa(L, u0, u1, nph, h0, nseg);
             else {
                 // every segment's q (and the new k / v rows where this CTA owns the head's last chunk): one L2 round trip
@@ -1741,6 +1741,9 @@ static int plan_create(const exl_decode_desc* d, int max_batch, const exl_decode
     cudaDeviceGetAttribute(&dev_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, p->device);
     p->grid = ds->num_sms;
     if (const char* eg = getenv("EXL_DS_GRID")) { int v = atoi(eg); if (v >= 1 && v <= ds->num_sms) p->grid = v; }
+    // ATT keeps two head segments per CTA: every head needs a CTA of its own in the plan's grid (EXL_DS_GRID included)
+    if (d->num_heads > p->grid || d->num_heads > DS_MAX_HEADS)
+        return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: more heads (%d) than the grid's %d CTAs (or than %d)", d->num_heads, p->grid, DS_MAX_HEADS));
     p->max_batch = max_batch;
     p->max_tokens = max_tokens; p->cache_seqs = cache_seqs;
     a.bsz = 1;
@@ -1761,7 +1764,6 @@ static int plan_create(const exl_decode_desc* d, int max_batch, const exl_decode
     int depth = ring_depth_for((size_t)dev_smem, fixed);
     if (const char* e = getenv("EXL_DS_DEPTH")) { int v = atoi(e); if (v >= 1 && v < depth) depth = v; }
     if (depth < 2) return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: model too wide for the shared-memory plan (%d ring stages per pipeline)", depth));
-    if (d->num_heads > ds->num_sms || d->num_heads > DS_MAX_HEADS) return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: more heads (%d) than SMs (or than %d)", d->num_heads, DS_MAX_HEADS));
     a.depth = depth;
     p->smem = smem_dynamic_bytes(fixed, depth);
     if ((size_t)H * 2 > (size_t)a.spt_max * 256) return plan_fail(p, exl_set_err(EXL_ERR_ARG, "decode_plan: internal: head staging does not fit"));

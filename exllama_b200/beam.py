@@ -21,8 +21,8 @@ import numpy as np
 import torch
 
 from . import capi, sampling
+from .slots import check_stack, open_plan, step_slots
 
-MAX_BEAMS = 64                                      # EXL_RAGGED_MAX_SEQ: rows and beams of one exl_beam_select call
 
 def select(dist, scores, beams, first=False, u=None, generator=None, out=None):
     """exl_beam_select.
@@ -36,14 +36,11 @@ def select(dist, scores, beams, first=False, u=None, generator=None, out=None):
     out      optional SelectResult to write into (one allocation reused across calls)
 
     Returns a SelectResult on the device, without synchronising; SelectResult.read() copies it to the host in one transfer."""
-    if dist.dim() != 2 or dist.dtype != torch.float32 or not dist.is_cuda or dist.stride(1) != 1:
-        raise ValueError(f"select: dist must be CUDA fp32 [rows, vocab] with unit stride along vocab, got {dist.dtype} "
-                         f"{tuple(dist.shape)} stride {dist.stride()} on {dist.device}")
-    rows, vocab = dist.shape
+    rows, vocab = sampling.check_rows("select", dist, "dist")
     if len(scores) != rows:
         raise ValueError(f"select: {len(scores)} scores for {rows} rows")
-    if not 1 <= beams <= MAX_BEAMS:
-        raise ValueError(f"select: beams {beams} outside [1, {MAX_BEAMS}]")
+    if not 1 <= beams <= capi.RAGGED_MAX_SEQ:
+        raise ValueError(f"select: beams {beams} outside [1, {capi.RAGGED_MAX_SEQ}]")
     dev = dist.device
     if first:
         if u is None:
@@ -51,10 +48,10 @@ def select(dist, scores, beams, first=False, u=None, generator=None, out=None):
         u = u.to(device=dev, dtype=torch.float32).contiguous()
     res = out if out is not None and out.beams == beams and out.rows >= rows else SelectResult(rows, beams, dev)
     sc = (C.c_double * rows)(*[float(s) for s in scores])
-    ld = dist.stride(0) if rows > 1 else vocab
     with torch.cuda.device(dev):
-        capi.check(capi.lib().exl_beam_select(capi._ptr(dist), rows, vocab, ld, sc, beams, capi.BEAM_FIRST if first else capi.BEAM_EXPAND,
-                                              capi._ptr(u) if first else None, capi._ptr(res.work), res.work.numel(),
+        capi.check(capi.lib().exl_beam_select(capi._ptr(dist), rows, vocab, sampling.row_ld(dist), sc, beams,
+                                              capi.BEAM_FIRST if first else capi.BEAM_EXPAND, capi._ptr(u) if first else None,
+                                              capi._ptr(res.work), res.work.numel(),
                                               capi._ptr(res.parent), capi._ptr(res.token), capi._ptr(res.prob), capi._ptr(res.score),
                                               capi._ptr(res.count), capi._stream()))
     return res
@@ -131,23 +128,18 @@ class BeamSearch:
     min_p 0, as gen_single_token does.  Otherwise each expansion steps every live beam, samples each beam's final distribution
     (penalty history: the committed sequence followed by the beam's window), keeps the best `beams` candidates across the beams'
     kept sets (exl_beam_select) and copies cache rows to the slots of cloned beams (exl_kv_copy_rows).  The step is
-    decode_step_fused_batch over slots 0 .. highest live slot when stack.make_plan() succeeds, else prefill_ragged over the live
-    slots.  trace: set to a list before begin() to record every selection's inputs and outputs (tests).  timings: set to a list
-    to record, per expansion, six CUDA events (start, after the step, the sampler, the selection, before and after the copies and
-    history updates), the host clock time of the selection read and the number of live beams (tools/beam_bench.py)."""
+    slots.step_slots: decode_step_fused_batch over slots 0 .. highest live slot when slots.open_plan makes the stack's plan, else a
+    ragged prefill over the live slots.  trace: set to a list before begin() to record every selection's inputs and outputs (tests).
+    timings: set to a list to record, per expansion, six CUDA events (start, after the step, the sampler, the selection, before and
+    after the copies and history updates), the host clock time of the selection read and the number of live beams
+    (tools/beam_bench.py)."""
 
     def __init__(self, stack, embed, beams, beam_length, settings=None, bos_token_id=None, banned=None, generator=None):
-        if stack.tp_size > 1:
-            raise NotImplementedError("beam search under tensor parallelism is not implemented")
-        if stack.lm_head is None:
-            raise ValueError("BeamSearch: the stack has no lm_head")
-        if not 1 <= int(beams) <= min(stack.batch, MAX_BEAMS):
-            raise ValueError(f"BeamSearch: beams {beams} outside [1, min(stack.batch {stack.batch}, {MAX_BEAMS})]")
+        check_stack("BeamSearch", stack, embed)
+        if not 1 <= int(beams) <= min(stack.batch, capi.RAGGED_MAX_SEQ):
+            raise ValueError(f"BeamSearch: beams {beams} outside [1, min(stack.batch {stack.batch}, {capi.RAGGED_MAX_SEQ})]")
         if int(beam_length) < 1:
             raise ValueError(f"BeamSearch: beam_length {beam_length} must be at least 1")
-        if embed.dtype != torch.float16 or tuple(embed.shape) != (stack.shape.vocab, stack.shape.hidden):
-            raise ValueError(f"BeamSearch: embed must be fp16 [{stack.shape.vocab}, {stack.shape.hidden}], got {embed.dtype} "
-                             f"{tuple(embed.shape)}")
         self.st, self.emb = stack, embed
         self.beams, self.beam_length = int(beams), int(beam_length)
         self.settings = settings if settings is not None else sampling.Settings()
@@ -157,15 +149,7 @@ class BeamSearch:
         self.max_seq = stack.max_seq
         self.max_beam_length = min(self.max_seq - self.beam_length, self.beam_length)
         self.simple = self.beams == 1 and self.beam_length == 1
-        if getattr(stack, "dplan", None) is not None:
-            stack.dplan.close()
-            stack.dplan = None
-        try:
-            stack.make_plan()
-            self.fused = True
-        except capi.ExlError:
-            stack.dplan = None
-            self.fused = False
+        self.fused = open_plan(stack) is None
         vocab = stack.shape.vocab
         self.hist = torch.zeros((self.beams, self.max_seq), dtype=torch.int64, device=self.dev)   # each slot's tokens
         self.dist = torch.empty((self.beams, vocab), dtype=torch.float32, device=self.dev)
@@ -252,24 +236,13 @@ class BeamSearch:
         self.idx[row, :n].copy_(self.pin[row, :n], non_blocking=True)
         return self.idx[row, :n]
 
-    def _step(self, pos, slots, idx=None):
-        """Logits [len(slots), vocab] of every live slot's token at position pos (rows in the order of slots; idx: slots on the
-        device)."""
-        st = self.st
-        if self.fused:
-            hi = max(slots)
-            pasts = [pos if s in slots else min(self.valid[s], self.max_seq - 1) for s in range(hi + 1)]
-            x = self.emb[self.hist[:hi + 1, pos]].view(hi + 1, 1, -1)
-            if st.batch == 1:
-                lg = st.decode_step_fused(x, pos).view(1, -1)
-            else:
-                lg = st.decode_step_fused_batch(x, pasts)
-            if slots != list(range(hi + 1)):
-                lg = lg.index_select(0, idx)
-            return lg
-        x = self.emb[self.hist[idx, pos]]
-        n = len(slots)
-        return st.prefill_ragged(x, [1] * n, [pos] * n, seqs=slots, last_only=False)     # one token each: every row is a last one
+    def _step(self, pos, slots, idx):
+        """Logits [len(slots), vocab] of every live slot's token at position pos, rows in the order of slots (idx: slots on the
+        device).  A dead slot below the highest live one is stepped at its valid length, so that it writes only a row that was not
+        valid (capped at max_seq - 1)."""
+        pasts = [pos if s in slots else min(self.valid[s], self.max_seq - 1) for s in range(max(slots) + 1)]
+        lg, rows = step_slots(self.st, self.fused, lambda i: self.emb[self.hist[i, pos]], slots, pasts, idx)
+        return lg if rows == slots else lg.index_select(0, idx)
 
     def _expand(self):
         n, m = len(self.seq), len(self.list[0].window)

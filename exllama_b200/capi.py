@@ -35,6 +35,8 @@ class ExlSampleParams(C.Structure):
                 ("rep_penalty_max", f32), ("rep_sustain", i32), ("rep_decay", i32), ("bos_token_id", i32),
                 ("banned", vp), ("n_banned", i32)]
 
+RAGGED_MAX_SEQ = 64                             # EXL_RAGGED_MAX_SEQ: sequences of one prefill_ragged, rows and beams of one
+                                                # exl_sample(_rows), exl_gen_advance or exl_beam_select
 CFG_MAX_PAIRS = 32                              # EXL_CFG_MAX_PAIRS
 
 

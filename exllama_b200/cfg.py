@@ -13,11 +13,9 @@ Differences from the reference, which left-pads both prompts to one length in a 
 """
 from __future__ import annotations
 
-import ctypes as C
-
 import torch
 
-from . import capi, generate, sampling
+from . import capi, sampling
 
 
 def mix(logits, pairs, alphas, settings, history=None, hist_lens=None):
@@ -33,36 +31,21 @@ def mix(logits, pairs, alphas, settings, history=None, hist_lens=None):
 
     Then sampling.sample of a mixed row with no history (and the request's bos id and banned list) draws the guided token.
     Returns logits."""
-    if logits.dim() != 2 or logits.dtype != torch.float32 or not logits.is_cuda or logits.stride(1) != 1:
-        raise ValueError(f"cfg.mix: logits must be CUDA fp32 [rows, vocab] with unit stride along vocab, got {logits.dtype} "
-                         f"{tuple(logits.shape)} stride {logits.stride()} on {logits.device}")
-    rows, vocab = logits.shape
-    dev = logits.device
+    rows, vocab = sampling.check_rows("cfg.mix", logits)
     pairs = [(int(a), int(b)) for a, b in pairs]
     n = len(pairs)
     alphas = [float(x) for x in alphas]
     settings = list(settings) if isinstance(settings, (list, tuple)) else [settings] * n
     if len(alphas) != n or len(settings) != n:
         raise ValueError(f"cfg.mix: {n} pairs, {len(alphas)} alphas and {len(settings)} settings")
-    hist_ptr, hist_ld, lens = None, 0, None
-    if history is not None:
-        if history.dim() != 2 or history.shape[0] != rows or history.dtype != torch.int64 or history.device != dev:
-            raise ValueError(f"cfg.mix: history must be int64 [rows = {rows}, hist_ld] on {dev}, got {history.dtype} "
-                             f"{tuple(history.shape)} on {history.device}")
-        history = history.contiguous()
-        hist_ld = history.shape[1]
-        hl = [hist_ld] * rows if hist_lens is None else [int(v) for v in hist_lens]
-        if len(hl) != rows:
-            raise ValueError(f"cfg.mix: {len(hl)} hist_lens for {rows} rows")
-        lens = (C.c_int * rows)(*hl)
-        hist_ptr = C.c_void_p(history.data_ptr())
+    history, hist_ld, lens = sampling.history_args("cfg.mix", history, hist_lens, rows, logits.device)
     arr = (capi.ExlCfgPair * max(n, 1))()
     for k, ((a, b), alpha, s) in enumerate(zip(pairs, alphas, settings)):
         arr[k] = capi.ExlCfgPair(a, b, alpha, s.token_repetition_penalty_max, s.token_repetition_penalty_sustain,
                                  s.token_repetition_penalty_decay)
-    ld = logits.stride(0) if rows > 1 else vocab
-    with torch.cuda.device(dev):
-        capi.check(capi.lib().exl_cfg_mix(capi._ptr(logits), rows, vocab, ld, hist_ptr, hist_ld, lens, arr, n, capi._stream()))
+    with torch.cuda.device(logits.device):
+        capi.check(capi.lib().exl_cfg_mix(capi._ptr(logits), rows, vocab, sampling.row_ld(logits), capi._ptr(history), hist_ld, lens,
+                                          arr, n, capi._stream()))
     return logits
 
 
@@ -71,13 +54,8 @@ def generate_cfg(stack, embed, prompt_pairs, alpha, max_new_tokens=128, settings
     generate.BatchGenerator, with settings used as given (sample_current keeps min_p), no bos mask, eos_token_id as the stop id,
     seed seed + i for pair i, and max_new_tokens clipped to what the longer prompt leaves in max_seq.  Returns each first prompt
     followed by its tokens (host lists of ids)."""
+    from . import generate                  # generate imports this module for mix
     s = settings if settings is not None else sampling.Settings()
-    gen = generate.BatchGenerator(stack, embed)
-    ids = []
-    for i, (p, q) in enumerate(prompt_pairs):
-        req = generate.Request(p, 1, s, stop_ids=() if eos_token_id is None else (eos_token_id,), seed=seed + i, banned=banned,
-                               cfg_prompt=q, cfg_alpha=alpha)
-        req.max_new_tokens = max(1, min(int(max_new_tokens), stack.max_seq - max(len(req.prompt), len(req.cfg_prompt))))
-        ids.append((req.prompt, gen.submit(req)))
-    res = gen.run()
-    return [prompt + res[rid].tokens for prompt, rid in ids]
+    return generate.run_prompts(stack, embed, [generate.Request(p, 1, s, stop_ids=() if eos_token_id is None else (eos_token_id,),
+                                                                seed=seed + i, banned=banned, cfg_prompt=q, cfg_alpha=alpha)
+                                               for i, (p, q) in enumerate(prompt_pairs)], max_new_tokens)

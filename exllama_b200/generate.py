@@ -7,12 +7,12 @@ stack's cache sequences, with a slot refilled as soon as its request finishes (c
 
 Cache sequence s of the stack is slot s.  Each step() steps every live request by one token, then admits waiting requests into the
 lowest free slots (their prompts in one prefill_ragged, their first tokens through one exl_sample_rows and one exl_gen_advance).  A
-step is one decode_step_fused_batch over slots 0 .. highest live slot (or one prefill_ragged when the stack has no fused plan), one
-exl_sample_rows with each row's own settings and one exl_gen_advance, which appends the tokens, tests the stop ids and writes the
-next step's input rows and uniforms on the device.  The host never waits on the step in flight: length and cache-full finishes are
-decided on the host, and the device status (stop, error) of step k - 1 is read after step k has been launched.  A request that
-stopped at step k - 1 is therefore stepped once more; exl_gen_advance ignores that row (the status is sticky), and its slot is
-freed one step late.
+step is one slots.step_slots (a decode_step_fused_batch over slots 0 .. highest live slot, or a ragged prefill when the stack has no
+fused plan), one exl_sample_rows with each row's own settings and one exl_gen_advance, which appends the tokens, tests the stop ids
+and writes the next step's input rows and uniforms on the device.  The host never waits on the step in flight: length and cache-full
+finishes are decided on the host, and the device status (stop, error) of step k - 1 is read after step k has been launched.  A
+request that stopped at step k - 1 is therefore stepped once more; exl_gen_advance ignores that row (the status is sticky), and its
+slot is freed one step late.
 
 Token j of a request is what sampling.sample returns for its logits row with the request's settings, bos id and banned list,
 history = prompt + tokens 0 .. j - 1, and u = uniform(seed, j) (include/exl_b200.h U), so a request's tokens do not depend on
@@ -35,7 +35,8 @@ import time
 
 import torch
 
-from . import capi, sampling
+from . import capi, cfg, sampling
+from .slots import check_stack, open_plan, step_slots
 
 MAX_STOP = capi.GEN_MAX_STOP
 _M64 = (1 << 64) - 1
@@ -286,15 +287,7 @@ class _Device:
         self.keep = [None] * n                               # the banned tensors rowp points into
         for s in range(n):
             self.release(s)
-        if getattr(stack, "dplan", None) is not None:
-            stack.dplan.close()
-            stack.dplan = None
-        try:
-            stack.make_plan()
-            self.fused = True
-        except capi.ExlError:
-            stack.dplan = None
-            self.fused = False
+        self.fused = open_plan(stack) is None
 
     def _up(self, values, dtype):
         """values (host) on the device without a host synchronisation: a pinned copy, which torch keeps until the copy is done."""
@@ -314,11 +307,9 @@ class _Device:
                                               capi._ptr(self.out_prob), self.max_seq, capi._stream()))
 
     def _sample(self, logits, params, history, hist_lens, u):
-        n = logits.shape[0]
-        lens = (C.c_int * n)(*hist_lens)
-        capi.check(capi.lib().exl_sample_rows(capi._ptr(logits), n, self.V, logits.stride(0) if n > 1 else self.V,
-                                              capi._ptr(history), self.max_seq, lens, params, capi._ptr(u), capi._ptr(self.tokens),
-                                              capi._ptr(self.probs), None, capi._stream()))
+        """exl_sample_rows with the cached per-slot params (history: one row per logits row)."""
+        hist = sampling.history_args("sample", history, hist_lens, logits.shape[0], self.dev)
+        sampling.launch(logits, hist, params, u, self.tokens, self.probs)
 
     def _mix(self, logits, rows, history, hist_lens):
         """exl_cfg_mix over the guided requests among rows (logits row i belongs to rows[i], a _Live or None), each row penalised
@@ -327,15 +318,7 @@ class _Device:
         pairs = [(i, at[id(lv.pair)]) for i, lv in enumerate(rows) if lv is not None and lv.pair is not None and not lv.shadow]
         if not pairs:
             return hist_lens
-        n = logits.shape[0]
-        arr = (capi.ExlCfgPair * len(pairs))()
-        for k, (a, b) in enumerate(pairs):
-            req = rows[a].req
-            s = req.settings
-            arr[k] = capi.ExlCfgPair(a, b, req.cfg_alpha, s.token_repetition_penalty_max, s.token_repetition_penalty_sustain,
-                                     s.token_repetition_penalty_decay)
-        capi.check(capi.lib().exl_cfg_mix(capi._ptr(logits), n, self.V, logits.stride(0) if n > 1 else self.V, capi._ptr(history),
-                                          self.max_seq, (C.c_int * n)(*hist_lens), arr, len(pairs), capi._stream()))
+        cfg.mix(logits, pairs, [rows[a].req.cfg_alpha for a, _ in pairs], [rows[a].req.settings for a, _ in pairs], history, hist_lens)
         return [0 if lv is not None and lv.pair is not None else h for lv, h in zip(rows, hist_lens)]
 
     def _trace(self, kind, logits, lives, u):
@@ -388,20 +371,14 @@ class _Device:
         if self.owner.timings is not None:
             ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
             ev[0].record()
-        st = self.st
-        by_slot = {lv.slot: lv for lv in lives}
-        if self.fused:
-            rows, pasts = fused_rows(lives)
-            hi = len(rows)
-            x = self.x_next[:hi].view(hi, 1, self.H)
-            logits = st.decode_step_fused(x, pasts[0]).view(1, -1) if st.batch == 1 else st.decode_step_fused_batch(x, pasts)
-            params, history, u = self.rowp, self.hist, self.u_next
+        by_slot, pasts = fused_rows(lives)
+        live = [s for s, lv in enumerate(by_slot) if lv is not None]
+        idx = None if self.fused else self._up(live, torch.int64)
+        logits, slots = step_slots(self.st, self.fused, lambda i: self.x_next[i], live, pasts, idx)
+        rows = [by_slot[s] for s in slots]
+        if self.fused:                  # the slot-ordered arrays in place: row s is slot s
+            params, history, u = self.rowp, self.hist[:len(rows)], self.u_next
         else:
-            slots = sorted(by_slot)
-            idx = self._up(slots, torch.int64)
-            rows = [by_slot[s] for s in slots]
-            logits = st.prefill_ragged(self.x_next.index_select(0, idx), [1] * len(rows), [lv.L + lv.n - 1 for lv in rows], seqs=slots,
-                                       last_only=False)
             params = (capi.ExlSampleParams * len(rows))(*[self.rowp[s] for s in slots])
             history, u = self.hist.index_select(0, idx), self.u_next.index_select(0, idx)
         if ev:
@@ -451,21 +428,16 @@ class BatchGenerator(Scheduler):
     embed   fp16 [vocab, hidden]: maps a token to the stack's input
 
     submit(Request) -> id; step() runs one iteration; run() steps until every request has finished and returns {id: Result}.
-    The step is decode_step_fused_batch when stack.make_plan() succeeds (fused is then True), else prefill_ragged with one token per
-    live slot (act-order, or more slots than the fused plan takes).  trace: set to a list to record every admission's and step's
-    logits rows with their request ids, slots, token indices and uniforms (tests).  timings: set to a list to record, per step,
-    four CUDA events (start, after the step, the sampler, the advance) and the number of requests stepped (tools/generate_bench.py)."""
+    The step is slots.step_slots: the fused batch step when slots.open_plan makes the stack's plan (fused is then True), else a
+    ragged prefill with one token per live slot (act-order, or more slots than the fused plan takes).  trace: set to a list to record
+    every admission's and step's logits rows with their request ids, slots, token indices and uniforms (tests).  timings: set to a
+    list to record, per step, four CUDA events (start, after the step, the sampler, the advance) and the number of requests stepped
+    (tools/generate_bench.py)."""
 
     def __init__(self, stack, embed):
-        if stack.tp_size > 1:
-            raise NotImplementedError("batched generation under tensor parallelism is not implemented")
-        if stack.lm_head is None:
-            raise ValueError("BatchGenerator: the stack has no lm_head")
-        if stack.batch > MAX_SLOTS:
-            raise ValueError(f"BatchGenerator: the stack holds {stack.batch} cache sequences, at most {MAX_SLOTS}")
-        if embed.dtype != torch.float16 or tuple(embed.shape) != (stack.shape.vocab, stack.shape.hidden) or not embed.is_contiguous():
-            raise ValueError(f"BatchGenerator: embed must be contiguous fp16 [{stack.shape.vocab}, {stack.shape.hidden}], got "
-                             f"{embed.dtype} {tuple(embed.shape)}")
+        check_stack("BatchGenerator", stack, embed, contiguous=True)
+        if stack.batch > capi.RAGGED_MAX_SEQ:
+            raise ValueError(f"BatchGenerator: the stack holds {stack.batch} cache sequences, at most {capi.RAGGED_MAX_SEQ}")
         self.trace = None
         self.timings = None
         super().__init__(_Device(stack, embed, self), stack.batch, stack.max_seq)
@@ -479,9 +451,6 @@ class BatchGenerator(Scheduler):
         return super().submit(req)
 
 
-MAX_SLOTS = 64                                          # EXL_RAGGED_MAX_SEQ: rows of one exl_sample_rows / exl_gen_advance
-
-
 def generate_simple(stack, embed, prompts, max_new_tokens=128, settings=None, eos_token_id=None, bos_token_id=None, banned=None,
                     seed=0):
     """ExLlamaGenerator.generate_simple over a list of prompts (lists of ids): each prompt is one request with min_p 0 and the bos
@@ -490,12 +459,17 @@ def generate_simple(stack, embed, prompts, max_new_tokens=128, settings=None, eo
     reference steps every row until all of them have one.  Returns each prompt followed by its tokens (host lists of ids)."""
     s = copy.copy(settings if settings is not None else sampling.Settings())
     s.min_p = 0.0
+    return run_prompts(stack, embed, [Request(p, 1, s, stop_ids=() if eos_token_id is None else (eos_token_id,), seed=seed + i,
+                                              bos_token_id=bos_token_id, banned=banned) for i, p in enumerate(prompts)], max_new_tokens)
+
+
+def run_prompts(stack, embed, reqs, max_new_tokens):
+    """reqs through one BatchGenerator, each with max_new_tokens clipped to what its longer prompt leaves in max_seq; returns each
+    request's prompt followed by its tokens (host lists of ids)."""
     gen = BatchGenerator(stack, embed)
     ids = []
-    for i, p in enumerate(prompts):
-        req = Request(p, 1, s, stop_ids=() if eos_token_id is None else (eos_token_id,), seed=seed + i, bos_token_id=bos_token_id,
-                      banned=banned)
-        req.max_new_tokens = max(1, min(int(max_new_tokens), stack.max_seq - len(req.prompt)))
+    for req in reqs:
+        req.max_new_tokens = max(1, min(int(max_new_tokens), stack.max_seq - max(len(req.prompt), len(req.cfg_prompt or ()))))
         ids.append((req.prompt, gen.submit(req)))
     res = gen.run()
     return [prompt + res[rid].tokens for prompt, rid in ids]

@@ -68,6 +68,48 @@ def row_params(settings, bsz, dev, bos_token_id=None, banned=None):
     return arr, keep
 
 
+def check_rows(who, t, name="logits"):
+    """(rows, vocab) of t, which the row-wise kernels take only as CUDA fp32 [rows, vocab] with unit stride along vocab."""
+    if t.dim() != 2 or t.dtype != torch.float32 or not t.is_cuda or t.stride(1) != 1:
+        raise ValueError(f"{who}: {name} must be CUDA fp32 [rows, vocab] with unit stride along vocab, got {t.dtype} "
+                         f"{tuple(t.shape)} stride {t.stride()} on {t.device}")
+    return t.shape
+
+
+def row_ld(t):
+    """The row stride of t [rows, vocab] as the row-wise kernels take it: a one-row view may carry any stride along rows."""
+    return t.stride(0) if t.shape[0] > 1 else t.shape[1]
+
+
+def history_args(who, history, hist_lens, rows, dev):
+    """A penalty history as the row-wise kernels take it: (history int64 [rows, hist_ld] contiguous -- keep it until the call is
+    made --, hist_ld, a c_int array of each row's length), or (None, 0, None) for history None.  hist_lens: host ints, default
+    hist_ld each."""
+    if history is None:
+        return None, 0, None
+    if history.dim() != 2 or history.shape[0] != rows or history.dtype != torch.int64 or history.device != dev:
+        raise ValueError(f"{who}: history must be int64 [rows = {rows}, hist_ld] on {dev}, got {history.dtype} "
+                         f"{tuple(history.shape)} on {history.device}")
+    history = history.contiguous()
+    hist_ld = history.shape[1]
+    hl = [hist_ld] * rows if hist_lens is None else [int(v) for v in hist_lens]
+    if len(hl) != rows:
+        raise ValueError(f"{who}: {len(hl)} hist_lens for {rows} rows")
+    return history, hist_ld, (C.c_int * rows)(*hl)
+
+
+def launch(logits, hist, p, u, tokens, probs, dist=None):
+    """exl_sample on the current device and stream, or exl_sample_rows when p is an array of ExlSampleParams (one per row, or
+    more) rather than one: logits as check_rows takes them, hist = history_args(...), u fp32 [rows] on the device; writes tokens,
+    probs and dist."""
+    rows, vocab = logits.shape
+    history, hist_ld, lens = hist
+    one = isinstance(p, capi.ExlSampleParams)
+    fn = capi.lib().exl_sample if one else capi.lib().exl_sample_rows
+    capi.check(fn(capi._ptr(logits), rows, vocab, row_ld(logits), capi._ptr(history), hist_ld, lens, C.byref(p) if one else p,
+                  capi._ptr(u), capi._ptr(tokens), capi._ptr(probs), capi._ptr(dist), capi._stream()))
+
+
 def sample(logits, settings, history=None, hist_lens=None, u=None, generator=None, bos_token_id=None, banned=None, dist=None):
     """One token per row of logits [bsz, vocab] fp32 (CUDA, unit stride along vocab; left unchanged).
 
@@ -83,28 +125,13 @@ def sample(logits, settings, history=None, hist_lens=None, u=None, generator=Non
 
     Returns (tokens int64 [bsz], probs fp32 [bsz]): the drawn token and its final probability; -1 / NaN for a row whose
     distribution is undefined (every logit -inf after masking, a NaN logit, a history id outside the vocabulary)."""
-    if logits.dim() != 2 or logits.dtype != torch.float32 or not logits.is_cuda or logits.stride(1) != 1:
-        raise ValueError(f"sample: logits must be CUDA fp32 [bsz, vocab] with unit stride along vocab, got {logits.dtype} "
-                         f"{tuple(logits.shape)} stride {logits.stride()} on {logits.device}")
-    bsz, vocab = logits.shape
+    bsz, vocab = check_rows("sample", logits)
     dev = logits.device
     if u is None:
         u = torch.rand(bsz, device=dev, generator=generator)
     u = u.to(device=dev, dtype=torch.float32).contiguous()
-    hist_ptr, hist_ld, lens = None, 0, None
-    if history is not None:
-        if history.dim() != 2 or history.shape[0] != bsz or history.dtype != torch.int64 or history.device != dev:
-            raise ValueError(f"sample: history must be int64 [bsz = {bsz}, hist_ld] on {dev}, got {history.dtype} "
-                             f"{tuple(history.shape)} on {history.device}")
-        history = history.contiguous()
-        hist_ld = history.shape[1]
-        hl = [hist_ld] * bsz if hist_lens is None else [int(v) for v in hist_lens]
-        if len(hl) != bsz:
-            raise ValueError(f"sample: {len(hl)} hist_lens for {bsz} rows")
-        lens = (C.c_int * bsz)(*hl)
-        hist_ptr = C.c_void_p(history.data_ptr())
-    per_row = isinstance(settings, (list, tuple))
-    if per_row:
+    hist = history_args("sample", history, hist_lens, bsz, dev)
+    if isinstance(settings, (list, tuple)):
         p, ban = row_params(settings, bsz, dev, bos_token_id, banned)
     else:
         p, ban = params(settings, dev, bos_token_id, banned)
@@ -112,9 +139,6 @@ def sample(logits, settings, history=None, hist_lens=None, u=None, generator=Non
     probs = torch.empty(bsz, dtype=torch.float32, device=dev)
     if dist is not None and (dist.shape != (bsz, vocab) or dist.dtype != torch.float32 or not dist.is_contiguous()):
         raise ValueError(f"sample: dist must be contiguous fp32 [{bsz}, {vocab}], got {dist.dtype} {tuple(dist.shape)}")
-    ld = logits.stride(0) if bsz > 1 else vocab          # a one-row view may carry any stride along rows
-    fn = capi.lib().exl_sample_rows if per_row else capi.lib().exl_sample
     with torch.cuda.device(dev):
-        capi.check(fn(capi._ptr(logits), bsz, vocab, ld, hist_ptr, hist_ld, lens, p if per_row else C.byref(p), capi._ptr(u),
-                      capi._ptr(tokens), capi._ptr(probs), capi._ptr(dist), capi._stream()))
+        launch(logits, hist, p, u, tokens, probs, dist)
     return tokens, probs

@@ -66,7 +66,7 @@ def perplexity(stack, embed, chunks, per_call=None):
     stack's input.  The chunks go through stack.prefill_ragged(..., targets=) in calls of at most per_call sequences (default
     min(stack.batch, RAGGED_MAX_SEQ)), each into cache sequences 0 .. n-1 at past_len 0; the sum stays on the device until the one
     host read at the end."""
-    cap = min(stack.batch, stack.RAGGED_MAX_SEQ)
+    cap = min(stack.batch, capi.RAGGED_MAX_SEQ)
     per_call = cap if per_call is None else int(per_call)
     if not 1 <= per_call <= cap:
         raise ValueError(f"perplexity: per_call {per_call} outside [1, {cap}]")

@@ -15,6 +15,7 @@ import ctypes as C
 import torch
 
 from . import capi, sampling
+from .slots import check_stack, open_plan
 
 
 def verify(target_logits, draft_tokens, draft_dist, settings: sampling.Settings, history=None, hist_len=None, u=None, generator=None,
@@ -31,11 +32,8 @@ def verify(target_logits, draft_tokens, draft_dist, settings: sampling.Settings,
 
     Returns (n_accepted int32 [1], tokens int64 [k + 1], probs fp32 [k + 1]) on the device, without synchronising: d_1 .. d_a, the
     correction or bonus token, then -1; n_accepted -1 and every token -1 when a row the walk reached is undefined."""
-    for name, t, dt in (("target_logits", target_logits, torch.float32), ("draft_dist", draft_dist, torch.float32)):
-        if t.dim() != 2 or t.dtype != dt or not t.is_cuda or t.stride(1) != 1:
-            raise ValueError(f"verify: {name} must be CUDA fp32 2-D with unit stride along vocab, got {t.dtype} {tuple(t.shape)} "
-                             f"stride {t.stride()} on {t.device}")
-    rows, vocab = target_logits.shape
+    rows, vocab = sampling.check_rows("verify", target_logits, "target_logits")
+    sampling.check_rows("verify", draft_dist, "draft_dist")
     k = rows - 1
     dev = target_logits.device
     if draft_tokens.shape != (k,) or draft_tokens.dtype != torch.int64 or draft_tokens.device != dev:
@@ -60,10 +58,9 @@ def verify(target_logits, draft_tokens, draft_dist, settings: sampling.Settings,
     n_acc = torch.empty(1, dtype=torch.int32, device=dev)
     tokens = torch.empty(k + 1, dtype=torch.int64, device=dev)
     probs = torch.empty(k + 1, dtype=torch.float32, device=dev)
-    ld = target_logits.stride(0) if rows > 1 else vocab
-    dld = draft_dist.stride(0) if k > 1 else vocab
     with torch.cuda.device(dev):
-        capi.check(capi.lib().exl_spec_verify(capi._ptr(target_logits), k, vocab, ld, capi._ptr(draft_tokens), capi._ptr(draft_dist), dld,
+        capi.check(capi.lib().exl_spec_verify(capi._ptr(target_logits), k, vocab, sampling.row_ld(target_logits), capi._ptr(draft_tokens),
+                                              capi._ptr(draft_dist), sampling.row_ld(draft_dist),
                                               hist_ptr, hl, C.byref(p), capi._ptr(u), capi._ptr(work), capi._ptr(n_acc),
                                               capi._ptr(tokens), capi._ptr(probs), capi._stream()))
     return n_acc, tokens, probs
@@ -74,8 +71,8 @@ class SpeculativeGenerator:
 
     target, draft          DecodeStacks with an lm_head; cache sequence 0 of each holds the sequence.  They take hidden states,
                            not token ids: target_embed / draft_embed fp16 [vocab, hidden] map a token to each stack's input.
-    k                      drafts per round; the target runs on a make_plan(max_tokens=k + 1) plan, the draft on a
-                           make_plan(max_tokens=2) plan (both made here; a plan a stack held is closed)
+    k                      drafts per round; the target runs on a multi-token plan of k + 1 tokens, the draft on one of 2
+                           (both opened here with slots.open_plan; a plan a stack held is closed)
     settings               the target's sampling settings: the emitted tokens follow exactly what sampling.sample would draw
     draft_settings         the draft's (default: settings); they change how many drafts are accepted, never the output's law
     bos_token_id, banned   as sampling.sample, for both models
@@ -90,23 +87,17 @@ class SpeculativeGenerator:
                  banned=None, generator=None):
         if k < 1:
             raise ValueError(f"SpeculativeGenerator: k {k} must be at least 1")
-        for name, st, emb in (("target", target, target_embed), ("draft", draft, draft_embed)):
-            if st.lm_head is None:
-                raise ValueError(f"SpeculativeGenerator: the {name} stack has no lm_head")
-            if emb.dtype != torch.float16 or tuple(emb.shape) != (st.shape.vocab, st.shape.hidden):
-                raise ValueError(f"SpeculativeGenerator: {name}_embed must be fp16 [{st.shape.vocab}, {st.shape.hidden}], got "
-                                 f"{emb.dtype} {tuple(emb.shape)}")
+        check_stack("SpeculativeGenerator (target)", target, target_embed)
+        check_stack("SpeculativeGenerator (draft)", draft, draft_embed)
         if target.shape.vocab != draft.shape.vocab:
             raise ValueError(f"SpeculativeGenerator: target vocab {target.shape.vocab} != draft vocab {draft.shape.vocab}")
-        for st in (target, draft):
-            if getattr(st, "dplan", None) is not None:
-                st.dplan.close()
-        try:
-            target.make_plan(max_tokens=k + 1)
-        except capi.ExlError as e:
+        e = open_plan(target, max_tokens=k + 1)
+        if e is not None:
             raise ValueError(f"SpeculativeGenerator: the target's multi-token plan cannot take k + 1 = {k + 1} tokens per step; "
                              f"speculation needs at least 2 (k >= 1) and k + 1 at most the plan's max_tokens ({e})") from e
-        draft.make_plan(max_tokens=2)
+        e = open_plan(draft, max_tokens=2)
+        if e is not None:
+            raise e
         self.target, self.draft, self.k = target, draft, k
         self.t_emb, self.d_emb = target_embed, draft_embed
         self.settings = settings if settings is not None else sampling.Settings()

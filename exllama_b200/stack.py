@@ -16,7 +16,7 @@ from __future__ import annotations
 import math
 import torch
 
-from . import cuda_ext
+from . import capi, cuda_ext
 from . import tp as tpmod
 
 ext = cuda_ext.exllama_ext
@@ -118,6 +118,7 @@ class DecodeStack:
                  layers=None, seed=0, tp_rank=0, tp_size=1, tp_group=None, with_head=True, batch=1):
         self.shape, self.groupsize, self.act_order = shape, groupsize, act_order
         self.batch = batch                     # sequences the KV caches hold (and the fused plan may step at once)
+        self.dplan = None                      # the plan of the last make_plan(), closed by close()
         self.device = torch.device(device)
         self.dev_index = self.device.index or 0
         self.max_seq = max_seq
@@ -288,9 +289,9 @@ class DecodeStack:
     # ---- decode: the whole token as ONE persistent kernel (csrc/decode_step.cu; SURVEY.md 8f-4 / 8f-2) -------------------
     def make_plan(self, with_head=True, max_tokens=None):
         """Build the exl_decode_plan over this stack's handles, norms, caches and tables (borrowed).  max_tokens (1..4): a
-        multi-token plan instead, for decode_step_fused_multi (up to max_tokens consecutive tokens of one cache sequence per launch)."""
-        from . import capi
-        hs = [[L.q.q4, L.k.q4, L.v.q4, L.o.q4, L.gate.q4, L.up.q4, L.down.q4] for L in self.layers]
+        multi-token plan instead, for decode_step_fused_multi (up to max_tokens consecutive tokens of one cache sequence per launch).
+        A plan the stack held before stays open: close it, or replace it with slots.open_plan."""
+        hs =[[L.q.q4, L.k.q4, L.v.q4, L.o.q4, L.gate.q4, L.up.q4, L.down.q4] for L in self.layers]
         head = self.lm_head if with_head else None
         multi = max_tokens is not None
         if multi and self.lora is not None:
@@ -439,8 +440,6 @@ class DecodeStack:
         hn = cuda_ext.ext_rms_norm(hidden, self.norm, self.shape.eps)
         return scoring.token_logprobs(hn.view(-1, self.shape.hidden), self.lm_head, targets.reshape(-1).contiguous())
 
-    RAGGED_MAX_SEQ = 64                        # EXL_RAGGED_MAX_SEQ: sequences of one prefill_ragged call
-
     def prefill_ragged(self, hidden, q_lens, past_lens, seqs=None, last_only=True, targets=None):
         """n prompts or follow-up turns of different lengths at different past_lens in one call.  hidden: [T, hidden] fp16, the
         sequences' tokens packed in order (sequence i owns rows [sum(q_lens[:i]), + q_lens[i])); sequence i fills rows
@@ -456,8 +455,8 @@ class DecodeStack:
         q_lens, past_lens = [int(v) for v in q_lens], [int(v) for v in past_lens]
         n = len(q_lens)
         seqs = list(range(n)) if seqs is None else [int(v) for v in seqs]
-        if not 1 <= n <= self.RAGGED_MAX_SEQ:
-            raise ValueError(f"prefill_ragged of {n} sequences: one call takes 1 .. {self.RAGGED_MAX_SEQ}")
+        if not 1 <= n <= capi.RAGGED_MAX_SEQ:
+            raise ValueError(f"prefill_ragged of {n} sequences: one call takes 1 .. {capi.RAGGED_MAX_SEQ}")
         if len(past_lens) != n or len(seqs) != n:
             raise ValueError(f"prefill_ragged: {n} q_lens, {len(past_lens)} past_lens and {len(seqs)} seqs")
         for ql, pl, sq in zip(q_lens, past_lens, seqs):
@@ -509,4 +508,6 @@ class DecodeStack:
         return torch.matmul(hn.view(-1, s.hidden), self.lm_head.t()).float()
 
     def close(self):
+        if self.dplan is not None:
+            self.dplan.close()
         ext.cleanup()

@@ -63,17 +63,14 @@ def lib_state():
 
 @pytest.fixture
 def stacks(lib_state):
-    """make_stack as a fixture: every stack made, and the plan it holds at the end of the test, is closed at teardown, pass or fail
-    (the plans first: closing a stack frees every q4 handle on the device, the ones another stack's plan reads included)."""
+    """make_stack as a fixture: every stack made, and the plan it holds at the end of the test (DecodeStack.close), is closed at
+    teardown, pass or fail."""
     made = []
 
     def make(shape=None, **kw):
         made.append(make_stack(shape, **kw))
         return made[-1]
     yield make
-    for st in made:
-        if getattr(st, "dplan", None) is not None:
-            st.dplan.close()
     for st in made:
         st.close()
 

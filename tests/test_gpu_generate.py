@@ -336,3 +336,29 @@ def test_greedy_batch_equals_alone(stacks):
             if top2[1] - top2[0] <= 2e-2 * np.sqrt((lg.astype(np.float64) ** 2).mean()):
                 break
             assert a.tokens[j] == b.tokens[j], (rid, j)
+
+
+def test_steady_steps_never_wait_on_the_device(stacks):
+    """On the fused route a step() of live requests launches the step, the sampler and the advance and reads the status copied one
+    step earlier behind its event: over 8 steady steps of 4 live requests torch's sync debug mode sees no synchronising call."""
+    import warnings
+    import torch
+    from exllama_b200.generate import BatchGenerator, Request
+    st = stacks(batch=4, seed=53, max_seq=256)
+    gen = BatchGenerator(st, _embed(st))
+    rng = np.random.default_rng(4)
+    for b in range(4):
+        gen.submit(Request(rng.integers(0, st.shape.vocab, 20 + b), 40, settings=_settings(**MIXED[b]), seed=b))
+    for _ in range(3):
+        gen.step()
+    with warnings.catch_warnings(record=True) as w:
+        warnings.simplefilter("always")
+        torch.cuda.set_sync_debug_mode("warn")
+        try:
+            for _ in range(8):
+                gen.step()
+        finally:
+            torch.cuda.set_sync_debug_mode("default")
+    syncs = [x for x in w if "called a synchronizing CUDA operation" in str(x.message)]
+    assert gen.fused and len(syncs) == 0, [str(x.message) for x in syncs[:3]]
+    assert all(r.finish == "length" and len(r.tokens) == 40 for r in gen.run().values())

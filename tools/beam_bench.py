@@ -188,8 +188,6 @@ def main():
                 line["reference_loop_tok_s_runs"] = [r["tok_s"] for r in runs_r]
             res["lines"][f"beams{beams}/len{bl}"] = line
             print(f"beams {beams} beam_length {bl}: {line}", flush=True)
-    if st.dplan is not None:
-        st.dplan.close()
     st.close()
     os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
     with open(args.out, "w") as f:

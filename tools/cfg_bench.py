@@ -184,8 +184,6 @@ def main():
         line["tok_s_runs"] = [r["tok_s"] for r in v]
         res["arms"][k] = line
         print(k, line, flush=True)
-    if st.dplan is not None:
-        st.dplan.close()
     st.close()
     os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
     with open(args.out, "w") as f:

@@ -175,14 +175,10 @@ def main():
     print("steady", res["steady_4_live"], flush=True)
     res["sampler_bsz4"] = sampler_rows_vs_one()
     print("sampler", res["sampler_bsz4"], flush=True)
-    if st.dplan is not None:
-        st.dplan.close()
     st.close()                                   # before the batch-1 stack: closing a stack frees every q4 handle on the device
     st1 = DecodeStack(shape, groupsize=128, device="cuda:0", max_seq=MAX_SEQ, layers=args.layers, seed=0, batch=1)
     for _ in range(2):
         runs["single/burst"].append(run_single(st1, emb, reqs))
-    if st1.dplan is not None:
-        st1.dplan.close()
     st1.close()
     for k, v in runs.items():
         line = max(v, key=lambda r: r["tok_s"])

@@ -183,7 +183,7 @@ def loop_times(args, gen):
         out[f"batch{bsz}"]["gpu_vs_bare"] = round(out[f"batch{bsz}"]["gpu"] / out[f"batch{bsz}"]["bare"], 4)
         out[f"batch{bsz}"]["host_vs_bare"] = round(out[f"batch{bsz}"]["host"] / out[f"batch{bsz}"]["bare"], 4)
         print(f"loop batch {bsz}: {out[f'batch{bsz}']} tok/s", flush=True)
-        st.dplan.close(); st.close()
+        st.close()
         del st
         torch.cuda.empty_cache()
     return out

@@ -189,9 +189,7 @@ def main():
     res["loop_7b_ctx1920"] = loops
     res["round_breakdown"] = breakdown
     for st in (draft, target):
-        if st.dplan is not None:
-            st.dplan.close()
-    target.close()
+        st.close()
     os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
     with open(args.out, "w") as f:
         json.dump(res, f, indent=1)

@@ -19,7 +19,7 @@ EXT_SO = os.path.join(HERE, "exllama_ext.so")
 
 CU_SOURCES = ["capi.cu", "q4_gemv.cu", "q4_matrix.cu", "elementwise.cu", "half_matmul.cu", "q4_gemm_tc.cu", "decode_attn.cu", "decode_step.cu",
               "prefill_attn.cu", "sample.cu", "logprob.cu", "beam.cu", "generate.cu",
-              "cfg.cu"]
+              "cfg.cu", "toplp.cu"]
 HEADERS = ["exl_common.cuh", "sample_select.cuh", "decode_step_sched.h", "prefill_attn_sched.h", "logprob_sched.h",
            os.path.join("..", "..", "include", "exl_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

@@ -38,6 +38,7 @@ class ExlSampleParams(C.Structure):
 RAGGED_MAX_SEQ = 64                             # EXL_RAGGED_MAX_SEQ: sequences of one prefill_ragged, rows and beams of one
                                                 # exl_sample(_rows), exl_gen_advance or exl_beam_select
 CFG_MAX_PAIRS = 32                              # EXL_CFG_MAX_PAIRS
+TOPLP_MAX = 20                                  # EXL_TOPLP_MAX: largest n_top of exl_top_logprobs
 
 
 class ExlCfgPair(C.Structure):
@@ -103,6 +104,7 @@ SIGNATURES = {
     "exl_sample": (i32, [vp, i32, i32, i64, vp, i64, C.POINTER(i32), C.POINTER(ExlSampleParams), vp, vp, vp, vp, vp]),
     "exl_sample_rows": (i32, [vp, i32, i32, i64, vp, i64, C.POINTER(i32), C.POINTER(ExlSampleParams), vp, vp, vp, vp, vp]),
     "exl_cfg_mix": (i32, [vp, i32, i32, i64, vp, i64, C.POINTER(i32), C.POINTER(ExlCfgPair), i32, vp]),
+    "exl_top_logprobs": (i32, [vp, i32, i32, i64, vp, i32, C.POINTER(i32), C.POINTER(i32), vp, i32, i64, vp, vp, vp, i64, vp]),
     "exl_gen_advance": (i32, [vp, vp, i32, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32), vp, i64, vp, vp, vp, i32, vp, i32, i32, vp, vp,
                               vp, vp, i64, vp]),
     "exl_spec_verify": (i32, [vp, i32, i32, i64, vp, vp, i64, vp, i32, C.POINTER(ExlSampleParams), vp, vp, vp, vp, vp, vp]),

@@ -75,7 +75,7 @@ __global__ void __cluster_dims__(SP_CL, 1, 1) __launch_bounds__(SP_THREADS, 1) b
     }
     const unsigned k = min((unsigned)a.beams, npos);
     const Row R;                                                     // no filter: every token is in, keyed by desc_key(p, id)
-    const unsigned long long thr = radix_descent(sh, ph, R, s_row, n, lo, 1, false, k, 0).key;
+    const unsigned long long thr = radix_descent(sh, ph, ProbEval{R, 1}, s_row, n, lo, false, k, 0).key;
     // this CTA's share of the best k goes after the shares of the lower ranks
     unsigned mine = 0;
     for (int i = threadIdx.x; i < n; i += SP_THREADS) mine += desc_key(s_row[i], lo + i) >= thr ? 1u : 0u;

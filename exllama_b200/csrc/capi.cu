@@ -76,11 +76,11 @@ int exl_own_scratch(ExlDevice* ds, int role, int64_t numel, half** out)
 extern "C" {
 
 const char* exl_last_error(void) { return t_err; }
-int exl_version(void) { return 111; }             // 101: exl_decode_desc.num_kv_heads; 102: batched decode plans and steps; 103: LoRA plans;
+int exl_version(void) { return 112; }             // 101: exl_decode_desc.num_kv_heads; 102: batched decode plans and steps; 103: LoRA plans;
                                                   // 104: exl_prefill_attn; 105: exl_prefill_attn_ragged, exl_rope_cache_ragged; 106: exl_sample;
                                                   // 107: exl_spec_verify; 108: exl_token_logprobs;
                                                   // 109: exl_beam_select, exl_kv_copy_rows; 110: exl_sample_rows, exl_gen_advance;
-                                                  // 111: exl_cfg_mix
+                                                  // 111: exl_cfg_mix; 112: exl_top_logprobs
 int64_t exl_launch_count(void) { return g_launches.load(); }
 const char* exl_last_q4_path(void) { return g_last_q4_path; }
 
@@ -640,6 +640,14 @@ int exl_cfg_mix(float* logits, int rows, int vocab, int64_t ld, const int64_t* h
                 const exl_cfg_pair* pairs_host, int n_pairs, void* stream)
 {
     return exl_cfg_mix_launch(logits, rows, vocab, ld, history, hist_ld, hist_len_host, pairs_host, n_pairs, (cudaStream_t)stream);
+}
+
+int exl_top_logprobs(const float* logits, int rows, int vocab, int64_t logits_ld, const int64_t* tokens, int n_top, const int* slot_host,
+                     const int* j_host, const int* status, int n_slots, int64_t out_ld, float* lp, int64_t* top_ids, float* top_lp,
+                     int64_t top_ld, void* stream)
+{
+    return exl_top_logprobs_launch(logits, rows, vocab, logits_ld, tokens, n_top, slot_host, j_host, status, n_slots, out_ld, lp, top_ids,
+                                   top_lp, top_ld, (cudaStream_t)stream);
 }
 
 int exl_gen_advance(const int64_t* tokens, const float* probs, int rows, const int* slot_host, const int* pos_host, const int* j_host,

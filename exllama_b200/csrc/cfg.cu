@@ -28,27 +28,6 @@ struct CfgArgs {
 };
 static_assert(sizeof(CfgArgs) <= 4096, "CfgArgs must fit the classic 4 KB kernel parameter space");
 
-// float64 sum over the cluster in one fixed order; the bits travel in Part::m
-__device__ double cluster_sum_d(Shared& sh, int& ph, double v)
-{
-    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) sh.redm[threadIdx.x >> 5] = (unsigned long long)__double_as_longlong(v);
-    __syncthreads();
-    Part p{};
-    if (threadIdx.x == 0) {
-        double s = 0.0;
-        for (int w = 0; w < SP_THREADS / 32; w++) s += __longlong_as_double((long long)sh.redm[w]);
-        p.m = (unsigned long long)__double_as_longlong(s);
-    }
-    cluster_exchange(sh, ph, p, [](const Part* ps, Part& o) {
-        double s = 0.0;
-        for (int r = 0; r < SP_CL; r++) s += __longlong_as_double((long long)ps[r].m);
-        o.m = (unsigned long long)__double_as_longlong(s);
-    });
-    return __longlong_as_double((long long)sh.bc.m);
-}
-
 __global__ void __cluster_dims__(SP_CL, 1, 1) __launch_bounds__(SP_THREADS, 1) cfg_mix_kernel(const __grid_constant__ CfgArgs a)
 {
     extern __shared__ __align__(16) float s_row[];

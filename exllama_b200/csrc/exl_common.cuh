@@ -185,6 +185,11 @@ int exl_spec_verify_launch(const float* target_logits, int k, int vocab, int64_t
 int exl_cfg_mix_launch(float* logits, int rows, int vocab, int64_t ld, const int64_t* history, int64_t hist_ld, const int* hist_len,
                        const exl_cfg_pair* pairs, int n_pairs, cudaStream_t stream);
 
+// toplp.cu
+int exl_top_logprobs_launch(const float* logits, int rows, int vocab, int64_t logits_ld, const int64_t* tokens, int n_top,
+                            const int* slot_host, const int* j_host, const int* status, int n_slots, int64_t out_ld, float* lp,
+                            int64_t* top_ids, float* top_lp, int64_t top_ld, cudaStream_t stream);
+
 // generate.cu
 int exl_gen_advance_launch(const int64_t* tokens, const float* probs, int rows, const int* slot_host, const int* pos_host,
                            const int* j_host, int64_t* hist, int64_t hist_ld, int* status, const int64_t* stop_ids,

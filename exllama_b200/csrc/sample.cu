@@ -108,7 +108,7 @@ __global__ void __cluster_dims__(SP_CL, 1, 1) __launch_bounds__(SP_THREADS, 1) s
     unsigned len = (unsigned)a.vocab;                                // length of the ordered list at the current stage
     // 4. top-k, then L1 normalisation
     if (rs.top_k > 0) {
-        R.kk = radix_descent(sh, ph, R, s_row, n, lo, 1, false, (unsigned)rs.top_k, 0).key;
+        R.kk = radix_descent(sh, ph, ProbEval{R, 1}, s_row, n, lo, false, (unsigned)rs.top_k, 0).key;
         len = (unsigned)rs.top_k;
         float s = 0.f;
         for (int i = threadIdx.x; i < n; i += SP_THREADS) if (desc_key(s_row[i], lo + i) >= R.kk) s += s_row[i];
@@ -117,7 +117,7 @@ __global__ void __cluster_dims__(SP_CL, 1, 1) __launch_bounds__(SP_THREADS, 1) s
     // 5. top-p with its min_p test, then renormalise
     if (rs.top_p > 0.0f) {
         const unsigned long long T = (unsigned long long)((double)fminf(rs.top_p, 2.0f) * SP_FIX);
-        const Descent c = radix_descent(sh, ph, R, s_row, n, lo, 1, true, 0, T);
+        const Descent c = radix_descent(sh, ph, ProbEval{R, 1}, s_row, n, lo, true, 0, T);
         const unsigned n_p = c.found ? c.before : len;
         unsigned cm = 0;
         for (int i = threadIdx.x; i < n; i += SP_THREADS) {
@@ -128,7 +128,7 @@ __global__ void __cluster_dims__(SP_CL, 1, 1) __launch_bounds__(SP_THREADS, 1) s
         const unsigned keep = max(1u, min(min(n_p, cm), len));
         if (c.found && keep == n_p) R.kp = c.key + 1;                // everything before the first token past top_p
         else if (keep == len) R.kp = 0;
-        else R.kp = radix_descent(sh, ph, R, s_row, n, lo, 1, false, keep, 0).key;
+        else R.kp = radix_descent(sh, ph, ProbEval{R, 1}, s_row, n, lo, false, keep, 0).key;
         len = keep;
         float s = 0.f;
         for (int i = threadIdx.x; i < n; i += SP_THREADS) {
@@ -146,12 +146,12 @@ __global__ void __cluster_dims__(SP_CL, 1, 1) __launch_bounds__(SP_THREADS, 1) s
         }
         R.negent = cluster_sum_f(sh, ph, s);
         const unsigned long long T = (unsigned long long)((double)fminf(rs.typical, 2.0f) * SP_FIX);
-        const Descent c = radix_descent(sh, ph, R, s_row, n, lo, 3, true, 0, T);
+        const Descent c = radix_descent(sh, ph, ProbEval{R, 3}, s_row, n, lo, true, 0, T);
         const unsigned n_t = c.found ? c.before : len;
         const unsigned keep = max(1u, min(n_t, len));
         if (c.found && keep == n_t) R.kt = c.key + 1;
         else if (keep == len) R.kt = 0;
-        else R.kt = radix_descent(sh, ph, R, s_row, n, lo, 3, false, keep, 0).key;
+        else R.kt = radix_descent(sh, ph, ProbEval{R, 3}, s_row, n, lo, false, keep, 0).key;
         float s2 = 0.f;
         for (int i = threadIdx.x; i < n; i += SP_THREADS) {
             const Tok t = eval(R, s_row[i], lo + i, 3);

@@ -1,4 +1,5 @@
-// sample_select.cuh -- the sampler's order keys, radix selector and repetition penalty (csrc/sample.cu), shared with csrc/beam.cu and csrc/cfg.cu.
+// sample_select.cuh -- the sampler's order keys, radix selector and repetition penalty (csrc/sample.cu), shared with csrc/beam.cu,
+// csrc/cfg.cu and csrc/toplp.cu.
 //
 // One thread-block cluster of SP_CL CTAs per row; CTA r keeps the slice [r * slice, (r + 1) * slice) of the row in shared memory.
 // Tokens are ordered by 50-bit keys (the float's bits above the inverted token id, so keys are unique and a tie goes to the lower
@@ -130,6 +131,28 @@ __device__ unsigned cluster_sum_c(Shared& sh, int& ph, unsigned v)
     return sh.bc.c;
 }
 
+// float64 sum over the cluster in one fixed order (thread strides, warp butterflies, warps in order, CTAs in rank order); the bits
+// travel in Part::m
+__device__ double cluster_sum_d(Shared& sh, int& ph, double v)
+{
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) sh.redm[threadIdx.x >> 5] = (unsigned long long)__double_as_longlong(v);
+    __syncthreads();
+    Part p{};
+    if (threadIdx.x == 0) {
+        double s = 0.0;
+        for (int w = 0; w < SP_THREADS / 32; w++) s += __longlong_as_double((long long)sh.redm[w]);
+        p.m = (unsigned long long)__double_as_longlong(s);
+    }
+    cluster_exchange(sh, ph, p, [](const Part* ps, Part& o) {
+        double s = 0.0;
+        for (int r = 0; r < SP_CL; r++) s += __longlong_as_double((long long)ps[r].m);
+        o.m = (unsigned long long)__double_as_longlong(s);
+    });
+    return __longlong_as_double((long long)sh.bc.m);
+}
+
 // ---- the repetition penalty of one row (apply_rep_penalty_cpu, bit-exact with exl_apply_rep_penalty), used by csrc/sample.cu and
 // csrc/cfg.cu.  penalty_scan leaves in s_int[i] the newest position j (0 = newest) in the history window of token lo + i of the slice
 // (INT_MAX: not in the window) and in sh.vtab the first SP_VTAB factors of the fp32 recurrence v += dv; it sets bad for a history
@@ -209,13 +232,21 @@ __device__ __forceinline__ Tok eval(const Row& R, float p, int id, int level)
     return t;
 }
 
+// eval at one level as radix_descent's evaluator: the sampler's and beam search's probability orders
+struct ProbEval {
+    const Row& R; int level;
+    __device__ __forceinline__ Tok operator()(float p, int id) const { return eval(R, p, id, level); }
+};
+
 struct Descent { unsigned long long key; unsigned before; bool found; };
 
-// Radix descent over the keys of the tokens `in` at `level`, in decreasing key order.
+// Radix descent over the keys of the tokens `in`, in decreasing key order; ev(s_row[i], lo + i) gives each token's Tok (ProbEval for
+// the probability orders; any evaluator whose keys fit SP_KEY_BITS and are unique).
 //   cross == false: the token of rank k (1-based).
 //   cross == true : the first token whose inclusive mass (fixed point, weights w) exceeds T.
-__device__ Descent radix_descent(Shared& sh, int& ph, const Row& R, const float* s_row, int n, int lo, int level, bool cross,
-                                 unsigned k, unsigned long long T)
+template <class Eval>
+__device__ Descent radix_descent(Shared& sh, int& ph, const Eval& ev, const float* s_row, int n, int lo, bool cross, unsigned k,
+                                 unsigned long long T)
 {
     cg::cluster_group cluster = cg::this_cluster();
     unsigned long long prefix = 0, acc = 0;
@@ -227,7 +258,7 @@ __device__ Descent radix_descent(Shared& sh, int& ph, const Row& R, const float*
         if (threadIdx.x == 0) sh.found_pos = -1;
         __syncthreads();
         for (int i = threadIdx.x; i < n; i += SP_THREADS) {
-            const Tok t = eval(R, s_row[i], lo + i, level);
+            const Tok t = ev(s_row[i], lo + i);
             if (!t.in || (t.key >> (shift + SP_DIGIT)) != (prefix >> (shift + SP_DIGIT))) continue;
             const int d = (int)(t.key >> shift) & (SP_BINS - 1);
             atomicAdd(&sh.cnt[buf][d], 1u);

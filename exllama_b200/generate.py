@@ -24,6 +24,11 @@ rows over its own slot's history and writes (1 - cfg_alpha) * l_prompt + cfg_alp
 token j is then sampling.sample of that mixed row with the request's settings, bos id and banned list, no history (the penalty
 was applied in the mix) and u = uniform(seed, j).  Both slots carry the same sampler settings and seed, so both rows draw the same
 token and exl_gen_advance appends it to both.
+
+A request with logprobs=N (1 .. capi.TOPLP_MAX) also gets, per token, the model's log-probability of that token and its N most likely
+tokens with theirs (DESIGN.md §4i): exl_top_logprobs runs between the sampler and exl_gen_advance over the same logits rows the
+sampler read (a guided request's mixed rows), whenever a row of the launch asks, and writes each asking row's results into its
+slot's output rows under exl_gen_advance's status gate.  The tokens, probs and finishes are those of the same request without it.
 """
 from __future__ import annotations
 
@@ -57,10 +62,11 @@ class Request:
     sampling.Settings (default its defaults), used as given; stop_ids: up to MAX_STOP ids that end the request (the stop token is
     kept); seed: the request's uniforms are uniform(seed, j); bos_token_id, banned: as sampling.sample.  cfg_prompt: None, or a
     non-empty list or tensor of ids, the guidance prompt of classifier-free guidance with weight cfg_alpha (a finite float; 0 gives
-    the prompt's log-probabilities, 1 the guidance prompt's); the request then takes two slots (module docstring)."""
+    the prompt's log-probabilities, 1 the guidance prompt's); the request then takes two slots (module docstring).  logprobs: 0 (off)
+    or N in 1 .. capi.TOPLP_MAX, the number of alternatives reported per token in Result.top_logprobs."""
 
     def __init__(self, prompt_ids, max_new_tokens, settings=None, stop_ids=(), seed=0, bos_token_id=None, banned=None, cfg_prompt=None,
-                 cfg_alpha=0.0):
+                 cfg_alpha=0.0, logprobs=0):
         self.prompt = [int(t) for t in torch.as_tensor(prompt_ids, dtype=torch.int64).reshape(-1).tolist()]
         self.max_new_tokens = int(max_new_tokens)
         self.settings = settings if settings is not None else sampling.Settings()
@@ -70,6 +76,9 @@ class Request:
         self.banned = None if banned is None else [int(t) for t in banned]
         self.cfg_prompt = None if cfg_prompt is None else [int(t) for t in torch.as_tensor(cfg_prompt, dtype=torch.int64).reshape(-1).tolist()]
         self.cfg_alpha = float(cfg_alpha)
+        self.logprobs = int(logprobs)
+        if not 0 <= self.logprobs <= capi.TOPLP_MAX:
+            raise ValueError(f"Request: logprobs {self.logprobs} outside [0, {capi.TOPLP_MAX}]")
         if self.cfg_prompt is not None and not self.cfg_prompt:
             raise ValueError("Request: the cfg_prompt is empty")
         if not math.isfinite(self.cfg_alpha):
@@ -86,19 +95,27 @@ class Result:
     """tokens, probs: host lists of the generated tokens and their final probabilities; finish: "stop" (the last token is a stop
     id), "length" (max_new_tokens), "max_seq" (the cache sequence is full) or "error" (an undefined distribution: NaN logits, or
     every token masked; tokens then holds the ones before it); t_first: seconds from submit() to the host's first sight of the
-    first token (one step after it was drawn, as every status read)."""
+    first token (one step after it was drawn, as every status read).  For a request with logprobs=N (None otherwise): logprobs, the
+    model's log-probability of each token (its raw logits row, or a guided request's mixed row, before any penalty, temperature or
+    filter); top_logprobs, per token a list of the N (id, log-probability) pairs with the largest logits, in descending order (fewer
+    when the row has fewer finite logits)."""
 
     def __init__(self):
         self.tokens, self.probs, self.finish, self.t_first = [], [], None, None
+        self.logprobs, self.top_logprobs = None, None
         self._fetch, self._n = None, None
 
     def _settle(self):
         if self._fetch is not None:
-            ev, tok, prob = self._fetch
+            ev, tok, prob, *lps = self._fetch
             ev.synchronize()
             t, p = tok.tolist(), prob.tolist()
             n = t.index(-1) if -1 in t else len(t)
             self.tokens, self.probs = t[:n], p[:n]
+            if lps:
+                lp, ids, top = (x.tolist() for x in lps)
+                self.logprobs = lp[:n]
+                self.top_logprobs = [[(i, v) for i, v in zip(ids[k], top[k]) if i >= 0] for k in range(n)]
             self._fetch = None
 
 
@@ -117,7 +134,7 @@ class _Live:
 class Scheduler:
     """The host side of batched generation: admission, slots, positions and finishes.  dev carries out the device work (_Device for
     a DecodeStack; tests substitute a fake): admit(lives), step(lives), copy_status() -> i (an index), read_status(i) -> the status of every slot when copy i was made (host int array), fetch(live, n)
-    -> (event, tokens, probs), release(slot)."""
+    -> (event, tokens, probs), or (event, tokens, probs, lp, ids, top) for a request with logprobs, release(slot)."""
 
     def __init__(self, dev, n_slots, max_seq):
         self.dev, self.n_slots, self.max_seq = dev, int(n_slots), int(max_seq)
@@ -278,6 +295,7 @@ class _Device:
         self.u_next = z((n,), torch.float32)
         self.out_tok = z((n, ms), torch.int64)
         self.out_prob = z((n, ms), torch.float32)
+        self.out_lp = self.out_ids = self.out_top = None     # [n, ms] and [n, ms, TOPLP_MAX], made when a request first asks
         self.tokens = z((n,), torch.int64)
         self.probs = z((n,), torch.float32)
         self.pin = torch.zeros((2, n), dtype=torch.int32).pin_memory()
@@ -320,6 +338,21 @@ class _Device:
             return hist_lens
         cfg.mix(logits, pairs, [rows[a].req.cfg_alpha for a, _ in pairs], [rows[a].req.settings for a, _ in pairs], history, hist_lens)
         return [0 if lv is not None and lv.pair is not None else h for lv, h in zip(rows, hist_lens)]
+
+    def _top_logprobs(self, logits, rows, js):
+        """exl_top_logprobs over logits (row i belongs to rows[i], a _Live or None, as its token j = js[i]) when a row asks, with the
+        largest N of those rows, into the asking rows' slots under the status gate (the shadow of a guided request never asks)."""
+        ask = [lv is not None and not lv.shadow and lv.req.logprobs > 0 for lv in rows]
+        if not any(ask):
+            return
+        if self.out_lp is None:
+            shape = (self.n_slots, self.max_seq)
+            self.out_lp = torch.full(shape, float("nan"), dtype=torch.float32, device=self.dev)
+            self.out_ids = torch.full(shape + (capi.TOPLP_MAX,), -1, dtype=torch.int64, device=self.dev)
+            self.out_top = torch.full(shape + (capi.TOPLP_MAX,), float("nan"), dtype=torch.float32, device=self.dev)
+        n = max(lv.req.logprobs for lv, a in zip(rows, ask) if a)
+        sampling.launch_top_logprobs(logits, self.tokens, n, self.out_lp, self.out_ids, self.out_top, capi.TOPLP_MAX,
+                                     [lv.slot if a else -1 for lv, a in zip(rows, ask)], js, self.status, self.max_seq)
 
     def _trace(self, kind, logits, lives, u):
         tr = self.owner.trace
@@ -364,6 +397,7 @@ class _Device:
         history = self.hist.index_select(0, idx)
         lens = self._mix(logits, lives, history, [lv.L for lv in lives])
         self._sample(logits, params, history, lens, u)
+        self._top_logprobs(logits, lives, [0] * n)
         self._advance(n, slots, [lv.L for lv in lives], [0] * n)
 
     def step(self, lives):
@@ -390,6 +424,7 @@ class _Device:
                         tr_u[[i for i, lv in enumerate(rows) if lv is not None]])
         lens = self._mix(logits, rows, history, [lv.L + lv.n if lv is not None else 0 for lv in rows])
         self._sample(logits, params, history, lens, u)
+        self._top_logprobs(logits, rows, [lv.n if lv is not None else 0 for lv in rows])
         if ev:
             ev[2].record()
         self._advance(len(rows), [lv.slot if lv is not None else -1 for lv in rows], [lv.L + lv.n if lv is not None else 0 for lv in rows],
@@ -416,9 +451,15 @@ class _Device:
         prob = torch.empty(n, dtype=torch.float32).pin_memory()
         tok.copy_(self.out_tok[lv.slot, :n], non_blocking=True)
         prob.copy_(self.out_prob[lv.slot, :n], non_blocking=True)
+        out = [tok, prob]
+        N = lv.req.logprobs
+        if N:
+            for src in (self.out_lp[lv.slot, :n], self.out_ids[lv.slot, :n, :N], self.out_top[lv.slot, :n, :N]):
+                out.append(torch.empty(src.shape, dtype=src.dtype).pin_memory())
+                out[-1].copy_(src, non_blocking=True)
         ev = torch.cuda.Event()
         ev.record()
-        return ev, tok, prob
+        return (ev, *out)
 
 
 class BatchGenerator(Scheduler):
@@ -431,7 +472,7 @@ class BatchGenerator(Scheduler):
     The step is slots.step_slots: the fused batch step when slots.open_plan makes the stack's plan (fused is then True), else a
     ragged prefill with one token per live slot (act-order, or more slots than the fused plan takes).  trace: set to a list to record
     every admission's and step's logits rows with their request ids, slots, token indices and uniforms (tests).  timings: set to a
-    list to record, per step, four CUDA events (start, after the step, the sampler, the advance) and the number of requests stepped
+    list to record, per step, four CUDA events (start, after the step, the sampler and exl_top_logprobs when a row asks, the advance) and the number of requests stepped
     (tools/generate_bench.py)."""
 
     def __init__(self, stack, embed):

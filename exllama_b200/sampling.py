@@ -6,6 +6,11 @@ exl_sample_rows when each row has its own settings).
 
 takes the logits of DecodeStack.decode_step_fused(_batch) or prefill_ragged as they come ([bsz, vocab] fp32 on the device) and
 returns int64 tokens and fp32 probabilities on the same device and stream, with no host synchronisation.
+
+    lp, ids, top = sampling.top_logprobs(logits, 5, tokens)
+
+gives the model's log-probability of each row's token and the row's 5 most likely tokens with theirs (csrc/toplp.cu, include/exl_b200.h
+exl_top_logprobs): the unprocessed distribution, before any penalty, temperature or filter.
 """
 from __future__ import annotations
 
@@ -142,3 +147,38 @@ def sample(logits, settings, history=None, hist_lens=None, u=None, generator=Non
     with torch.cuda.device(dev):
         launch(logits, hist, p, u, tokens, probs, dist)
     return tokens, probs
+
+
+def top_logprobs(logits, n, tokens=None):
+    """The model's log-probabilities at each row of logits [rows, vocab] (as check_rows takes them; left unchanged): exl_top_logprobs.
+
+    n       0 .. capi.TOPLP_MAX alternatives per row
+    tokens  int64 [rows] on the device (e.g. sample's tokens), or None
+
+    Returns (lp fp32 [rows], ids int64 [rows, n], top fp32 [rows, n]) on the device, without synchronising: lp the log-probability of
+    tokens[r] (NaN for no token, a token outside the vocabulary or an undefined row); ids / top the n largest finite logits' ids and
+    log-probabilities in descending order, a tie to the lower id (-1 / -inf past the row's finite entries; -1 / NaN on an undefined
+    row: a NaN or +inf logit, or no finite one)."""
+    rows, vocab = check_rows("top_logprobs", logits)
+    dev = logits.device
+    n = int(n)
+    if tokens is not None and (tokens.shape != (rows,) or tokens.dtype != torch.int64 or tokens.device != dev or not tokens.is_contiguous()):
+        raise ValueError(f"top_logprobs: tokens must be contiguous int64 [{rows}] on {dev}, got {tokens.dtype} {tuple(tokens.shape)} "
+                         f"on {tokens.device}")
+    lp = torch.empty(rows, dtype=torch.float32, device=dev)
+    ids = torch.empty((rows, n), dtype=torch.int64, device=dev)
+    top = torch.empty((rows, n), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        launch_top_logprobs(logits, tokens, n, lp, ids, top, max(n, 1))
+    return lp, ids, top
+
+
+def launch_top_logprobs(logits, tokens, n, lp, ids, top, top_ld, slots=None, js=None, status=None, out_ld=0):
+    """exl_top_logprobs on the current device and stream (logits as check_rows takes them); with slots (host ints, -1: none), js
+    (host ints) and status (int32 device), row r writes lp / ids / top row [slots[r]][js[r]] while that slot is live."""
+    rows, vocab = logits.shape
+    arr = lambda v: None if v is None else (C.c_int * rows)(*[int(x) for x in v])
+    n_slots = 0 if status is None else status.shape[0]
+    capi.check(capi.lib().exl_top_logprobs(capi._ptr(logits), rows, vocab, row_ld(logits), capi._ptr(tokens), n, arr(slots), arr(js),
+                                           capi._ptr(status), n_slots, out_ld, capi._ptr(lp), capi._ptr(ids), capi._ptr(top), top_ld,
+                                           capi._stream()))

@@ -77,18 +77,25 @@ class SpeculativeGenerator:
     draft_settings         the draft's (default: settings); they change how many drafts are accepted, never the output's law
     bos_token_id, banned   as sampling.sample, for both models
     generator              a CUDA torch.Generator for every uniform
+    logprobs               0 (off) or N in 1 .. capi.TOPLP_MAX: every round appends, per emitted token, the target's log-probability
+                           of it to token_logprobs and its N (id, log-probability) alternatives to top_logprobs (sampling.top_logprobs
+                           of target row i for emitted token i of the round: the model's distribution, before any penalty or filter)
 
     A round drafts d_1 .. d_k one token at a time (sampling.sample(..., dist=) of the draft's logits), runs the target once over
     [last token, d_1 .. d_k], and verify() keeps d_1 .. d_a plus one token of the target's.  Token ids, the history and the
     embedding gathers stay on the device; the one host synchronisation per round reads a, because the next round's past_len is a
-    host argument of the step.  Rows past the accepted ones are left stale in both caches and overwritten by the next round."""
+    host argument of the step.  Rows past the accepted ones are left stale in both caches and overwritten by the next round.  With
+logprobs, exl_top_logprobs runs over the k + 1 target rows with the verification's tokens, and its results come to the host in the
+same synchronisation."""
 
     def __init__(self, target, draft, target_embed, draft_embed, k=3, settings=None, draft_settings=None, bos_token_id=None,
-                 banned=None, generator=None):
+                 banned=None, generator=None, logprobs=0):
         if k < 1:
             raise ValueError(f"SpeculativeGenerator: k {k} must be at least 1")
         check_stack("SpeculativeGenerator (target)", target, target_embed)
         check_stack("SpeculativeGenerator (draft)", draft, draft_embed)
+        if not 0 <= int(logprobs) <= capi.TOPLP_MAX:
+            raise ValueError(f"SpeculativeGenerator: logprobs {logprobs} outside [0, {capi.TOPLP_MAX}]")
         if target.shape.vocab != draft.shape.vocab:
             raise ValueError(f"SpeculativeGenerator: target vocab {target.shape.vocab} != draft vocab {draft.shape.vocab}")
         e = open_plan(target, max_tokens=k + 1)
@@ -111,6 +118,12 @@ class SpeculativeGenerator:
         self.q = torch.empty((k, target.shape.vocab), dtype=torch.float32, device=self.dev)
         self.n = 0                          # tokens of the sequence: prompt + emitted; the last one is in neither cache yet
         self.catch_up = False               # the last round accepted every draft: the draft has not processed d_k
+        self.logprobs = int(logprobs)
+        self.token_logprobs, self.top_logprobs = [], []     # per token emitted by round(), in order
+        if self.logprobs:
+            self._lp_pin = [torch.empty(shape, dtype=dt).pin_memory()
+                            for shape, dt in (((k + 1,), torch.float32), ((k + 1, self.logprobs), torch.int64),
+                                              ((k + 1, self.logprobs), torch.float32))]
 
     def _sample(self, logits, settings, hist_len, dist=None):
         return sampling.sample(logits, settings, history=self.hist.view(1, -1), hist_lens=[hist_len], generator=self.gen,
@@ -148,10 +161,17 @@ class SpeculativeGenerator:
         n_acc, tokens, _ = verify(logits, self.hist[n:n + k], self.q, self.settings, history=self.hist, hist_len=n, generator=self.gen,
                                   bos_token_id=self.bos, banned=self.banned)
         self.hist[n:n + k + 1] = tokens
+        if self.logprobs:
+            for pin, d in zip(self._lp_pin, sampling.top_logprobs(logits, self.logprobs, tokens)):
+                pin.copy_(d, non_blocking=True)
         a = int(n_acc.item())                                    # the round's one host synchronisation
         if a < 0:
             raise RuntimeError(f"round at {n} tokens: a distribution the verification reached is undefined (NaN logits, or every "
                                f"token masked)")
+        if self.logprobs:
+            lp, ids, top = (x.tolist() for x in self._lp_pin)
+            self.token_logprobs += lp[:a + 1]
+            self.top_logprobs += [[(i, v) for i, v in zip(ids[r], top[r]) if i >= 0] for r in range(a + 1)]
         self.n, self.catch_up = n + a + 1, a == k
         return a
 

@@ -532,6 +532,37 @@ int exl_gen_advance(const int64_t* tokens, const float* probs, int rows, const i
                     const void* embed, int vocab, int hidden, void* x_next, float* u_next, int64_t* out_tokens, float* out_probs,
                     int64_t out_ld, void* stream);
 
+/* --- log-probabilities of generated tokens (exllama_b200/csrc/toplp.cu) ------------------------------------------------------ */
+
+#define EXL_TOPLP_MAX 20   /* largest n_top of exl_top_logprobs */
+
+/* The model's log-probabilities at each row of fp32 logits [rows][logits_ld] (1 .. EXL_RAGGED_MAX_SEQ rows, vocab 1 .. 262144): the
+   row exactly as exl_sample(_rows) reads it (for a guided row, what exl_cfg_mix wrote), with no penalty, temperature, bos mask,
+   banned list or filter applied -- the model's distribution, not the sampling distribution.
+   A row x is undefined if it holds a NaN or a +inf, or no finite entry.  Otherwise, with m = its largest finite entry,
+     S = sum over the finite entries of exp((double)x_i - m), in float64 in one fixed order;  lse = m + log(S) in float64;
+     logprob(i) = (float)((double)x_i - lse)                    (-inf for a -inf logit).
+   Outputs of a row (output row o, below):
+     lp[o]               logprob(tokens[r]) (tokens: device int64 [rows], e.g. the sampler's draws); NaN for a token outside
+                         [0, vocab) -- the sampler's -1 included -- for tokens == NULL, and for an undefined row;
+     top_ids[o][i], top_lp[o][i] for i < n_top (0 .. EXL_TOPLP_MAX; row stride top_ld >= n_top): the n_top finite entries with the
+                         largest logits in descending order, a tie to the lower id.  The order is on the logit itself (its bits under
+                         the sign flip, -0 read as +0: an exact total order), not on exp(x - m), so underflow never ties distinct
+                         logits.  Positions past the number of finite entries get id -1 and -inf; on an undefined row every id is -1
+                         and every log-probability NaN.  int64 ids, fp32 log-probabilities.
+   Routing: slot_host == NULL: output row o = r.  Otherwise slot_host and j_host are host arrays of rows entries, status a device
+   int32 [n_slots] (exl_gen_advance's): row r writes output row o = slot_host[r] * out_ld + j_host[r] only if slot_host[r] >= 0 and
+   status[slot_host[r]] == EXL_GEN_LIVE, else nothing -- exactly exl_gen_advance's gate, so a call between exl_sample_rows and
+   exl_gen_advance reports the stop token too.  lp is then [n_slots][out_ld], top_ids / top_lp [n_slots][out_ld][top_ld].
+   Host values are read during the call (baked into a CUDA-graph capture).  One launch, one cluster per row; no allocation, no
+   floating-point atomics: two calls are bitwise equal.
+   EXL_ERR_ARG (naming the value, and the row for a routing entry) for rows, vocab or n_top outside their bounds, logits_ld < vocab,
+   n_top > 0 with a NULL top_ids / top_lp or top_ld < n_top, a NULL logits or lp, slot_host without j_host or status, n_slots
+   outside 1 .. EXL_RAGGED_MAX_SEQ, a slot outside [-1, n_slots) or named twice, or a j outside [0, out_ld). */
+int exl_top_logprobs(const float* logits, int rows, int vocab, int64_t logits_ld, const int64_t* tokens, int n_top,
+                     const int* slot_host, const int* j_host, const int* status, int n_slots, int64_t out_ld,
+                     float* lp, int64_t* top_ids, float* top_lp, int64_t top_ld, void* stream);
+
 /* --- token log-probabilities (exllama_b200/csrc/logprob.cu; the reference: matmul + log_softmax + gather, perplexity.py:118-121) --- */
 
 /* Per row t of the final-normed hidden states hn fp16 [T][H] (row-major) against lm_head fp16 [V][H] (row-major) and targets int64
